@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- ALS user+item row-updates/sec at f=64 (BASELINE.json metric) on N B200s.
+"""bench.py -- ALS user+item row-updates/sec at f=64 (BASELINE.json metric) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2] [--scale S]
+                    [--dump-outputs DIR]
 
 A "step" is one ALS iteration of the hot path (user half + item half, each = Gramian + fused
 per-row Cholesky solve [+ factor all-gather at N > 1]) over the synthetic last.fm-shaped matrix C2
@@ -11,7 +12,9 @@ per-row Cholesky solve [+ factor all-gather at N > 1]) over the synthetic last.f
 3 iterations from pinned host CSR arrays (H2D), device transpose, and the factors read back (D2H).
 
 One process per GPU (torchrun-compatible env: RANK / LOCAL_RANK / WORLD_SIZE / MASTER_ADDR / MASTER_PORT);
-rank 0 prints exactly one JSON line.  --impl reference times the reference's own Cython/OpenMP CPU
+rank 0 prints exactly one JSON line.  --dump-outputs DIR writes what the timed path computed in its last step as
+DIR/<name>.npy (float32 / float64; a fixed, seeded row sample of the factor matrices), so that two builds can be
+compared output for output on identical inputs.  --impl reference times the reference's own Cython/OpenMP CPU
 path (oracle/_ref when it was built where /root/reference exists, else the C restatement) on a
 bounded row sample of the same workload, on rank 0 only.
 """
@@ -50,7 +53,34 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--trace-e2e", action="store_true", help="cProfile of the last end-to-end fit, to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (our implementation only)")
     return ap.parse_args()
+
+
+DUMP_ROWS = 32768  # per factor matrix: 2 x 32768 rows x f=128 (C3) x 4 bytes = 32 MB at most
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> numpy array, written as out_dir/<name>.npy in float32 (float64 for integer data: exact)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float32 if a.dtype.kind == "f" and a.itemsize <= 4 else np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+DUMP_BLOCK = 1024  # rows per downloaded block of the sample
+
+
+def sampled_factor_rows(name, F):
+    """A fixed, seeded sample of DUMP_ROWS rows of the device factor matrix F (all rows when it has fewer): seeded
+    blocks of DUMP_BLOCK consecutive rows, so that only the sample crosses to the host."""
+    if F.rows <= DUMP_ROWS:
+        return {name: F.download()}
+    starts = np.sort(np.random.default_rng(2024).choice(F.rows // DUMP_BLOCK, DUMP_ROWS // DUMP_BLOCK, replace=False)) * DUMP_BLOCK
+    rows = (starts[:, None] + np.arange(DUMP_BLOCK)[None, :]).ravel()
+    return {name: np.concatenate([F.download(int(r0), DUMP_BLOCK) for r0 in starts]), name + "_rows": rows}
 
 
 # --------------------------------------------------------------------------------------- helpers
@@ -62,28 +92,17 @@ def algorithmic_bytes_half(nnz, rows, n_other, f):
     return solve, gram
 
 
-def ncu_traffic(kernel, scale, world):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, averaged over the
-    two halves, from the committed ncu capture of this same workload (profiles/ncu_traffic.json, written by
-    tools/ncu_traffic.py).  None when no capture matches the run (other scale / sharded run)."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if scale != 1.0 or world != 1 or not os.path.exists(path):
-        return None
-    with open(path) as fh:
-        return json.load(fh).get(kernel, {}).get("bytes_per_launch")
-
-
 def measured_peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region (B200_PROFILING.md recipe): `nvidia-smi -lms 100`, plus -- the
+    """SM clock / throttle reasons DURING the timed region: `nvidia-smi -lms 100`, plus -- the
     timed region of a multi-GPU step is shorter than nvidia-smi's start-up and sampling period -- an in-process NVML
     poll every 10 ms (nvidia-ml-py; best effort: any failure leaves the nvidia-smi samples as the only source)."""
 
@@ -107,7 +126,7 @@ class ClockSampler:
             self.nvml = (pynvml, pynvml.nvmlDeviceGetHandleByIndex(int(self.index)))
             self.nvml_thread = threading.Thread(target=self._poll, daemon=True)
             self.nvml_thread.start()
-        except Exception:  # noqa: BLE001  (no NVML binding / no permission: nvidia-smi below is the recipe's source anyway)
+        except Exception:  # noqa: BLE001  (no NVML binding / no permission: nvidia-smi below is the other source)
             self.nvml = None
         try:
             self.proc = subprocess.Popen(
@@ -265,7 +284,7 @@ def run_reference(args):
 def workload_config(cfg, args, world):
     return {"workload": f"{args.config}: synthetic power-law CSR {cfg['users']}x{cfg['items']}, {cfg['nnz']} nnz, "
                         f"factors={cfg['factors']}, {'CG(3)' if cfg['use_cg'] else 'Cholesky'}, lambda=0.01, seed={cfg['seed']}",
-            "scale": args.scale, "l2": "inputs_exceed_l2 (CSR + factors > 126 MB)" if cfg["nnz"] * 8 > 126e6 else "l2_flush",
+            "scale": args.scale, "l2": "inputs_exceed_l2 (CSR + factors > 50 MB)" if cfg["nnz"] * 8 > 50e6 else "l2_flush",
             "parallelism": (f"row-sharded dp{world}, solved rows mirrored to peer replicas over NVLink by the solve kernel"
                             if world > 1 else "single GPU"),
             "e2e_step": f"fit(host CSR) x {E2E_ITERS} iterations + factors read back"}
@@ -338,7 +357,7 @@ def run_ours(args):
         half(Cui_s, X, Y, usplit)
         half(Ciu_s, Y, X, isplit)
 
-    flush = cfg["nnz"] * 8 <= 126e6  # small debug scales fit in L2: flush it between iterations
+    flush = cfg["nnz"] * 8 <= 50e6  # small debug scales fit in the 50 MB L2: flush it between iterations
     scaling = "weak" if on_device else "strong"  # C4 is the configuration sized for 8 GPUs; C2 / C3 are fixed problems
     for _ in range(max(args.warmup, 3)):
         iteration()
@@ -370,6 +389,8 @@ def run_ours(args):
     launches = ctx.launch_count() - launches0
     ms_max = pg.allreduce_max(ms) if world > 1 else ms
     value = (users + items) * args.steps / (ms_max * 1e-3)
+    if args.dump_outputs and args.steps > 0 and rank == 0:  # X and Y after the last timed iteration (full replicas on every rank)
+        dump_outputs(args.dump_outputs, {**sampled_factor_rows("user_factors", X), **sampled_factor_rows("item_factors", Y)})
 
     # ---- N > 1: the sharded result against a single-GPU run of the same iterations (rank 0 holds full replicas
     #      and the whole CSR): every row of both factor matrices, so the scaling line is a checked result
@@ -414,10 +435,10 @@ def run_ours(args):
     bytes_per_launch = (su + si + extra) / 2.0
     peak, peak_src = measured_peak_gbs()
     achieved = (bytes_per_launch * k_n) / (k_ms * 1e-3) / 1e9 if k_ms > 0 else None
-    roofline = {"bound": "hbm", "kernel": ("cholesky half: cholesky_half_kernel (rows > 48 nnz) + short_batch_kernel<4,{48..8}> + tcgen05 whitening + giant-row pass"
+    roofline = {"bound": "hbm", "kernel": ("cholesky half: cholesky_half_kernel (rows > 48 nnz) + short_batch_kernel<4,{48..8}> + wgmma whitening + giant-row pass"
                            if not use_cg else "cg_rows_kernel (+ giant-row passes)"), "achieved": achieved,
                 "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak if achieved else None,
-                "traffic": ncu_traffic(main_kernel, args.scale, world), "algorithmic_bytes_per_launch": bytes_per_launch,
+                "traffic": None, "algorithmic_bytes_per_launch": bytes_per_launch,
                 "avg_launch_ms": k_ms / k_n if k_n else None,
                 "kernel_share_of_step": k_ms / ms if ms else None,
                 "gramian_ms_per_launch": prof["gramian"][0] / max(prof["gramian"][1], 1)}
@@ -529,8 +550,8 @@ def run_ours(args):
 
 
 # --------------------------------------------------------------------------------------- C5: recommend
-# batch: two full waves of the top-k kernel's 256-query CTAs on 148 SMs (the 1M-user sweep is 13.2 such batches)
-C5 = dict(users=1_000_000, items=1_000_000, factors=64, k=10, liked_per_user=20, batch=2 * 148 * 256, seed=5)
+# batch: two full waves of the top-k kernel's 256-query CTAs on an H100's 132 SMs (the 1M-user sweep is 14.8 such batches)
+C5 = dict(users=1_000_000, items=1_000_000, factors=64, k=10, liked_per_user=20, batch=2 * 132 * 256, seed=5)
 
 
 def c5_inputs(scale):
@@ -623,13 +644,15 @@ def run_topk(args):
     t0 = time.perf_counter()
     for step in range(warm, warm + args.steps):
         lo, rows = batch_rows(step)
-        _lib.topk(ctx, di, dq, k, query_rows=rows, liked=liked_dev[lo])
+        ids, scores = _lib.topk(ctx, di, dq, k, query_rows=rows, liked=liked_dev[lo])
     ctx.sync()
     wall = time.perf_counter() - t0
     clocks = sampler.stop()
     prof = ctx.profile_read()
     ctx.profile(False)
     launches = ctx.launch_count() - launches0
+    if args.dump_outputs and args.steps > 0:  # the last timed batch: what recommend() hands back for those users
+        dump_outputs(args.dump_outputs, {"topk_ids": ids, "topk_scores": scores, "topk_query_rows": rows})
     k_ms, k_n = prof["topk"]
     ms = k_ms  # device time of the fused kernel(s): CUDA events around each launch on the library's stream
     value = batch * args.steps / (ms * 1e-3)
@@ -639,7 +662,7 @@ def run_topk(args):
             bf16 = float(json.load(fh)["bf16_tflops"])
         peak_src = "measured 16-bit tensor burst (MEASURED_PEAKS.json bf16_tflops) / 3: fp16 hi/lo operands, three MMAs per product"
     except Exception:
-        bf16, peak_src = 1590.0, "fallback 16-bit tensor 1.59 PFLOP/s / 3 (fp16 hi/lo operands, three MMAs per product)"
+        bf16, peak_src = 989.0, "fallback H100 SXM data sheet dense 16-bit tensor 989 TFLOP/s / 3 (fp16 hi/lo operands, three MMAs per product)"
     peak = bf16 / 3.0
     achieved = flops * k_n / (k_ms * 1e-3) / 1e12
     roofline = {"bound": "tensor", "kernel": "topk kernel (scores + filters + ordered select)", "achieved": achieved, "peak": peak,
@@ -690,7 +713,7 @@ def run_topk(args):
     print(json.dumps({
         "metric": "recommend() user-queries/sec at f=64, k=10", "value": value, "unit": "queries/s", "n_gpus": 1,
         "steps": args.steps, "warmup": warm, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": None, "dtype": "f32 (fp16 hi/lo split tensor-core scores: three tcgen05 MMAs per product, fp32-faithful)", "data": "synthetic",
+        "vs_baseline": None, "dtype": "f32 (fp16 hi/lo split tensor-core scores: three wgmma MMAs per product, fp32-faithful)", "data": "synthetic",
         "config": c5_config(Q, I, batch, args), "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
         "roofline": roofline, "cpu_baseline": cpu, "wall_s_timed_region": wall}))
 
@@ -746,7 +769,7 @@ def run_reference_gpu(args):
         "steps": int(len(timed)), "warmup": args.warmup, "ms_per_step": float(timed.mean()), "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": dict(workload_config(dict(cfg, use_cg=True), args, 1),
-                       note="the reference's GPU path is CG-only: implicit/gpu/als.cu least_squares_cg_kernel + cublasSgemm Gramian, compiled for sm_100a"),
+                       note="the reference's GPU path is CG-only: implicit/gpu/als.cu least_squares_cg_kernel + cublasSgemm Gramian, compiled for sm_90a"),
         "ms_per_iteration": [round(float(x), 3) for x in ms],
         "ours_cg_same_workload": {"ms_per_step": ours_ms, "value": (users + items) / (ours_ms * 1e-3),
                                   "speedup_over_reference_gpu": float(timed.mean()) / ours_ms,

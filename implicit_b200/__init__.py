@@ -1,4 +1,4 @@
-"""implicit_b200: a B200-native (sm_100a) ALS fit / recommend hot path behind benfred/implicit's API.
+"""implicit_b200: an H100-native (sm_90a) ALS fit / recommend hot path behind benfred/implicit's API.
 
     from implicit_b200 import AlternatingLeastSquares
     model = AlternatingLeastSquares(factors=64, use_cg=False)

@@ -1,7 +1,7 @@
 """ctypes binding of libals_b200.so (include/als_b200.h) -- the only way Python reaches the GPU here.
 
 There is deliberately no fallback: if the shared library is missing it is built with nvcc; if that
-fails, or there is no B200 to run on, the caller gets an exception.
+fails, or there is no H100 to run on, the caller gets an exception.
 """
 import ctypes
 import os

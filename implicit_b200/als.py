@@ -1,10 +1,10 @@
-"""Implicit Alternating Least Squares on B200 -- the host-side mirror of the reference model classes.
+"""Implicit Alternating Least Squares on H100 -- the host-side mirror of the reference model classes.
 
 Same surface as ``implicit.als.AlternatingLeastSquares`` (factory, implicit/als.py:7-80) /
 ``implicit.cpu.als.AlternatingLeastSquares`` (implicit/cpu/als.py:20-477) for the ALS hot path:
 ``fit``, ``recommend``, ``recalculate_user`` / ``recalculate_item``, ``partial_fit_users`` /
 ``partial_fit_items``, ``similar_items`` / ``similar_users``, ``save`` / ``load`` and the attributes the
-reference exposes.  All arithmetic runs in libals_b200.so (hand-written sm_100a CUDA) through ctypes;
+reference exposes.  All arithmetic runs in libals_b200.so (hand-written sm_90a CUDA) through ctypes;
 this file only orders the calls the way the reference does and keeps its error behaviour.
 """
 import logging
@@ -21,7 +21,7 @@ log = logging.getLogger("implicit")
 
 
 class AlternatingLeastSquares:
-    """Alternating Least Squares (Hu, Koren & Volinsky 2008; CG variant Takacs et al. 2011) on one or more B200s.
+    """Alternating Least Squares (Hu, Koren & Volinsky 2008; CG variant Takacs et al. 2011) on one or more H100s.
 
     Parameters mirror implicit/als.py:7-19.  ``use_gpu`` must stay True and ``dtype`` float32: this
     package has no CPU path and computes in fp32.  New: ``device`` (CUDA ordinal) and
@@ -182,7 +182,7 @@ class AlternatingLeastSquares:
         self._p2p = False
         if pg is not None and pg.world > 1:
             # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
-            # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros (profiles/r01_cholesky_ablation*.txt)
+            # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
             row_cost = 20 if self.use_cg else 60
             usplit = nnz_balanced_splits(Cui_host.indptr, pg.world, row_cost)
             isplit = nnz_balanced_splits(Ciu.indptr_host(), pg.world, row_cost)

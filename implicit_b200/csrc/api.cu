@@ -291,8 +291,8 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   ALS_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   ALS_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("als_ctx_create: device %d is sm_%d%d; libals_b200 is built for sm_100a only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("als_ctx_create: device %d is sm_%d%d; libals_b200 is built for sm_90a only", device, prop.major,
               prop.minor);
     return ALS_E_UNSUPPORTED;
   }
@@ -906,7 +906,7 @@ ALS_API int als_least_squares(als_ctx *ctx, const als_csr *C, als_factors *X, co
   return finish_cholesky(ctx, C, X, Y, regularization, bad_row);
 }
 
-// W = Y (2^14 P) / 2^14 and Z = Y G^-1 of the short-row path, downloaded (tests and tools: the tcgen05 apply of
+// W = Y (2^14 P) / 2^14 and Z = Y G^-1 of the short-row path, downloaded (tests and tools: the wgmma apply of
 // dense.cu against an fp64 product).  Leaves the Gramian of Y in the context like als_gramian.
 ALS_API int als_whitened_factors(als_ctx *ctx, const als_factors *Y, double regularization, float *W_host, float *Z_host) {
   ALS_REQUIRE(ctx && Y && W_host && Z_host, "als_whitened_factors: NULL argument");

@@ -389,8 +389,7 @@ int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors 
     set_error("cg: X and Y strides differ (%d vs %d)", X->ld, Y->ld);
     return ALS_E_INVALID;
   }
-  // float4 words per lane (knob cg_nv): measured on B200: C2 (f=64) 6.0 ms/iter at 2 vs 6.6 (1) and 9.3 (4);
-  // C3 (f=128) 9.9 vs 11.2 and 11.9
+  // float4 words per lane: knob cg_nv
   if (Y->ld > 128) {
     // wide models (the reference's CUDA path takes up to 1024 factors, implicit/gpu/als.cu:177-178): the padded width is
     // a multiple of 128, a whole warp per nonzero with ld / 128 float4 words per lane

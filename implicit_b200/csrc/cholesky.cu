@@ -310,8 +310,8 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
   int64_t n_main = Cm->n_work;
   if (short_max > 0) {
     const int64_t begin = Cm->le_begin[(48 - short_max) / 8];  // kShortThresholds: 48, 40, ..., 8
-    // worth it when the short rows outweigh whitening all of Y: W = Y P costs ~0.24 ns per row of Y, a short row
-    // saves ~4 ns (profiles/r01_short_rows_ab_v4.txt, r01_launches_summary_v2.txt) -> break-even near 1 : 17
+    // worth it when the short rows outweigh whitening all of Y: one short row saves roughly what whitening 16 rows
+    // of Y costs
     if ((Cm->n_work - begin) * 16 >= Y->rows) n_main = begin;
     else short_max = 0;
   }
@@ -332,7 +332,7 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
       if (rc != ALS_OK) return rc;
     }
     if (n_main && NB == 4 && cholesky_tc_eligible(ctx, Cm, Y->ld)) {
-      // whole rows: normal equations on the tcgen05 tensor cores; chunks of giant rows: the mma.sync kernel
+      // whole rows: normal equations on the wgmma tensor cores; chunks of giant rows: the mma.sync kernel
       int rc = launch_cholesky_tc(ctx, Cm, X, Y, n_main, ctx->stream);
       if (rc != ALS_OK) return rc;
       if (Cm->n_slots) {

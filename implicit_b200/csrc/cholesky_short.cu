@@ -709,7 +709,7 @@ int short_rows_prepare(als_ctx *ctx, const als_factors *Y, cudaStream_t stream) 
   whiten_factor_kernel<<<1, 1024, smem, stream>>>(ctx->Greg, F, ctx->Pinv, ctx->Ginv, ctx->counters + kCtrWhitenOk);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
-  // 64 padded factors: one pass on the tcgen05 tensor cores (dense.cu); the whiten_fma knob keeps the fp32 FMA tiles
+  // 64 padded factors: one pass on the wgmma tensor cores (dense.cu); the whiten_fma knob keeps the fp32 FMA tiles
   if (F == 64 && Y->rows >= 128 && !ctx->knobs.whiten_fma) return launch_dense_whiten(ctx, Y, stream);  // (a TMA box is 128 rows)
   switch (F / 16) {
     case 2: return run_whiten_rows<2>(ctx, Y, stream);

@@ -1,51 +1,50 @@
-// R1, rows of more than 48 nonzeros at 64 padded factors: the normal equations on the tcgen05 tensor cores
+// R1, rows of more than 48 nonzeros at 64 padded factors: the normal equations on the Hopper tensor cores (wgmma)
 // (reference: _least_squares, implicit/cpu/_als.pyx:76-142; the mma.sync kernel of cholesky.cu stays as the path for
-// chunks of giant rows, finish items, CSRs with weights below 1 and the other factor widths).
+// chunks of giant rows, finish items, CSRs with weights below 1 and the other factor widths).  Opt-in: knob long_tc.
 //
 //   A_u = (Y^T Y + lambda I) + sum_k w_k y_k y_k^T  with  w_k = |c_k| - 1 >= 0   is   G + Z^T Z,  Z = [sqrt(w_k) y_k]:
 //   a GEMM whose operand rows are exactly what the gather produces.  One persistent CTA per SM, warp specialised:
 //
-//   producers (7 warps)  take 32 nonzeros of the current row per ring stage: 16-byte cp.async copies of the gathered
-//                        factor rows into a private landing zone (two halves of 16 rows: the next stage's gathers are
-//                        in flight while this one is converted; its indices are fetched a stage ahead), scale by
-//                        sigma sqrt(w), split into fp16 hi + lo (both rounded to nearest) and
-//                        store the two 32 x 64 tiles MN-major with the 128-byte swizzle -- a nonzero is one 128-byte
-//                        row of the tile.  b_u = sum c_k y_k rides along in fp32 (one partial per producer, summed in
-//                        a fixed order);
-//   MMA warp (one lane)  per 16 nonzeros two tcgen05.mma.kind::f16 (M = 64, K = 16):  hi^T [hi | lo]  (N = 128) and
-//                        lo^T hi (N = 64, onto the second half) into one of four 128-column fp32 accumulators in TMEM;
-//                        tcgen05.commit frees the stage / hands the row over.  The large term hi^T hi has its own
-//                        64 columns: the accumulator is TRUNCATED on every MMA (measured: profiles/
-//                        r02_long_rows_tcgen05_v1_ab.txt), and adding the small terms into the same columns tripled
-//                        the number of truncations of the large sums;
-//   solvers (8 warps)    two groups of four: the four warps of a group drain four finished accumulators (a warp can read
-//                        only its own quarter of the TMEM lanes; large + small halves are added here) into the packed
-//                        panel layout of the blocked Cholesky,
-//                        then every warp adds sigma^2 (Y^T Y + lambda I), factors and solves one row in registers
-//                        (factor_solve of cholesky_device.cuh, shared with the mma.sync kernel) and stores x, also to
-//                        the peer replicas.
+//   producers (warpgroup 3)  take 32 nonzeros of the current row per ring stage: 16-byte cp.async copies of the
+//                        gathered factor rows into a private landing zone (two halves of 16 rows: the next stage's
+//                        gathers are in flight while this one is converted; its indices are fetched a stage ahead),
+//                        scale by sigma sqrt(w), split into fp16 hi + lo (both rounded to nearest) and store the two
+//                        32 x 64 tiles MN-major with the 128-byte swizzle -- a nonzero is one 128-byte row of the tile.
+//                        b_u = sum c_k y_k rides along in fp32 (one partial per producer, summed in a fixed order);
+//   MMA (warpgroup 2)    per 16 nonzeros two wgmma.m64nNk16.f16 with both operands MN-major:  hi^T [hi | lo]
+//                        (N = 128) and lo^T hi (N = 64, onto the second half) into 64 fp32 registers per thread.  The
+//                        large term hi^T hi has its own 64 columns, so the small terms never round into the large
+//                        sums.  At the end of a row the warpgroup adds the halves and writes the matrix, with b_u, into
+//                        the packed panel layout of the blocked Cholesky of one solver warp;
+//   solvers (warpgroups 0, 1)  two groups of four warps, four rows per group and batch: every warp adds
+//                        sigma^2 (Y^T Y + lambda I), factors and solves one row in registers (factor_solve of
+//                        cholesky_device.cuh, shared with the mma.sync kernel) and stores x, also to the peer replicas.
 // Rows are dealt to the CTAs round robin from the length-sorted work list, so all roles of a CTA walk the same
-// sequence without talking to each other; the only synchronisation is four sets of mbarriers (stage full / free,
-// accumulator done / free).  Deterministic: nothing depends on scheduling.  Registers are rebalanced with setmaxnreg:
-// the solvers' warpgroups take 168 each, the producer / MMA warpgroups give back down to 80 (2 K registers of slack in the exchange).
+// sequence without talking to each other; the only synchronisation is mbarriers (stage full / free, b partials ready /
+// consumed, solver panels full / free).  Deterministic: nothing depends on scheduling.  Registers are rebalanced with
+// setmaxnreg: the solvers' warpgroups take 168 each, the MMA warpgroup 96 and the producers 80.
 #include "cholesky_device.cuh"
+#include "sm90.cuh"
 
 namespace als {
 
 namespace {
+
+using namespace sm90;
 
 constexpr int kTcF = 64;
 constexpr int kTcStageNnz = 32;                     // nonzeros per ring stage
 constexpr int kTcTile = kTcStageNnz * 128;          // one fp16 tile: 32 rows of 64 halves
 constexpr int kTcStageBytes = 2 * kTcTile;          // hi | lo
 constexpr int kTcStages = 8;
-constexpr int kTcSlots = 4;                         // TMEM accumulators of 128 columns: hi^T hi | hi^T lo + lo^T hi
-constexpr int kTcSlotCols = 128;
-constexpr int kTcProducers = 7;
+constexpr int kTcSlots = 4;                         // b partials in flight (rows)
 constexpr int kTcSolvers = 8;
-constexpr int kTcMmaWarp = kTcSolvers;
-constexpr int kTcThreads = 32 * (kTcSolvers + 1 + kTcProducers);
+constexpr int kTcMmaWarp0 = kTcSolvers;             // warpgroup 2
+constexpr int kTcProducerWarp0 = kTcSolvers + 4;    // warpgroup 3
+constexpr int kTcProducers = 4;
+constexpr int kTcThreads = 32 * (kTcSolvers + 4 + kTcProducers);
 static_assert(kTcThreads == 512, "four warpgroups: setmaxnreg below assumes 128 registers per thread at launch");
+static_assert(2 * 128 * 168 + 128 * 96 + 128 * 80 <= 65536, "setmaxnreg budget");
 constexpr int kTcSolverFloats = Cfg<4>::U_FLOATS + kTcF;  // packed panels + rhs
 constexpr int kTcOffRing = 0;
 constexpr int kTcOffSolver = kTcStages * kTcStageBytes;
@@ -53,98 +52,11 @@ constexpr int kTcRawBytes = 2 * 16 * 256;           // per producer: two halves 
 constexpr int kTcOffRaw = kTcOffSolver + kTcSolvers * kTcSolverFloats * 4;
 constexpr int kTcOffBpart = kTcOffRaw + kTcProducers * kTcRawBytes;
 constexpr int kTcOffBar = kTcOffBpart + kTcSlots * kTcProducers * kTcF * 4;
-// "row done" has 2 kTcSlots barriers (row n uses n % 8): a solver group then sees consecutive phases of its own four
-// barriers.  With one barrier per accumulator the two groups would alternate on its phases, and a parity wait cannot
-// tell "two phases behind" from "done" (first attempt: deadlock, profiles/r02_long_rows_tcgen05_hang.txt).
 constexpr int kTcDone = 2 * kTcSlots;
 enum { kTcFull = 0, kTcEmpty = kTcStages, kTcRowDone = 2 * kTcStages, kTcSlotFree = 2 * kTcStages + kTcDone,
-       kTcNumBars = 2 * kTcStages + kTcDone + kTcSlots };
+       kTcPanelFull = kTcSlotFree + kTcSlots, kTcPanelFree = kTcPanelFull + 2, kTcNumBars = kTcPanelFree + 2 };
 constexpr int kTcSmem = kTcOffBar + 8 * kTcNumBars + 16 + 1024;
 static_assert(kTcSmem <= 227 * 1024, "shared memory budget");
-
-__device__ __forceinline__ uint32_t tc_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void tc_mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void tc_mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(bar), "r"(parity)
-      : "memory");
-}
-// MN-major fp16 operand tile, 128B swizzle: a row of the tile is one nonzero (K index) holding the 64 halves of the M / N
-// extent; groups of 8 nonzeros are 1024 bytes apart (SBO).  Descriptor version 1, layout type 2 = SWIZZLE_128B.
-#ifndef ALS_TC_LBO
-#define ALS_TC_LBO 256  // 4096 bytes between the 64-element atoms along N: the hi tile, then the lo tile (N = 128 only)
-#define ALS_TC_SBO 64   // 1024 bytes between groups of 8 nonzeros
-#endif
-__device__ __forceinline__ uint64_t tc_desc_mn_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3fffu) | ((uint64_t)ALS_TC_LBO << 16) | ((uint64_t)ALS_TC_SBO << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16: fp16 operands (format 0), fp32 accumulate, A and B MN-major (bits 15, 16), M = 64, N = 64 / 128
-constexpr uint32_t kTcIdesc64 = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
-constexpr uint32_t kTcIdesc128 = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-}
-// Where the roles wait (cycles per warp), only in -DALS_TC_STATS builds (tools/long_stats.py)
-#ifdef ALS_TC_STATS
-__device__ unsigned long long g_tc_stats[160 * 16 * 4];
-__device__ volatile int *g_tc_dbg = nullptr;  // host-mapped: [8 CTAs][16 warps][4] = {what the warp waits on, row, stage, done flag}
-#define TC_TIMED(i, stmt)                \
-  do {                                   \
-    const long long t0__ = clock64();    \
-    stmt;                                \
-    wt[i] += clock64() - t0__;           \
-  } while (0)
-#define TC_MARK(code, a, b)                                                       \
-  do {                                                                            \
-    if (g_tc_dbg && blockIdx.x < 8 && (threadIdx.x & 31) == 0) {                  \
-      volatile int *d__ = g_tc_dbg + ((int)blockIdx.x * 16 + (threadIdx.x >> 5)) * 4; \
-      d__[0] = (code);                                                            \
-      d__[1] = (a);                                                               \
-      d__[2] = (b);                                                               \
-    }                                                                             \
-  } while (0)
-#else
-#define TC_TIMED(i, stmt) stmt
-#define TC_MARK(code, a, b)
-#endif
-__device__ __forceinline__ void tc_group_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 __global__ void __launch_bounds__(kTcThreads, 1)
 cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict__ data, const float *__restrict__ Y,
@@ -154,14 +66,15 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
   using C = Cfg<4>;
   constexpr int F = kTcF;
   extern __shared__ unsigned char tc_smem_raw[];
-  const uint32_t raw = tc_smem_u32(tc_smem_raw);
+  const uint32_t raw = smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   unsigned char *gbase = tc_smem_raw + (base - raw);
   const uint32_t bars = base + kTcOffBar;
   auto bar = [&](int i) -> uint32_t { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(gbase + kTcOffBar + 8 * kTcNumBars);
   float *bpart = reinterpret_cast<float *>(gbase + kTcOffBpart);
+  float *panels = reinterpret_cast<float *>(gbase + kTcOffSolver);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 7, 0);  // warpgroup, visibly uniform to the compiler
   // this CTA's rows: work[blockIdx.x + n gridDim.x], n = 0 .. n_mine - 1
   const int n_mine = ((int)blockIdx.x < n_work) ? (n_work - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto load_item = [&](int n) -> WorkItem {
@@ -170,38 +83,26 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
   };
   const float sigma = pow2_scale_below_2_14(sqrtf(__uint_as_float(*wmax_bits)) * __uint_as_float(*yabsmax_bits));
   const float sigma2 = sigma * sigma;
-#ifdef ALS_TC_STATS
-  long long wt[4] = {0, 0, 0, 0};
-  const long long t_start = clock64();
-#endif
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kTcStages; ++i) {
-      tc_mbar_init(bar(kTcFull + i), 1);
-      tc_mbar_init(bar(kTcEmpty + i), 1);
+      mbar_init(bar(kTcFull + i), 1);
+      mbar_init(bar(kTcEmpty + i), 1);
     }
-    for (int i = 0; i < kTcDone; ++i) tc_mbar_init(bar(kTcRowDone + i), 1 + kTcProducers);
-    for (int i = 0; i < kTcSlots; ++i) tc_mbar_init(bar(kTcSlotFree + i), 4);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int i = 0; i < kTcDone; ++i) mbar_init(bar(kTcRowDone + i), kTcProducers);
+    for (int i = 0; i < kTcSlots; ++i) mbar_init(bar(kTcSlotFree + i), 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(bar(kTcPanelFull + i), 4);   // one arrival per row of a batch (MMA warpgroup)
+      mbar_init(bar(kTcPanelFree + i), 4);   // one arrival per solver warp of the group
+    }
+    mbar_init_fence();
   }
-  if (warp == kTcMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32((const void *)tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  TC_MARK(1, 0, 0);
-  if (warp >= kTcSolvers) {
+  if (wg == kTcProducerWarp0 / 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-    TC_MARK(2, 0, 0);  // both warpgroups of the producer / MMA side
-    if (warp > kTcMmaWarp) {
       // ===== producers ==========================================================================================
-      const int pw = warp - kTcMmaWarp - 1;
+      const int pw = warp - kTcProducerWarp0;
       const int hl = lane >> 4, cl = lane & 15;  // the row of a pair, the 16-byte word of the factor row
       unsigned char *rawb = gbase + kTcOffRaw + pw * kTcRawBytes;
       // This warp's stages are the CTA's stages G = pw, pw + P, pw + 2 P, ...  A cursor names one of them: the row n
@@ -249,11 +150,10 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
         bs.y += __shfl_xor_sync(0xffffffffu, bs.y, 16);
         bs.z += __shfl_xor_sync(0xffffffffu, bs.z, 16);
         bs.w += __shfl_xor_sync(0xffffffffu, bs.w, 16);
-        TC_MARK(12, n, 0);
-        if (n >= kTcSlots) TC_TIMED(1, tc_mbar_wait(bar(kTcSlotFree + slot), (uint32_t)((n / kTcSlots - 1) & 1)));
+        if (n >= kTcSlots) mbar_wait(bar(kTcSlotFree + slot), (uint32_t)((n / kTcSlots - 1) & 1));
         if (lane < 16) *reinterpret_cast<float4 *>(bpart + (slot * kTcProducers + pw) * F + 4 * cl) = bs;
         __syncwarp();
-        if (lane == 0) tc_mbar_arrive(bar(kTcRowDone + n % kTcDone));
+        if (lane == 0) mbar_arrive(bar(kTcRowDone + n % kTcDone));
       };
       const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
 
@@ -291,18 +191,16 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
         const int nnv = (nxt.n < n_mine) ? min(kTcStageNnz, nxt.wi.k1 - (nxt.wi.k0 + kTcStageNnz * nxt.s)) : 0;
 
         const int rs = cur.G % kTcStages, use = cur.G / kTcStages;
-        const int nvalid = min(kTcStageNnz, cur.wi.k1 - (cur.wi.k0 + kTcStageNnz * cur.s));
         // A += w y y^T with w = |c| - 1 (>= 0 here: CSRs with smaller weights take the mma.sync kernel);
         // b += c y for c > 0   (_als.pyx:115-124)
         const float sw = (idx >= 0) ? sigma * __fsqrt_rn(fmaxf(fabsf(cf) - 1.f, 0.f)) : 0.f;
         const float cp = (idx >= 0 && cf > 0.f) ? cf : 0.f;
         unsigned char *hi = gbase + kTcOffRing + rs * kTcStageBytes, *lo = hi + kTcTile;
-        TC_MARK(11, cur.n, cur.G);
-        if (use > 0) TC_TIMED(0, tc_mbar_wait(bar(kTcEmpty + rs), (uint32_t)((use - 1) & 1)));  // the MMAs of the previous use are done
+        if (use > 0) mbar_wait(bar(kTcEmpty + rs), (uint32_t)((use - 1) & 1));  // the MMAs of the previous use are done
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           cp_async_wait<1>();  // this half has landed (every lane reads back only what it copied itself)
-          if (h == 0 || nvalid > 16) {  // the MMA warp skips an empty second half as well
+          {  // an empty second half is written as zeros (invalid nonzeros read as zero): the MMAs always take 32 rows
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const int r = 16 * h + 2 * j + hl;
@@ -324,9 +222,9 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
           }
           issue_half(nidx, h, nxt.n < n_mine && (h == 0 || nnv > 16));  // the landing zone of this half is free again
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> the tensor core's reads
+        fence_proxy_async();  // generic-proxy stores -> the tensor core's reads
         __syncwarp();
-        if (lane == 0) tc_mbar_arrive(bar(kTcFull + rs));
+        if (lane == 0) mbar_arrive(bar(kTcFull + rs));
         // rows that end between this stage and the next one of this warp
         if (nxt.n != cur.n) {
           finish_row(done_rows++, bs);
@@ -338,100 +236,74 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
         cf = ncf;
       }
       cp_async_wait<0>();
-    } else {
-      // ===== MMA issue ==========================================================================================
-      if (lane == 0) {
-        int G = 0;
-        for (int n = 0; n < n_mine; ++n) {
-          const WorkItem wi = load_item(n);
-          const int nnz = (wi.slot == -1) ? wi.k1 - wi.k0 : 0;
-          const int nst = (nnz + kTcStageNnz - 1) / kTcStageNnz;
-          const int slot = n % kTcSlots;
-          TC_MARK(21, n, G);
-          if (n >= kTcSlots) TC_TIMED(1, tc_mbar_wait(bar(kTcSlotFree + slot), (uint32_t)((n / kTcSlots - 1) & 1)));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d = tmem_base + (uint32_t)(slot * kTcSlotCols);
-          uint32_t acc = 0;
-          for (int s = 0; s < nst; ++s, ++G) {
-            const int rs = G % kTcStages;
-            TC_MARK(22, n, G);
-            TC_TIMED(0, tc_mbar_wait(bar(kTcFull + rs), (uint32_t)((G / kTcStages) & 1)));
-            TC_MARK(23, n, G);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t hi = base + kTcOffRing + rs * kTcStageBytes, lo = hi + kTcTile;
-            const int nk = (nnz - kTcStageNnz * s > 16) ? 2 : 1;
-            for (int ks = 0; ks < nk; ++ks) {
-              const uint64_t dh = tc_desc_mn_sw128(hi + ks * 2048), dl = tc_desc_mn_sw128(lo + ks * 2048);
-              tc_mma(d, dh, dh, kTcIdesc128, acc);     // [hi^T hi | hi^T lo]: B spans the hi tile and, one LBO on, the lo tile
-              tc_mma(d + 64, dl, dh, kTcIdesc64, 1);   // + lo^T hi
-              acc = 1;
-            }
-            tc_commit(bar(kTcEmpty + rs));
-          }
-          tc_commit(bar(kTcRowDone + n % kTcDone));
+  } else if (wg == kTcMmaWarp0 / 4) {
+    // ===== MMA warpgroup: accumulate a row in registers, drain it into a solver panel ===========================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 96;");
+    const int t = threadIdx.x - 32 * kTcMmaWarp0;  // 0 .. 127
+    int G = 0;
+    const int n_batched = (n_mine + 3) & ~3;      // whole batches of four rows: the solver groups count four arrivals
+    for (int n = 0; n < n_batched; ++n) {
+      const int B = n >> 2, e = B & 1, j = n & 3;
+      if (j == 0 && B >= 2) mbar_wait(bar(kTcPanelFree + e), (uint32_t)(((B >> 1) - 1) & 1));  // batch B - 2 is solved
+      if (n < n_mine) {
+        const WorkItem wi = load_item(n);
+        const int nnz = (wi.slot == -1) ? wi.k1 - wi.k0 : 0;
+        const int nst = (nnz + kTcStageNnz - 1) / kTcStageNnz;
+        const int slot = n % kTcSlots;
+        float d[64];
+        float(&d_small)[32] = *reinterpret_cast<float(*)[32]>(&d[32]);  // columns 64..127 of the accumulator
+#pragma unroll
+        for (int v = 0; v < 64; ++v) d[v] = 0.f;
+        for (int s = 0; s < nst; ++s, ++G) {
+          const int rs = G % kTcStages;
+          mbar_wait(bar(kTcFull + rs), (uint32_t)((G / kTcStages) & 1));
+          const uint32_t hi = base + kTcOffRing + rs * kTcStageBytes, lo = hi + kTcTile;
+          wgmma_fence();
+          // [hi^T hi | hi^T lo]: B spans the hi tile and, one LBO (kTcTile bytes) on, the lo tile; then + lo^T hi
+          wgmma_f16_mn_m64n128k16(d, wgmma_desc_mn_sw128(hi, kTcTile), wgmma_desc_mn_sw128(hi, kTcTile), s > 0);
+          wgmma_f16_mn_m64n64k16(d_small, wgmma_desc_mn_sw128(lo, kTcTile), wgmma_desc_mn_sw128(hi, kTcTile), 1);
+          // second 16 nonzeros (zero rows where the stage holds fewer)
+          wgmma_f16_mn_m64n128k16(d, wgmma_desc_mn_sw128(hi + 2048, kTcTile), wgmma_desc_mn_sw128(hi + 2048, kTcTile), 1);
+          wgmma_f16_mn_m64n64k16(d_small, wgmma_desc_mn_sw128(lo + 2048, kTcTile), wgmma_desc_mn_sw128(hi + 2048, kTcTile), 1);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand(d);
+          if (t == 0) mbar_arrive(bar(kTcEmpty + rs));  // the stage may be refilled
         }
+        mbar_wait(bar(kTcRowDone + n % kTcDone), (uint32_t)((n / kTcDone) & 1));  // every producer's b partial is in
+        if (wi.slot == -1 && wi.k1 > wi.k0) {
+          float *Uj = panels + (4 * e + j) * kTcSolverFloats;
+#pragma unroll
+          for (int v = 0; v < 32; v += 2) {
+            // accumulator row m -> panel m / 8, columns >= 8 (m / 8): large term + small terms
+            const int m = wgmma_row(t, v), col = wgmma_col(t, v);
+            const int pm = m >> 3;
+            const int po = 8 * (pm * F - 4 * pm * (pm - 1) + 8 * ((pm + 1) >> 1));
+            const int ps = F - 8 * pm + ((pm & 1) ? 0 : 8);
+            if (col >= 8 * pm)
+              *reinterpret_cast<float2 *>(Uj + po + (m & 7) * ps - 8 * pm + col) = make_float2(d[v] + d[v + 32], d[v + 1] + d[v + 33]);
+          }
+          if (t < F) {  // b_u: the producers' partials in a fixed order
+            float b = 0.f;
+#pragma unroll
+            for (int p = 0; p < kTcProducers; ++p) b += bpart[(slot * kTcProducers + p) * F + t];
+            Uj[C::U_FLOATS + t] = b;
+          }
+        }
+        named_sync(3, 128);  // the panel is written and the b partials are read
+        if (t == 0) mbar_arrive(bar(kTcSlotFree + slot));
       }
+      if (t == 0) mbar_arrive(bar(kTcPanelFull + e));
     }
   } else {
-    // ===== drain + solve ======================================================================================
+    // ===== solvers ============================================================================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 168;");
-    TC_MARK(3, 0, 0);
     const int e = warp >> 2, q = warp & 3;
     const int g = lane >> 2, t = lane & 3;
-    float *Uown = reinterpret_cast<float *>(gbase + kTcOffSolver) + warp * kTcSolverFloats;
+    float *Uown = panels + warp * kTcSolverFloats;
     float *zown = Uown + C::U_FLOATS;
     for (int B = e; 4 * B < n_mine; B += 2) {
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        const int n = 4 * B + j;
-        if (n >= n_mine) break;
-        const int slot = n % kTcSlots;
-        const WorkItem wi = load_item(n);
-        const bool real = wi.slot == -1 && wi.k1 > wi.k0;
-        TC_MARK(32, n, j);
-        TC_TIMED(0, tc_mbar_wait(bar(kTcRowDone + n % kTcDone), (uint32_t)((n / kTcDone) & 1)));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (real) {
-          float *Uj = reinterpret_cast<float *>(gbase + kTcOffSolver) + (4 * e + j) * kTcSolverFloats;
-          // accumulator row m = 16 q + lane (lanes 0..15 of this warp's TMEM quarter) -> panel m / 8, columns >= 8 (m / 8)
-          const int pm = 2 * q + ((lane >> 3) & 1);
-          const int po = 8 * (pm * F - 4 * pm * (pm - 1) + 8 * ((pm + 1) >> 1));
-          const int ps = F - 8 * pm + ((pm & 1) ? 0 : 8);
-          float *dst = Uj + po + (lane & 7) * ps - 8 * pm;
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            float v[32], w[32];
-            tc_tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(slot * kTcSlotCols + 32 * half), v);
-            tc_tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(slot * kTcSlotCols + 64 + 32 * half), w);
-#pragma unroll
-            for (int c = 0; c < 32; ++c) v[c] += w[c];  // large term + small terms
-            if (lane < 16) {
-#pragma unroll
-              for (int c4 = 0; c4 < 8; ++c4) {
-                const int col = 32 * half + 4 * c4;
-                if (col >= 8 * pm)
-                  *reinterpret_cast<float4 *>(dst + col) = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-              }
-            }
-          }
-          if (q == 0) {  // b_u: the producers' partials in a fixed order
-            float2 b = make_float2(0.f, 0.f);
-#pragma unroll
-            for (int p = 0; p < kTcProducers; ++p) {
-              const float2 x = *reinterpret_cast<const float2 *>(bpart + (slot * kTcProducers + p) * F + 2 * lane);
-              b.x += x.x;
-              b.y += x.y;
-            }
-            *reinterpret_cast<float2 *>(Uj + C::U_FLOATS + 2 * lane) = b;
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) tc_mbar_arrive(bar(kTcSlotFree + slot));
-      }
-      TC_MARK(33, B, 0);
-      TC_TIMED(1, tc_group_sync(1 + e));  // the group's four matrices are complete in shared memory
-      TC_MARK(34, B, 0);
+      mbar_wait(bar(kTcPanelFull + e), (uint32_t)((B >> 1) & 1));  // the group's four matrices are in shared memory
       const int n = 4 * B + q;
       if (n < n_mine) {
         const WorkItem wi = load_item(n);
@@ -468,49 +340,19 @@ cholesky_tc_kernel(const int32_t *__restrict__ indices, const float *__restrict_
           __syncwarp();
           bool ok = true;
           float xx[(F + 31) / 32];
-          TC_TIMED(2, factor_solve<4>(st, Uown, zown, lane, ok, 0, xx));
+          factor_solve<4>(st, Uown, zown, lane, ok, 0, xx);
           if (ok) store_solution<F>(xx, X + xoff, lane, peers, n_peers, xoff);
           if (!ok && lane == 0) atomicMin(bad_row, (long long)(row_offset + wi.row));
           __syncwarp();
         }
       }
-      TC_MARK(35, B, 0);
-      TC_TIMED(1, tc_group_sync(1 + e));  // the panel buffers are free for the next drain
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar(kTcPanelFree + e));  // this warp's panel buffer is free for batch B + 2
     }
-  }
-  TC_MARK(99, 0, 0);
-#ifdef ALS_TC_STATS
-  if (lane == 0 && blockIdx.x < 160) {
-    wt[3] = clock64() - t_start;
-    for (int i = 0; i < 4; ++i) g_tc_stats[((int)blockIdx.x * 16 + warp) * 4 + i] = (unsigned long long)wt[i];
-  }
-#endif
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == kTcMmaWarp) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
 }  // namespace
-
-#ifdef ALS_TC_STATS
-extern "C" __attribute__((visibility("default"))) int als_debug_tc_stats(unsigned long long *out) {
-  return (int)cudaMemcpyFromSymbol(out, g_tc_stats, sizeof(unsigned long long) * 160 * 16 * 4);
-}
-// progress markers in host-mapped memory: readable from the host while a kernel hangs
-extern "C" __attribute__((visibility("default"))) int als_debug_tc_hostbuf(int **host) {
-  int *h = nullptr, *d = nullptr;
-  cudaError_t e = cudaHostAlloc((void **)&h, 8 * 16 * 4 * sizeof(int), cudaHostAllocMapped);
-  if (e != cudaSuccess) return (int)e;
-  for (int i = 0; i < 8 * 16 * 4; ++i) h[i] = 0;
-  if ((e = cudaHostGetDevicePointer((void **)&d, h, 0)) != cudaSuccess) return (int)e;
-  if ((e = cudaMemcpyToSymbol(g_tc_dbg, &d, sizeof(d))) != cudaSuccess) return (int)e;
-  *host = h;
-  return 0;
-}
-#endif
 
 bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld) {
   return ld == kTcF && ctx->knobs.long_tc && C->neg_w_known && !C->has_neg_w;

@@ -1,4 +1,4 @@
-// Internal declarations shared by the translation units of libals_b200.so (sm_100a only).
+// Internal declarations shared by the translation units of libals_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -55,11 +55,11 @@ constexpr int kChunkNnz = 2048;   // ... into chunks of this many nonzeros (mult
 struct als_knobs {
   int short_max = 48;         // ALS_B200_SHORT_MAX: longest row (nonzeros) of the n x n short-row path: 0, 8, ..., 48
   int short_serial = 0;       // ALS_B200_SHORT_SERIAL: short-row kernels on the compute stream instead of the aux stream
-  int whiten_fma = 0;         // ALS_B200_WHITEN_FMA: fp32 FMA tiles for W = Y P, Z = Y G^-1 instead of the tcgen05 apply
+  int whiten_fma = 0;         // ALS_B200_WHITEN_FMA: fp32 FMA tiles for W = Y P, Z = Y G^-1 instead of the wgmma apply
   int gramian_mma = 0;        // ALS_B200_GRAMIAN_MMA: legacy mma.sync Gramian
-  int topk_legacy = 0;        // ALS_B200_TOPK_LEGACY: mma.sync top-k kernel for every call (no tcgen05 path)
-  int gramian_fma = 0;        // ALS_B200_GRAMIAN_FMA: fp32 FMA Gramian instead of the tcgen05 one (64 padded factors)
-  int long_tc = 0;            // ALS_B200_LONG_TC: experimental tcgen05 kernel for the long rows of a Cholesky half (cholesky_tc.cu)
+  int topk_legacy = 0;        // ALS_B200_TOPK_LEGACY: mma.sync top-k kernel for every call (no wgmma path)
+  int gramian_fma = 0;        // ALS_B200_GRAMIAN_FMA: fp32 FMA Gramian instead of the wgmma one (64 padded factors)
+  int long_tc = 0;            // ALS_B200_LONG_TC: experimental wgmma kernel for the long rows of a Cholesky half (cholesky_tc.cu)
   int cg_nv = 2;              // ALS_B200_CG_NV: float4 words per lane of the CG kernel (1 / 2 / 4)
 };
 
@@ -97,7 +97,7 @@ struct als_ctx {
   int64_t whitened_bytes = 0;
   float *zfactors = nullptr;  // Z = Y G^-1
   int64_t zfactors_bytes = 0;
-  float *dense_bt = nullptr;  // [2^14 P | G^-1]^T split into TF32 hi / lo parts for the tcgen05 apply (dense.cu)
+  float *dense_bt = nullptr;  // [2^14 P | G^-1]^T split into TF32 hi / lo parts for the wgmma apply (dense.cu)
   als::WorkItem *deferred = nullptr;
   int64_t deferred_cap = 0;
   // generic scratch (giant-row partial slots, L2 flush, top-k staging)
@@ -153,7 +153,7 @@ struct als_csr {
   int64_t max_row_nnz = 0;     // longest row (known once the schedule is built)
   unsigned *wmax_dev = nullptr;  // device: [0] bits of max | |c| - 1 | over the values, [1] != 0 when some |c| < 1 (cholesky.cu), computed lazily
   bool wmax_valid = false;
-  bool neg_w_known = false, has_neg_w = false;  // host copy of wmax_dev[1]: weights |c| - 1 < 0 exist (then no tcgen05 long-row path)
+  bool neg_w_known = false, has_neg_w = false;  // host copy of wmax_dev[1]: weights |c| - 1 < 0 exist (then no wgmma long-row path)
   bool sched_pending = false;  // transposed on the device: the schedule is built at first use (ensure_schedule)
   als::WorkItem *finish = nullptr;  // finish pass: one per giant row (row, first slot, #slots)
   int64_t n_finish = 0;
@@ -205,15 +205,15 @@ int comm_allreduce_gramian(als_ctx *ctx, int n_floats);                   // sum
 int launch_regularize(als_ctx *ctx, int f, int ld, float lambda);         // ctx->G -> ctx->Greg
 int launch_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);
 int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);
-// long rows on the tcgen05 tensor cores (cholesky_tc.cu): 64 padded factors, no weights |c| - 1 < 0
+// long rows on the wgmma tensor cores (cholesky_tc.cu): 64 padded factors, no weights |c| - 1 < 0
 bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld);
 int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items, cudaStream_t stream);
 // short-row path (cholesky_short.cu).  prepare: P and W from ctx->Greg and Y.  launch: items [begin, n_work) of
 // C->work, all of at most `max_len` nonzeros; whatever it cannot take lands in ctx->deferred / counters[kCtrDeferredCount].
 int short_rows_prepare(als_ctx *ctx, const als_factors *Y, cudaStream_t stream);
-// W = Y (2^14 P) and Z = Y G^-1 in one pass on the tcgen05 tensor cores (dense.cu; 64 padded factors)
+// W = Y (2^14 P) and Z = Y G^-1 in one pass on the wgmma tensor cores (dense.cu; 64 padded factors)
 int launch_dense_whiten(als_ctx *ctx, const als_factors *Y, cudaStream_t stream);
-// G = Y^T Y on the tcgen05 tensor cores (dense.cu; 64 padded factors, Y of at least one row) -> ctx->G
+// G = Y^T Y on the wgmma tensor cores (dense.cu; 64 padded factors, Y of at least one row) -> ctx->G
 int launch_gramian_tc(als_ctx *ctx, const als_factors *Y);
 int launch_gramian_reduce(als_ctx *ctx, int nparts, int n);  // ctx->gram_partials (nparts x n) -> ctx->G, fixed-order fp64 sums
 int short_rows_launch(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t begin, int max_len,
@@ -221,7 +221,7 @@ int short_rows_launch(als_ctx *ctx, const als_csr *C, als_factors *X, const als_
 int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int cg_steps);
 int launch_loss(als_ctx *ctx, const als_csr *C, const als_factors *X, const als_factors *Y, float reg,
                 double *loss);
-// tcgen05 path of the fused top-k (topk_tc.cu): 64 padded factors, k <= 16, large query batches, no item norms
+// wgmma path of the fused top-k (topk_tc.cu): 64 padded factors, k <= 16, large query batches, no item norms
 bool topk_tc_eligible(int ld, int64_t n_query, int64_t n_items, int k, bool has_norms);
 int64_t topk_tc_scratch_bytes(int64_t n_query, int64_t n_items);
 int launch_topk_tc(als_ctx *ctx, const float *items, int64_t n_items, const float *queries, const int32_t *query_rows,

@@ -1,4 +1,4 @@
-// Dense "apply" on the 5th-generation tensor cores: OUT[rows x 128] = Y[rows x 64] * B[64 x 128], fp32-faithful.
+// Dense "apply" on the Hopper tensor cores: OUT[rows x 128] = Y[rows x 64] * B[64 x 128], fp32-faithful.
 //
 // This is the one true dense contraction on the Cholesky half besides the Gramian: the whitened factors
 // W = Y (2^14 P) and the solved factors Z = Y G^-1 of the short-row path (cholesky_short.cu) are two
@@ -6,113 +6,47 @@
 // (The reference has no counterpart: it solves every row with the F x F normal equations, _als.pyx:96-130; the
 // Gramian it precomputes, _als.pyx:70, is what P and G^-1 are derived from.)
 //
-// Blackwell-native data path, one persistent CTA per SM:
-//   warp 0      TMA producer: cp.async.bulk.tensor (128B-swizzled 128 x 32-float boxes) of the Y tile into a
-//               2-stage ring, mbarrier complete_tx; B (hi and lo parts, K-major) is loaded once per CTA;
-//   warp 1      allocates TMEM (2 x 128 columns) and issues tcgen05.mma.kind::tf32, M = 128, N = 128, K = 8:
-//               three products per k-step (hi*hi + lo*hi + hi*lo, the 3xTF32 split) -> 24 MMAs per tile,
-//               accumulators in TMEM, completion signalled with tcgen05.commit;
-//   warps 2-5   split the landed tile in place into its TF32-rounded hi part and the exact remainder lo
-//               (the only SIMT arithmetic), then drain the previous tile's accumulators with tcgen05.ld,
-//               stage them 128B-swizzled in shared memory (W as fp16 hi / lo pairs, the operand format of the
-//               short-row kernel's mma.sync.m16n8k16; Z as fp32) and hand them to TMA stores.
-// The MMAs of tile t run while the workers drain tile t - 1; the kernel is bound by HBM (96 KB per 128 rows).
+// Data path, one persistent CTA per SM with two warpgroups, each owning 64 rows of every 128-row tile:
+//   thread 0    TMA: cp.async.bulk.tensor (128B-swizzled 128 x 32-float boxes) of the Y tiles into a 2-stage ring
+//               (the next tile is in flight while this one is multiplied), mbarrier complete_tx; B (hi and lo parts,
+//               K-major) is loaded once per CTA;
+//   warpgroup   splits its 64 landed rows in place into their TF32-rounded hi part and the exact remainder lo, then
+//               issues wgmma.m64n128k8.tf32: three products per k-step (hi*hi + lo*hi + hi*lo, the 3xTF32 split),
+//               24 wgmmas per tile, accumulators in registers; stages them 128B-swizzled in shared memory (W as fp16
+//               hi / lo pairs, the operand format of the short-row kernel's mma.sync.m16n8k16; Z as fp32) and hands
+//               them to TMA stores, which drain while the next tile is multiplied.
+// The kernel is bound by HBM (96 KB per 128 rows).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
 #include "common.h"
+#include "sm90.cuh"
 
 namespace als {
 
 namespace {
+
+using namespace sm90;
 
 constexpr int kDenseF = 64;        // K: padded factors (the short-row path is only used for F = 64 here)
 constexpr int kDenseN = 128;       // N: [W | Z]
 constexpr int kTileM = 128;
 constexpr int kBoxBytes = kTileM * 128;          // one 128-row x 32-float box, 128B swizzle
 constexpr int kAStage = 2 * kBoxBytes;           // both K halves of a Y tile
-constexpr int kDenseThreads = 192;
+constexpr int kDenseThreads = 256;               // two warpgroups
+constexpr int kOutBox = 64 * 128;                // one 64-row x 32-float output box
 
 // shared memory map (bytes from a 1024-aligned base)
 constexpr int kOffA = 0;                          // 2 stages x 32 KB: raw tile, split in place into its hi part
 constexpr int kOffALo = kOffA + 2 * kAStage;      // 32 KB
 constexpr int kOffBHi = kOffALo + kAStage;        // 32 KB
 constexpr int kOffBLo = kOffBHi + kAStage;        // 32 KB
-constexpr int kOffOut = kOffBLo + kAStage;        // 2 x 16 KB output staging boxes
-constexpr int kOffBar = kOffOut + 2 * kBoxBytes;  // mbarriers + the TMEM base address
+constexpr int kOffOut = kOffBLo + kAStage;        // per warpgroup 4 output boxes (W words 0-31, 32-63, Z 0-31, 32-63)
+constexpr int kOffBar = kOffOut + 2 * 4 * kOutBox;  // mbarriers
 constexpr int kDenseSmem = kOffBar + 128 + 1024;  // + slack for the 1024-byte alignment
+static_assert(kDenseSmem <= 227 * 1024, "dense apply: more shared memory than a Hopper block may have");
 
-enum { kBarFull0 = 0, kBarFull1, kBarB, kBarLoReady, kBarMma0, kBarMma1, kBarTmemFree0, kBarTmemFree1, kNumBars };
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(bar), "r"(parity)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(map)),
-               "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-
-// K-major operand tile, 128B swizzle: rows 128 bytes apart, 8-row groups 1024 bytes apart (SBO), LBO unused (1),
-// descriptor version 1 (Blackwell), layout type 2 = SWIZZLE_128B.  The tile base is 1024-byte aligned.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::tf32, fp32 accumulate, both operands K-major, M = 128, N = 128
-constexpr uint32_t kIdescTf32 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kDenseN >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdescTf32), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
+enum { kBarFull0 = 0, kBarFull1, kBarB, kNumBars };
 
 // hi = x rounded to nearest TF32 (low 13 bits cleared), lo = x - hi exactly (the tensor core drops lo's last bits)
 __device__ __forceinline__ void split4(float4 x, float4 &hi, float4 &lo) {
@@ -126,6 +60,9 @@ __device__ __forceinline__ void split4(float4 x, float4 &hi, float4 &lo) {
   lo.w = x.w - hi.w;
 }
 
+// byte offset of float column c (0..31) of row r in a 128B-swizzled box of 128-byte rows
+__device__ __forceinline__ int sw128(int r, int c) { return r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + ((c & 3) << 2); }
+
 __global__ void __launch_bounds__(kDenseThreads, 1)
 dense_apply_kernel(const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_bhi,
                    const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_w,
@@ -136,155 +73,102 @@ dense_apply_kernel(const __grid_constant__ CUtensorMap map_y, const __grid_const
   unsigned char *gbase = dense_smem_raw + (base - raw);
   const uint32_t bars = base + kOffBar;
   auto bar = [&](int i) -> uint32_t { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(gbase + kOffBar + 8 * kNumBars);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles blockIdx.x + t gridDim.x
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles blockIdx.x + i gridDim.x
+  auto tile_row0 = [&](int i) { return ((int)blockIdx.x + i * (int)gridDim.x) * kTileM; };
 
   if (threadIdx.x == 0) {
     mbar_init(bar(kBarFull0), 1);
     mbar_init(bar(kBarFull1), 1);
     mbar_init(bar(kBarB), 1);
-    mbar_init(bar(kBarLoReady), 128);
-    mbar_init(bar(kBarMma0), 1);
-    mbar_init(bar(kBarMma1), 1);
-    mbar_init(bar(kBarTmemFree0), 128);
-    mbar_init(bar(kBarTmemFree1), 128);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void *)tmem_slot)),
-                 "r"(2 * kDenseN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      mbar_expect_tx(bar(kBarB), 2 * kAStage);
-      tma_load_2d(base + kOffBHi, &map_bhi, bar(kBarB), 0, 0);
-      tma_load_2d(base + kOffBHi + kBoxBytes, &map_bhi, bar(kBarB), 32, 0);
-      tma_load_2d(base + kOffBLo, &map_blo, bar(kBarB), 0, 0);
-      tma_load_2d(base + kOffBLo + kBoxBytes, &map_blo, bar(kBarB), 32, 0);
-      for (int t = 0; t < my_tiles; ++t) {
-        const int s = t & 1;
-        if (t >= 2) mbar_wait(bar(kBarMma0 + s), (uint32_t)(((t >> 1) - 1) & 1));  // the MMAs of tile t - 2 have read the stage
-        const int row0 = ((int)blockIdx.x + t * (int)gridDim.x) * kTileM;
-        mbar_expect_tx(bar(kBarFull0 + s), kAStage);
-        tma_load_2d(base + kOffA + s * kAStage, &map_y, bar(kBarFull0 + s), 0, row0);
-        tma_load_2d(base + kOffA + s * kAStage + kBoxBytes, &map_y, bar(kBarFull0 + s), 32, row0);
-      }
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(bar(kBarB), 2 * kAStage);
+    tma_load_2d(base + kOffBHi, &map_bhi, bar(kBarB), 0, 0);
+    tma_load_2d(base + kOffBHi + kBoxBytes, &map_bhi, bar(kBarB), 32, 0);
+    tma_load_2d(base + kOffBLo, &map_blo, bar(kBarB), 0, 0);
+    tma_load_2d(base + kOffBLo + kBoxBytes, &map_blo, bar(kBarB), 32, 0);
+    for (int i = 0; i < 2 && i < my_tiles; ++i) {
+      mbar_expect_tx(bar(kBarFull0 + i), kAStage);
+      tma_load_2d(base + kOffA + i * kAStage, &map_y, bar(kBarFull0 + i), 0, tile_row0(i));
+      tma_load_2d(base + kOffA + i * kAStage + kBoxBytes, &map_y, bar(kBarFull0 + i), 32, tile_row0(i));
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      mbar_wait(bar(kBarB), 0);
-      for (int t = 0; t < my_tiles; ++t) {
-        const int s = t & 1;
-        mbar_wait(bar(kBarLoReady), (uint32_t)(t & 1));
-        if (t >= 2) mbar_wait(bar(kBarTmemFree0 + s), (uint32_t)(((t >> 1) - 1) & 1));  // accumulator s drained
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d = tmem_base + (uint32_t)(s * kDenseN);
-        const uint32_t a_hi = base + kOffA + s * kAStage, a_lo = base + kOffALo;
-        const uint32_t b_hi = base + kOffBHi, b_lo = base + kOffBLo;
-        uint32_t acc = 0;
-#pragma unroll
-        for (int term = 0; term < 3; ++term) {  // lo * hi, hi * lo, hi * hi (small terms first)
-          const uint32_t a0 = term == 0 ? a_lo : a_hi;
-          const uint32_t b0 = term == 1 ? b_lo : b_hi;
-#pragma unroll
-          for (int ks = 0; ks < kDenseF / 8; ++ks) {
-            const uint32_t off = (uint32_t)((ks >> 2) * kBoxBytes + (ks & 3) * 32);
-            umma_tf32(d, umma_desc_k_sw128(a0 + off), umma_desc_k_sw128(b0 + off), acc);
-            acc = 1;
-          }
-        }
-        umma_commit(bar(kBarMma0 + s));
-      }
-    }
-  } else {
-    // ===== workers: split, then drain the previous tile =====
-    const int wt = threadIdx.x - 64;       // 0..127
-    const int quarter = warp & 3;          // the TMEM lanes this warp may read: 32 quarter .. 32 quarter + 31
-    const int row = 32 * quarter + lane;   // output row of the tile this thread drains
-    auto epilogue = [&](int t) {
-      const int s = t & 1;
-      mbar_wait(bar(kBarMma0 + s), (uint32_t)((t >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int row0 = ((int)blockIdx.x + t * (int)gridDim.x) * kTileM;
-#pragma unroll 1
-      for (int c = 0; c < kDenseN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(32 * quarter) << 16) + (uint32_t)(s * kDenseN + 32 * c), v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        // the staging box of this chunk must have been read by its previous TMA store (2 boxes, 2 groups in flight)
-        if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        unsigned char *box = gbase + kOffOut + (c & 1) * kBoxBytes;
-        if (c < 2) {
-          // W leaves in the split format the short-row kernel multiplies with (cholesky_short.cu): per 16 dimensions
-          // 8 words of fp16 pairs "hi" and 8 words "lo"; this 32-dimension chunk is two such phases = 128 bytes
-          uint32_t w[32];
-#pragma unroll
-          for (int pp = 0; pp < 2; ++pp)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float x0 = __uint_as_float(v[16 * pp + 2 * j]), x1 = __uint_as_float(v[16 * pp + 2 * j + 1]);
-              const __half2 h = __floats2half2_rn(x0, x1);
-              const float2 hf = __half22float2(h);
-              const __half2 lo = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-              w[16 * pp + j] = *reinterpret_cast<const uint32_t *>(&h);
-              w[16 * pp + 8 + j] = *reinterpret_cast<const uint32_t *>(&lo);
-            }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = w[j];
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int pj = j ^ (row & 7);
-          *reinterpret_cast<uint4 *>(box + row * 128 + pj * 16) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (wt == 0) {
-          const CUtensorMap *m = c < 2 ? &map_w : &map_z;
-          tma_store_2d(m, base + kOffOut + (c & 1) * kBoxBytes, 32 * (c & 1), row0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(bar(kBarTmemFree0 + s));
-    };
-    for (int t = 0; t < my_tiles; ++t) {
-      const int s = t & 1;
-      mbar_wait(bar(kBarFull0 + s), (uint32_t)((t >> 1) & 1));
-      if (t >= 1) mbar_wait(bar(kBarMma0 + ((t - 1) & 1)), (uint32_t)(((t - 1) >> 1) & 1));  // the lo buffer is free
-      float4 *a = reinterpret_cast<float4 *>(gbase + kOffA + s * kAStage);
-      float4 *alo = reinterpret_cast<float4 *>(gbase + kOffALo);
+  }
+  mbar_wait(bar(kBarB), 0);
+  unsigned char *out = gbase + kOffOut + wg * 4 * kOutBox;
+  for (int i = 0; i < my_tiles; ++i) {
+    const int s = i & 1;
+    mbar_wait(bar(kBarFull0 + s), (uint32_t)((i >> 1) & 1));
+    // split this warpgroup's 64 rows (8 KB of each K-half box) in place; the swizzle is the same for both buffers
 #pragma unroll 4
-      for (int e = wt; e < kAStage / 16; e += 128) {  // the swizzle is the same for both buffers: a flat pass
-        float4 hi, lo;
-        split4(a[e], hi, lo);
-        a[e] = hi;
-        alo[e] = lo;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(bar(kBarLoReady));
-      if (t >= 1) epilogue(t - 1);
+    for (int e = t; e < 2 * 64 * 8; e += 128) {
+      const int off = (e >> 9) * kBoxBytes + wg * 64 * 128 + (e & 511) * 16;
+      float4 *a = reinterpret_cast<float4 *>(gbase + kOffA + s * kAStage + off);
+      float4 hi, lo;
+      split4(*a, hi, lo);
+      *a = hi;
+      *reinterpret_cast<float4 *>(gbase + kOffALo + off) = lo;
     }
-    if (my_tiles > 0) epilogue(my_tiles - 1);
-    if (wt == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    fence_proxy_async();
+    named_sync(1 + wg, 128);
+    float d[64] = {};
+    const uint32_t a_hi = base + kOffA + s * kAStage + wg * 64 * 128, a_lo = base + kOffALo + wg * 64 * 128;
+    const uint32_t b_hi = base + kOffBHi, b_lo = base + kOffBLo;
+    wgmma_fence();
+#pragma unroll
+    for (int term = 0; term < 3; ++term) {  // lo * hi, hi * lo, hi * hi (small terms first)
+      const uint32_t a0 = term == 0 ? a_lo : a_hi;
+      const uint32_t b0 = term == 1 ? b_lo : b_hi;
+#pragma unroll
+      for (int ks = 0; ks < kDenseF / 8; ++ks) {
+        const uint32_t off = (uint32_t)((ks >> 2) * kBoxBytes + (ks & 3) * 32);
+        wgmma_tf32_m64n128k8(d, wgmma_desc_k_sw128(a0 + off), wgmma_desc_k_sw128(b0 + off), term + ks > 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(d);
+    __syncthreads();  // both warpgroups are done with stage s: refill it with tile i + 2
+    if (threadIdx.x == 0 && i + 2 < my_tiles) {
+      mbar_expect_tx(bar(kBarFull0 + s), kAStage);
+      tma_load_2d(base + kOffA + s * kAStage, &map_y, bar(kBarFull0 + s), 0, tile_row0(i + 2));
+      tma_load_2d(base + kOffA + s * kAStage + kBoxBytes, &map_y, bar(kBarFull0 + s), 32, tile_row0(i + 2));
+    }
+    // epilogue: the staging boxes must have been read by the previous tile's TMA stores
+    if (t == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    named_sync(1 + wg, 128);
+#pragma unroll
+    for (int v = 0; v < 64; v += 2) {
+      const int r = wgmma_row(t, v), c = wgmma_col(t, v);  // c even: the pair (c, c + 1)
+      if (c < kDenseF) {
+        // W leaves in the split format the short-row kernel multiplies with (cholesky_short.cu): per 16 dimensions
+        // 8 words of fp16 pairs "hi" and 8 words "lo"
+        const __half2 h = __floats2half2_rn(d[v], d[v + 1]);
+        const float2 hf = __half22float2(h);
+        const __half2 lo = __floats2half2_rn(d[v] - hf.x, d[v + 1] - hf.y);
+        const int m = c >> 1, w = 16 * (m >> 3) + (m & 7);
+        *reinterpret_cast<__half2 *>(out + (w >> 5) * kOutBox + sw128(r, w & 31)) = h;
+        *reinterpret_cast<__half2 *>(out + ((w + 8) >> 5) * kOutBox + sw128(r, (w + 8) & 31)) = lo;
+      } else {
+        const int z = c - kDenseF;
+        *reinterpret_cast<float2 *>(out + (2 + (z >> 5)) * kOutBox + sw128(r, z & 31)) = make_float2(d[v], d[v + 1]);
+      }
+    }
+    fence_proxy_async();
+    named_sync(1 + wg, 128);
+    if (t == 0) {
+      const int row0 = tile_row0(i) + 64 * wg;
+      const uint32_t ob = base + kOffOut + wg * 4 * kOutBox;
+      tma_store_2d(&map_w, ob, 0, row0);
+      tma_store_2d(&map_w, ob + kOutBox, 32, row0);
+      tma_store_2d(&map_z, ob + 2 * kOutBox, 0, row0);
+      tma_store_2d(&map_z, ob + 3 * kOutBox, 32, row0);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * kDenseN) : "memory");
-  }
+  if (t == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 // B^T = [2^14 P | G^-1]^T (128 x 64, K-major) split into its TF32-rounded hi part and the remainder
@@ -299,41 +183,27 @@ __global__ void dense_prepare_b_kernel(const float *__restrict__ Ps, const float
   }
 }
 
-// ---- Gramian G = Y^T Y on tcgen05 (R4; reference: np.dot(Y.T, Y), implicit/cpu/_als.pyx:70,164,268) ----------
-// The contraction runs over the ROWS of Y, so both operands are the transposed tile.  The worker warps, which have
-// to touch every element anyway for the TF32 hi / lo split, write the split halves TRANSPOSED into a K-major,
+// ---- Gramian G = Y^T Y on the tensor cores (R4; reference: np.dot(Y.T, Y), implicit/cpu/_als.pyx:70,164,268) -------
+// The contraction runs over the ROWS of Y, so both operands are the transposed tile.  The first warpgroup, which has
+// to touch every element anyway for the TF32 hi / lo split, writes the split halves TRANSPOSED into a K-major,
 // 128B-swizzled operand tile T = [hi^T ; lo^T] (128 operand rows = 64 factors hi + 64 factors lo, K = the 128 rows of
-// the landed Y tile): A = hi^T (M = 64) and B = T (N = 128) start at the same address, and one tcgen05.mma
-// kind::tf32 per 8 rows of Y yields hi^T hi (columns 0..63) and hi^T lo (columns 64..127) at once; lo^T hi is the
-// transpose of the second block and is added when the partials are reduced: G = S1 + S2 + S2^T (the 3xTF32 split
-// at two thirds of the tensor work).  Per CTA: TMA producer (128-row tiles, 2 stages), one MMA-issuing lane, four
-// worker warps.  The 64 x 128 accumulator stays in TMEM for the whole sweep and is written once, as this CTA's
-// partial; partials are summed in fp64 in a fixed order.
+// the landed Y tile): A = hi^T (M = 64) and B = T (N = 128) start at the same address, and one wgmma.m64n128k8.tf32
+// per 8 rows of Y yields hi^T hi (columns 0..63) and hi^T lo (columns 64..127) at once; lo^T hi is the transpose of
+// the second block and is added at the end: G = S1 + S2 + S2^T (the 3xTF32 split at two thirds of the tensor work).
+// Per CTA: thread 0 issues the TMA loads (128-row tiles, 2 stages), warpgroup 0 splits and transposes, warpgroup 1
+// multiplies (T is double buffered, so tile t + 1 is transposed while tile t is multiplied).  The 64 x 128 sum is
+// written once, as this CTA's partial; partials are summed in fp64 in a fixed order.
 constexpr int kGramRaw = 2 * kBoxBytes;           // a landed Y tile: cols 0-31 | cols 32-63
 constexpr int kGramT = 4 * kBoxBytes;             // [128 operand rows][128 K] as 4 K-chunks of 32
 constexpr int kGramOffT = 2 * kGramRaw;           // after the 2 raw stages
 constexpr int kGramOffBar = kGramOffT + 2 * kGramT;
 constexpr int kGramSmem = kGramOffBar + 128 + 1024;
-enum { kGFull0 = 0, kGFull1, kGRawFree0, kGRawFree1, kGReady0, kGReady1, kGMma0, kGMma1, kGAccFull0, kGAccFull1, kGAccFree0,
-       kGAccFree1, kGNumBars };
+static_assert(kGramSmem <= 227 * 1024, "Gramian: more shared memory than a Hopper block may have");
+enum { kGFull0 = 0, kGFull1, kGReady0, kGReady1, kGTFree0, kGTFree1, kGNumBars };
 
-// kind::tf32, fp32 accumulate, A and B K-major, M = 64, N = 128
-constexpr uint32_t kIdescGram = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32_idesc(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// The tensor core adds into its fp32 accumulator with truncation (measured: a 250-step chain over all-positive
-// data is biased by 1.2e-5), so a chain is kept to 8 MMAs = 64 rows of Y: two TMEM accumulators alternate, and the
-// worker warps drain each finished chain into fp32 registers with ordinary round-to-nearest additions.
+// A chain is kept to 8 MMAs = 64 rows of Y and each finished chain is added into fp32 registers with ordinary
+// round-to-nearest additions, so that a tensor core that truncates while it accumulates (measured on the previous
+// generation's tensor cores; not measured on H100's wgmma) cannot bias a long all-positive sum.
 __global__ void __launch_bounds__(kDenseThreads, 1)
 gramian_tc_kernel(const __grid_constant__ CUtensorMap map_y, int n_tiles, float *__restrict__ partials) {
   extern __shared__ unsigned char dense_smem_raw[];
@@ -342,98 +212,38 @@ gramian_tc_kernel(const __grid_constant__ CUtensorMap map_y, int n_tiles, float 
   unsigned char *gbase = dense_smem_raw + (base - raw);
   const uint32_t bars = base + kGramOffBar;
   auto bar = [&](int i) -> uint32_t { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(gbase + kGramOffBar + 8 * kGNumBars);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  const int n_chains = 2 * my_tiles;
+  auto tile_row0 = [&](int i) { return ((int)blockIdx.x + i * (int)gridDim.x) * kTileM; };
 
   if (threadIdx.x == 0) {
     mbar_init(bar(kGFull0), 1);
     mbar_init(bar(kGFull1), 1);
-    mbar_init(bar(kGRawFree0), 128);
-    mbar_init(bar(kGRawFree1), 128);
     mbar_init(bar(kGReady0), 128);
     mbar_init(bar(kGReady1), 128);
-    mbar_init(bar(kGMma0), 1);
-    mbar_init(bar(kGMma1), 1);
-    mbar_init(bar(kGAccFull0), 1);
-    mbar_init(bar(kGAccFull1), 1);
-    mbar_init(bar(kGAccFree0), 128);
-    mbar_init(bar(kGAccFree1), 128);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(bar(kGTFree0), 128);
+    mbar_init(bar(kGTFree1), 128);
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void *)tmem_slot)),
-                 "r"(256)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int t = 0; t < my_tiles; ++t) {
-        const int s = t & 1;
-        if (t >= 2) mbar_wait(bar(kGRawFree0 + s), (uint32_t)(((t >> 1) - 1) & 1));  // the workers have read raw stage s
-        const int row0 = ((int)blockIdx.x + t * (int)gridDim.x) * kTileM;
-        mbar_expect_tx(bar(kGFull0 + s), kGramRaw);
-        tma_load_2d(base + s * kGramRaw, &map_y, bar(kGFull0 + s), 0, row0);
-        tma_load_2d(base + s * kGramRaw + kBoxBytes, &map_y, bar(kGFull0 + s), 32, row0);
+  float racc[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) racc[j] = 0.f;
+  if (wg == 0) {
+    // ===== split + transpose the landed tile into the operand tile =====
+    if (t == 0)
+      for (int i = 0; i < 2 && i < my_tiles; ++i) {
+        mbar_expect_tx(bar(kGFull0 + i), kGramRaw);
+        tma_load_2d(base + i * kGramRaw, &map_y, bar(kGFull0 + i), 0, tile_row0(i));
+        tma_load_2d(base + i * kGramRaw + kBoxBytes, &map_y, bar(kGFull0 + i), 32, tile_row0(i));
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int t = 0; t < my_tiles; ++t) {
-        const int s = t & 1;
-        mbar_wait(bar(kGReady0 + s), (uint32_t)((t >> 1) & 1));
-        const uint32_t T = base + kGramOffT + s * kGramT;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {  // a chain = 8 MMAs = 64 rows of Y into accumulator (2t + h) & 1
-          const int c = 2 * t + h, a = c & 1;
-          if (c >= 2) mbar_wait(bar(kGAccFree0 + a), (uint32_t)(((c >> 1) - 1) & 1));  // chain c - 2 has been drained
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-          for (int k8 = 0; k8 < 8; ++k8) {
-            const int ks = 8 * h + k8;  // 8 rows of Y (the K extent of a tf32 MMA) per instruction
-            const uint64_t d = umma_desc_k_sw128(T + (uint32_t)((ks >> 2) * kBoxBytes + (ks & 3) * 32));
-            umma_tf32_idesc(tmem_base + (uint32_t)(a * 128), d, d, kIdescGram, k8 ? 1u : 0u);
-          }
-          umma_commit(bar(kGAccFull0 + a));
-        }
-        umma_commit(bar(kGMma0 + s));  // the operand tile may be overwritten
-      }
-    }
-  } else {
-    // ===== workers: split + transpose the landed tile into the operand tile; drain finished chains =====
-    const int w4 = warp & 3;               // K-chunk of the operand tile = rows 32 w4 .. 32 w4 + 31 of the Y tile
-    const int r = 32 * w4 + lane;          // this lane's row of the Y tile
-    // lanes 0..15 of warp quarter w4 hold row 16 w4 + lane of the 64 x 128 accumulator (M = 64 uses half of every
-    // 32-lane quarter): columns 0..63 = hi^T hi, 64..127 = hi^T lo
-    float racc[128];
-#pragma unroll
-    for (int j = 0; j < 128; ++j) racc[j] = 0.f;
-    auto drain = [&](int c) {
-      const int a = c & 1;
-      mbar_wait(bar(kGAccFull0 + a), (uint32_t)((c >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(32 * w4) << 16) + (uint32_t)(a * 128 + 32 * q), v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 32; ++j) racc[32 * q + j] += __uint_as_float(v[j]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(bar(kGAccFree0 + a));
-    };
-    for (int t = 0; t < my_tiles; ++t) {
-      const int s = t & 1;
-      mbar_wait(bar(kGFull0 + s), (uint32_t)((t >> 1) & 1));
-      if (t >= 2) mbar_wait(bar(kGMma0 + s), (uint32_t)(((t >> 1) - 1) & 1));  // the MMAs of tile t - 2 have read T[s]
+    const int w4 = t >> 5, lane = t & 31;  // K-chunk of the operand tile = rows 32 w4 .. 32 w4 + 31 of the Y tile
+    const int r = t;                       // this thread's row of the Y tile
+    for (int i = 0; i < my_tiles; ++i) {
+      const int s = i & 1;
+      mbar_wait(bar(kGFull0 + s), (uint32_t)((i >> 1) & 1));
+      if (i >= 2) mbar_wait(bar(kGTFree0 + s), (uint32_t)(((i >> 1) - 1) & 1));  // the MMAs of tile i - 2 have read T[s]
       const unsigned char *src = gbase + s * kGramRaw;
       unsigned char *dst = gbase + kGramOffT + s * kGramT + w4 * kBoxBytes;
 #pragma unroll 4
@@ -444,50 +254,64 @@ gramian_tc_kernel(const __grid_constant__ CUtensorMap map_y, int n_tiles, float 
         split4(x, hi, lo);
         const float h[4] = {hi.x, hi.y, hi.z, hi.w}, l[4] = {lo.x, lo.y, lo.z, lo.w};
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int c = 4 * c4 + i;  // operand row c (hi) / 64 + c (lo); K index within the chunk = lane
+        for (int j = 0; j < 4; ++j) {
+          const int c = 4 * c4 + j;  // operand row c (hi) / 64 + c (lo); K index within the chunk = lane
           const int off = (((lane >> 2) ^ (c & 7)) << 4) + ((lane & 3) << 2);  // (64 + c) % 8 == c % 8
-          *reinterpret_cast<float *>(dst + c * 128 + off) = h[i];
-          *reinterpret_cast<float *>(dst + (64 + c) * 128 + off) = l[i];
+          *reinterpret_cast<float *>(dst + c * 128 + off) = h[j];
+          *reinterpret_cast<float *>(dst + (64 + c) * 128 + off) = l[j];
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      fence_proxy_async();
       mbar_arrive(bar(kGReady0 + s));
-      mbar_arrive(bar(kGRawFree0 + s));
-      if (t >= 1) {  // the two chains of the previous tile (its MMAs ran while this tile was transposed)
-        drain(2 * t - 2);
-        drain(2 * t - 1);
+      named_sync(1, 128);  // every thread has read raw stage s: refill it with tile i + 2
+      if (t == 0 && i + 2 < my_tiles) {
+        mbar_expect_tx(bar(kGFull0 + s), kGramRaw);
+        tma_load_2d(base + s * kGramRaw, &map_y, bar(kGFull0 + s), 0, tile_row0(i + 2));
+        tma_load_2d(base + s * kGramRaw + kBoxBytes, &map_y, bar(kGFull0 + s), 32, tile_row0(i + 2));
       }
     }
-    if (my_tiles > 0) {
-      drain(n_chains - 2);
-      drain(n_chains - 1);
-    }
-    // partial of this CTA, symmetrised: P = S1 + S2 + S2^T (S2^T through shared memory: raw stage 0 is free now)
-    float *s2 = reinterpret_cast<float *>(gbase);  // [64][65]
-    const int row = 16 * w4 + lane;
-    if (lane < 16) {
+  } else {
+    // ===== multiply: two chains of 8 wgmmas per tile, each added into racc =====
+    for (int i = 0; i < my_tiles; ++i) {
+      const int s = i & 1;
+      mbar_wait(bar(kGReady0 + s), (uint32_t)((i >> 1) & 1));
+      const uint32_t T = base + kGramOffT + s * kGramT;
 #pragma unroll
-      for (int j = 0; j < 64; ++j) s2[row * 65 + j] = racc[64 + j];
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    if (lane < 16) {
-      float *out = partials + ((size_t)blockIdx.x * 64 + row) * 64;
+      for (int h = 0; h < 2; ++h) {
+        float d[64] = {};
+        wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 64; ++j) out[j] = racc[j] + (racc[64 + j] + s2[j * 65 + row]);
+        for (int k8 = 0; k8 < 8; ++k8) {
+          const int ks = 8 * h + k8;  // 8 rows of Y (the K extent of a tf32 MMA) per instruction
+          const uint64_t desc = wgmma_desc_k_sw128(T + (uint32_t)((ks >> 2) * kBoxBytes + (ks & 3) * 32));
+          wgmma_tf32_m64n128k8(d, desc, desc, k8);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operand(d);
+#pragma unroll
+        for (int j = 0; j < 64; ++j) racc[j] += d[j];
+      }
+      mbar_arrive(bar(kGTFree0 + s));
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
+  __syncthreads();  // every TMA load has landed and been read: raw stage 0 is free
+  if (wg == 1) {
+    // partial of this CTA, symmetrised: P = S1 + S2 + S2^T (S2^T through shared memory)
+    float *s2 = reinterpret_cast<float *>(gbase);  // [64][65]
+#pragma unroll
+    for (int v = 32; v < 64; ++v) s2[wgmma_row(t, v) * 65 + wgmma_col(t, v) - 64] = racc[v];
+    named_sync(2, 128);
+    float *out = partials + (size_t)blockIdx.x * 64 * 64;
+#pragma unroll
+    for (int v = 0; v < 32; ++v) {
+      const int r = wgmma_row(t, v), c = wgmma_col(t, v);
+      out[r * 64 + c] = racc[v] + (racc[v + 32] + s2[c * 65 + r]);
+    }
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+typedef sm90::EncodeTiledFn EncodeTiledFn;
 
 EncodeTiledFn encode_fn() {
   static EncodeTiledFn fn = nullptr;
@@ -503,8 +327,8 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// rows x 64 fp32 row-major matrix, boxes of 128 rows x 32 floats, 128B swizzle
-int make_map(CUtensorMap *m, const float *ptr, int64_t rows) {
+// rows x 64 fp32 row-major matrix, boxes of `box_rows` rows x 32 floats, 128B swizzle
+int make_map(CUtensorMap *m, const float *ptr, int64_t rows, int box_rows = kTileM) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) {
     set_error("dense: cuTensorMapEncodeTiled is not available from this driver");
@@ -512,7 +336,7 @@ int make_map(CUtensorMap *m, const float *ptr, int64_t rows) {
   }
   const cuuint64_t dims[2] = {(cuuint64_t)kDenseF, (cuuint64_t)rows};
   const cuuint64_t strides[1] = {(cuuint64_t)kDenseF * sizeof(float)};
-  const cuuint32_t box[2] = {32, (cuuint32_t)kTileM};
+  const cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(ptr), dims, strides, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -543,8 +367,8 @@ int launch_dense_whiten(als_ctx *ctx, const als_factors *Y, cudaStream_t stream)
   if ((rc = make_map(&my, Y->d, rows)) != ALS_OK) return rc;
   if ((rc = make_map(&mbh, bt_hi, kDenseN)) != ALS_OK) return rc;
   if ((rc = make_map(&mbl, bt_lo, kDenseN)) != ALS_OK) return rc;
-  if ((rc = make_map(&mw, ctx->whitened, rows)) != ALS_OK) return rc;
-  if ((rc = make_map(&mz, ctx->zfactors, rows)) != ALS_OK) return rc;
+  if ((rc = make_map(&mw, ctx->whitened, rows, 64)) != ALS_OK) return rc;
+  if ((rc = make_map(&mz, ctx->zfactors, rows, 64)) != ALS_OK) return rc;
   const int n_tiles = (int)ceil_div(rows, kTileM);
   const int grid = std::min(n_tiles, ctx->sm_count);
   ALS_CUDA(cudaFuncSetAttribute(dense_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDenseSmem));
@@ -554,7 +378,7 @@ int launch_dense_whiten(als_ctx *ctx, const als_factors *Y, cudaStream_t stream)
   return ALS_OK;
 }
 
-// G = Y^T Y for a 64-wide Y on the tcgen05 tensor cores -> ctx->G (the caller regularises)
+// G = Y^T Y for a 64-wide Y on the tensor cores (wgmma) -> ctx->G (the caller regularises)
 int launch_gramian_tc(als_ctx *ctx, const als_factors *Y) {
   const int64_t rows = std::max<int64_t>(Y->rows, 1);
   const int n_tiles = (int)ceil_div(rows, kTileM);

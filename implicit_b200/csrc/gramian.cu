@@ -317,11 +317,11 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
     ctx->launches += 2;
     return ALS_OK;
   }
-  // The mma.sync version is ~25 % faster but the tensor core truncates its fp32 accumulator on every add, which
-  // biases the all-positive diagonal of G by ~1e-6 relative; the FMA version (round to nearest) is the default.
+  // Other widths: the FMA version (round to nearest) is the default; the mma.sync one is kept behind a knob because a
+  // tensor core that truncates while accumulating biases the all-positive diagonal of G.
   if (F == 64 && Y->rows >= 128 && !ctx->knobs.gramian_mma && !ctx->knobs.gramian_fma) {  // (a TMA box is 128 rows)
     ProfScope prof(ctx, kProfGramian);
-    return launch_gramian_tc(ctx, Y);  // tcgen05 + TMA (dense.cu)
+    return launch_gramian_tc(ctx, Y);  // wgmma + TMA (dense.cu)
   }
   const bool mma = F <= 64 && ctx->knobs.gramian_mma;
   const int64_t steps = mma ? ceil_div(std::max<int64_t>(Y->rows, 1), 8 * kGramWarps)

@@ -33,7 +33,7 @@ struct TkCfg {
   static constexpr int LDF = F + 4;              // operand row stride: conflict-free mma fragment reads
   static constexpr int SLD = IT + 4;             // score tile stride
   // 16 warps for the common 64-row block: with 144 KB of shared memory only one CTA fits per SM, and 8
-  // warps (2 per scheduler) left the tensor pipe idle 2/3 of the time (profiles/r01_topk_*_v3.txt)
+  // warps (2 per scheduler) cannot keep the tensor pipe busy
   static constexpr int NW = (TQ >= 4) ? 16 : 8;
   static constexpr int THREADS = 32 * NW;
   static constexpr int ROWS_PER_WARP = QB / NW;
@@ -530,7 +530,7 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
   const int64_t o_nrm = take(item_norms_host ? I * 4 : 0);
   const int64_t o_mask = take(n_filter ? I : 0);
   const int64_t o_fl = take(n_filter * 4);
-  // Large batches at 64 padded factors go to the tcgen05 kernel (topk_tc.cu).  It skips filtered items instead of
+  // Large batches at 64 padded factors go to the wgmma kernel (topk_tc.cu).  It skips filtered items instead of
   // keeping them at -FLT_MAX, which is the same thing as long as every row has k unfiltered items left.
   const bool use_tc = !ctx->knobs.topk_legacy && topk_tc_eligible(items->ld, n_query, I, k_eff, item_norms_host != nullptr) &&
                       (!liked || !liked->sched_pending) &&

@@ -1,25 +1,23 @@
-// R3 on the 5th-generation tensor cores: fused scores + filter + top-k for large query batches at 64 padded factors
+// R3 on the Hopper tensor cores: fused scores + filter + top-k for large query batches at 64 padded factors
 // (reference: topk.topk / _topk_batch, implicit/cpu/topk.pyx:15-67; select<T>, implicit/cpu/select.h:12-39).
 //
 // The score matrix  S = Q I^T  is the one large dense contraction of the hot path (C5: 1M x 1M x 64).  Here it runs
-// on tcgen05.mma with TMEM accumulators and TMA-fed operands; the selection is the epilogue, so a score never
-// leaves the SM:
+// on wgmma with TMA-fed operands; the selection is the epilogue, so a score never leaves the SM:
 //   pre-pass   both factor matrices are split ONCE per call into fp16 hi / lo halves (x 2^e, e from the matrix's
 //              absolute maximum, so the halves carry 22 bits): scores = (Qh + Ql)(Ih + Il)^T ~ Ql Ih^T + Qh Il^T + Qh Ih^T,
 //              fp32-faithful like the 3xTF32 split of topk.cu at half the tensor work and half the operand bytes;
 //   CTA        2 x 128 query rows (hi and lo tiles resident in shared memory, K-major, 128B swizzle) sweep ALL items;
 //              every landed item tile is multiplied with BOTH query tiles (half the L2 -> SM operand traffic of one
-//              query tile per CTA: the sweep streams 256 B per item and CTA):
-//              warp 0   TMA producer: 256-item hi + lo boxes into a 2-stage ring (mbarrier complete_tx);
-//              warp 1   one lane issues, per item tile and query tile, 12 tcgen05.mma.kind::f16 (M = 128, N = 256,
-//                       K = 16) into that query tile's 128 x 256 fp32 accumulator in TMEM (2 x 256 = all 512
-//                       columns), tcgen05.commit per accumulator: tile A is selected from while tile B is multiplied;
-//              warps 2-9 (four per query tile) one THREAD per query row: tcgen05.ld of its 256 scores, a running threshold (the k-th best
-//                       so far) rejects almost everything with one max + compare per 32 scores; survivors are checked
-//                       against the row's liked list (a cursor: both advance in item order) and the global filter
-//                       mask, then inserted into a sorted k-list held in REGISTERS with exactly the reference's
-//                       admission rule (`size < k || score > min.score`, evict the lexicographic (score, id) minimum),
-//                       so ties resolve like select.h.  The MMAs of tile t + 1 run while tile t is selected.
+//              query tile per CTA):
+//              warp 8        TMA producer: 64-item hi + lo boxes into a 4-stage ring (mbarrier complete_tx);
+//              warpgroups    one per query tile: 24 wgmma.m64n64k16.f16 per item tile (two 64-row halves x three
+//              0 and 1       terms x four k-steps) into fp32 registers, parked in shared memory, then one THREAD per
+//                            query row: a running threshold (the k-th best so far) rejects almost everything with one
+//                            max + compare per 32 scores; survivors are checked against the row's liked list (a
+//                            cursor: both advance in item order) and the global filter mask, then inserted into a
+//                            sorted k-list held in REGISTERS with exactly the reference's admission rule
+//                            (`size < k || score > min.score`, evict the lexicographic (score, id) minimum), so ties
+//                            resolve like select.h.  One warpgroup selects while the other one multiplies.
 // Filtered items are skipped instead of being kept at -FLT_MAX: identical to the reference whenever every row has at
 // least k unfiltered items; the caller (topk.cu) checks that bound and uses the mma.sync kernel otherwise.
 #include <cuda.h>
@@ -28,93 +26,33 @@
 #include <limits.h>
 
 #include "common.h"
+#include "sm90.cuh"
 
 namespace als {
 
 namespace {
 
-constexpr int kTkF = 64;
-constexpr int kTkQ = 128;                // query rows per MMA tile
-constexpr int kTkG = 2;                  // query tiles per CTA: both are multiplied with every landed item tile
-constexpr int kTkI = 256;                // items per tile
-constexpr int kTkThreads = 64 + 128 * kTkG;
-constexpr int kQBytes = kTkQ * 128;      // one 128-row x 64-half tile
-constexpr int kIBytes = kTkI * 128;      // one 256-row x 64-half tile
-constexpr int kTkOffQ = 0;               // per query tile: Qh | Ql
-constexpr int kTkOffI = kTkG * 2 * kQBytes;        // 2 stages x (Ih | Il)
-constexpr int kTkOffCand = kTkOffI + 4 * kIBytes;  // [32][256] floats: a chunk of scores per selecting thread, column major
-constexpr int kTkOffBar = kTkOffCand + 32 * 128 * kTkG * 4;
-constexpr int kTkSmem = kTkOffBar + 128 + 1024;
-enum { kTQFull = 0, kTFull0, kTFull1, kTMma0, kTMma1, kTAccFull0, kTAccFull1, kTAccFree0, kTAccFree1, kTNumBars };
+using namespace sm90;
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(bar), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-// K-major fp16 operand tile, 128B swizzle: a row is the 64 halves (128 bytes) of one factor row, 8-row groups are
-// 1024 bytes apart (SBO); descriptor version 1, layout type 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16: A, B fp16 (format 0), fp32 accumulate, both K-major, M = 128, N = 256
-constexpr uint32_t kIdescF16 = (1u << 4) | ((uint32_t)(kTkI >> 3) << 17) | ((uint32_t)(kTkQ >> 4) << 24);
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdescF16), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// tcgen05.ld is asynchronous: the registers are valid only after tcgen05.wait::ld.  The wait below takes the registers as
-// read-write operands, so every use of the values depends on it and the compiler cannot hoist one above the wait; this
-// lets the NEXT chunk's load be in flight while the current chunk is scanned.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+constexpr int kTkF = 64;
+constexpr int kTkQ = 128;                // query rows per warpgroup
+constexpr int kTkG = 2;                  // query tiles (warpgroups) per CTA: both are multiplied with every landed item tile
+constexpr int kTkI = 64;                 // items per tile
+constexpr int kTkStages = 4;
+constexpr int kTkThreads = 128 * kTkG + 32;
+constexpr int kTkProducerWarp = 4 * kTkG;
+constexpr int kQBytes = kTkQ * 128;      // one 128-row x 64-half tile
+constexpr int kIBytes = kTkI * 128;      // one 64-row x 64-half tile
+constexpr int kScLd = kTkI + 1;          // parked scores: one row per query, padded against bank conflicts
+constexpr int kTkOffQ = 0;               // per query tile: Qh | Ql
+constexpr int kTkOffI = kTkG * 2 * kQBytes;               // kTkStages x (Ih | Il)
+constexpr int kTkOffSc = kTkOffI + kTkStages * 2 * kIBytes;  // per query tile [128][kScLd] floats
+constexpr int kTkOffBar = kTkOffSc + kTkG * kTkQ * kScLd * 4;
+constexpr int kTkSmem = kTkOffBar + 128 + 1024;
+static_assert(kTkSmem <= 227 * 1024, "top-k: more shared memory than a Hopper block may have");
+enum { kTQFull = 0, kTFull0, kTEmpty0 = kTFull0 + kTkStages, kTNumBars = kTEmpty0 + kTkStages };
+
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // ---- pre-pass -------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) tk_absmax_kernel(const float *__restrict__ x, int ld, const int32_t *__restrict__ rows,
@@ -187,36 +125,22 @@ topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   unsigned char *gbase = tk_smem_raw + (base - raw);
   const uint32_t bars = base + kTkOffBar;
   auto bar = [&](int i) -> uint32_t { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(gbase + kTkOffBar + 8 * kTNumBars);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int n_tiles = (n_items + kTkI - 1) / kTkI;
   const int q0 = (int)blockIdx.x * kTkQ * kTkG;
 
   if (threadIdx.x == 0) {
     mbar_init(bar(kTQFull), 1);
-    mbar_init(bar(kTFull0), 1);
-    mbar_init(bar(kTFull1), 1);
-    mbar_init(bar(kTMma0), 1);
-    mbar_init(bar(kTMma1), 1);
-    mbar_init(bar(kTAccFull0), 1);
-    mbar_init(bar(kTAccFull1), 1);
-    mbar_init(bar(kTAccFree0), 128);
-    mbar_init(bar(kTAccFree1), 128);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < kTkStages; ++s) {
+      mbar_init(bar(kTFull0 + s), 1);
+      mbar_init(bar(kTEmpty0 + s), kTkG);
+    }
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void *)tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp == kTkProducerWarp) {
+    if ((threadIdx.x & 31) == 0) {
       mbar_expect_tx(bar(kTQFull), kTkG * 2 * kQBytes);
 #pragma unroll
       for (int gq = 0; gq < kTkG; ++gq) {
@@ -224,150 +148,124 @@ topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
         tma_load_2d(base + kTkOffQ + gq * 2 * kQBytes + kQBytes, &map_ql, bar(kTQFull), 0, q0 + gq * kTkQ);
       }
       for (int t = 0; t < n_tiles; ++t) {
-        const int s = t & 1;
-        if (t >= 2) mbar_wait(bar(kTMma0 + s), (uint32_t)(((t >> 1) - 1) & 1));  // the MMAs of tile t - 2 have read the stage
+        const int s = t % kTkStages;
+        if (t >= kTkStages) mbar_wait(bar(kTEmpty0 + s), (uint32_t)((t / kTkStages - 1) & 1));  // both warpgroups have read it
         mbar_expect_tx(bar(kTFull0 + s), 2 * kIBytes);
         tma_load_2d(base + kTkOffI + s * 2 * kIBytes, &map_ih, bar(kTFull0 + s), 0, t * kTkI);
         tma_load_2d(base + kTkOffI + s * 2 * kIBytes + kIBytes, &map_il, bar(kTFull0 + s), 0, t * kTkI);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(bar(kTQFull), 0);
-      for (int t = 0; t < n_tiles; ++t) {
-        const int s = t & 1;
-        mbar_wait(bar(kTFull0 + s), (uint32_t)((t >> 1) & 1));
-        const uint32_t ih = base + kTkOffI + s * 2 * kIBytes, il = ih + kIBytes;
+    return;
+  }
+
+  // ===== one warpgroup per query tile: multiply, park the scores, select with one thread per query row =====
+  const int gq = warp >> 2;
+  const int st = threadIdx.x & 127;
+  float *sc = reinterpret_cast<float *>(gbase + kTkOffSc) + gq * kTkQ * kScLd;
+  const float *my_row = sc + st * kScLd;
+  const int q = q0 + gq * kTkQ + st;
+  const bool live = q < n_query;
+  float ls[KMAX];
+  int lc[KMAX];
 #pragma unroll
-        for (int gq = 0; gq < kTkG; ++gq) {
-          if (t >= 1) mbar_wait(bar(kTAccFree0 + gq), (uint32_t)((t - 1) & 1));  // tile t - 1 has been selected from
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d = tmem_base + (uint32_t)(gq * kTkI);
-          const uint32_t qh = base + kTkOffQ + gq * 2 * kQBytes, ql = qh + kQBytes;
-          uint32_t acc = 0;
-#pragma unroll
-          for (int term = 0; term < 3; ++term) {  // lo * hi, hi * lo, hi * hi (small terms first)
-            const uint32_t a0 = term == 0 ? ql : qh;
-            const uint32_t b0 = term == 1 ? il : ih;
-#pragma unroll
-            for (int ks = 0; ks < kTkF / 16; ++ks) {
-              umma_f16(d, umma_desc_k_sw128(a0 + ks * 32), umma_desc_k_sw128(b0 + ks * 32), acc);
-              acc = 1;
-            }
-          }
-          umma_commit(bar(kTAccFull0 + gq));
-        }
-        umma_commit(bar(kTMma0 + s));  // both query tiles have read the stage
-      }
-    }
-  } else {
-    // ===== selection: one thread per query row =====
-    const int quarter = warp & 3;      // the TMEM lanes this warp may read
-    const int gq = (warp - 2) >> 2;    // which query tile (accumulator) this warp selects from
-    const int st = threadIdx.x - 64;   // 0 .. 128 kTkG - 1
-    constexpr int kCandLd = 128 * kTkG;
-    float *cand = reinterpret_cast<float *>(gbase + kTkOffCand);
-    const int q = q0 + gq * kTkQ + 32 * quarter + lane;
-    const bool live = q < n_query;
-    float ls[KMAX];
-    int lc[KMAX];
-#pragma unroll
-    for (int j = 0; j < KMAX; ++j) {
-      ls[j] = -INFINITY;  // empty slots rank below every real (score, id)
-      lc[j] = -1;
-    }
-    float thr = -INFINITY;  // score of the k-th best so far (raw, scaled domain): admission is score > thr
-    int lp = 0, lend = 0, lnext = INT_MAX;
-    if (live && liked_indptr) {
-      lp = liked_indptr[q];
-      lend = liked_indptr[q + 1];
+  for (int j = 0; j < KMAX; ++j) {
+    ls[j] = -INFINITY;  // empty slots rank below every real (score, id)
+    lc[j] = -1;
+  }
+  float thr = -INFINITY;  // score of the k-th best so far (raw, scaled domain): admission is score > thr
+  int lp = 0, lend = 0, lnext = INT_MAX;
+  if (live && liked_indptr) {
+    lp = liked_indptr[q];
+    lend = liked_indptr[q + 1];
+    lnext = lp < lend ? liked_indices[lp] : INT_MAX;
+  }
+  auto consider = [&](float s, int id) {
+    if (id >= n_items) return;
+    while (lnext < id) {  // both the candidates and the liked list come in increasing item order
+      ++lp;
       lnext = lp < lend ? liked_indices[lp] : INT_MAX;
     }
-    auto consider = [&](float sc, int id) {
-      if (id >= n_items) return;
-      while (lnext < id) {  // both the candidates and the liked list come in increasing item order
-        ++lp;
-        lnext = lp < lend ? liked_indices[lp] : INT_MAX;
-      }
-      if (lnext == id) return;                    // topk.pyx:51-54
-      if (item_mask && item_mask[id]) return;     // topk.pyx:55-56
-      float cs = sc;
-      int ci = id;
+    if (lnext == id) return;                    // topk.pyx:51-54
+    if (item_mask && item_mask[id]) return;     // topk.pyx:55-56
+    float cs = s;
+    int ci = id;
 #pragma unroll
-      for (int j = 0; j < KMAX; ++j) {  // carry the smaller element down the sorted list
-        const bool sw = pair_greater(cs, ci, ls[j], lc[j]);
-        const float ts = ls[j];
-        const int ti = lc[j];
-        ls[j] = sw ? cs : ts;
-        lc[j] = sw ? ci : ti;
-        cs = sw ? ts : cs;
-        ci = sw ? ti : ci;
-      }
-#pragma unroll
-      for (int j = 0; j < KMAX; ++j)
-        if (j == k - 1) thr = ls[j];
-    };
-    // one 32-column chunk of the accumulator row: skip it unless something beats the k-th best so far
-    auto scan = [&](const uint32_t (&r)[32], int id0) {
-      float m[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) m[j] = fmax3(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]));
-#pragma unroll
-      for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], __uint_as_float(r[4 * j + 3]));
-      const float mm = fmaxf(fmax3(m[0], m[1], m[2]), fmaxf(fmax3(m[3], m[4], m[5]), fmaxf(m[6], m[7])));
-      if (live && mm > thr) {
-        // rare after the first tiles: park the chunk in shared memory (one column per thread, conflict free) and walk
-        // it in item order with a rolled loop, so the k-list code exists once and its arrays stay in registers
-#pragma unroll
-        for (int j = 0; j < 32; ++j) cand[j * kCandLd + st] = __uint_as_float(r[j]);
-#pragma unroll 1
-        for (int j = 0; j < 32; ++j) {
-          const float sc = cand[j * kCandLd + st];
-          if (sc > thr) consider(sc, id0 + j);
-        }
-      }
-    };
-    const uint32_t trow = tmem_base + ((uint32_t)(32 * quarter) << 16) + (uint32_t)(gq * kTkI);
-    for (int t = 0; t < n_tiles; ++t) {
-      mbar_wait(bar(kTAccFull0 + gq), (uint32_t)(t & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t ra[32], rb[32];
-      tmem_ld32_issue(trow, ra);
-#pragma unroll 1
-      for (int c = 0; c < kTkI / 32; c += 2) {
-        tmem_ld32_wait(ra);
-        tmem_ld32_issue(trow + 32 * (c + 1), rb);
-        scan(ra, t * kTkI + 32 * c);
-        tmem_ld32_wait(rb);
-        if (c + 2 < kTkI / 32) tmem_ld32_issue(trow + 32 * (c + 2), ra);
-        scan(rb, t * kTkI + 32 * (c + 1));
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(bar(kTAccFree0 + gq));
+    for (int j = 0; j < KMAX; ++j) {  // carry the smaller element down the sorted list
+      const bool sw = pair_greater(cs, ci, ls[j], lc[j]);
+      const float ts = ls[j];
+      const int ti = lc[j];
+      ls[j] = sw ? cs : ts;
+      lc[j] = sw ? ci : ti;
+      cs = sw ? ts : cs;
+      ci = sw ? ti : ci;
     }
-    if (live) {
-      // scores leave the scaled domain: exact multiplications by powers of two
-      const float inv_q = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_q)) << 23);
-      const float inv_i = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_i)) << 23);
 #pragma unroll
-      for (int j = 0; j < KMAX; ++j)
-        if (j < k && lc[j] >= 0) {  // the tail stays zero when fewer than k items qualified (topk.pyx:20-21)
-          out_ids[(int64_t)q * k + j] = lc[j];
-          out_scores[(int64_t)q * k + j] = ls[j] * inv_q * inv_i;
-        }
+    for (int j = 0; j < KMAX; ++j)
+      if (j == k - 1) thr = ls[j];
+  };
+  // one 32-column chunk of the parked row: skip it unless something beats the k-th best so far
+  auto scan = [&](const float *r, int id0) {
+    float m[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) m[j] = fmax3(r[4 * j], r[4 * j + 1], r[4 * j + 2]);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], r[4 * j + 3]);
+    const float mm = fmaxf(fmax3(m[0], m[1], m[2]), fmaxf(fmax3(m[3], m[4], m[5]), fmaxf(m[6], m[7])));
+    if (live && mm > thr) {
+      // rare after the first tiles: walk the chunk in item order with a rolled loop, so the k-list code exists once
+      // and its arrays stay in registers
+#pragma unroll 1
+      for (int j = 0; j < 32; ++j) {
+        const float s = r[j];
+        if (s > thr) consider(s, id0 + j);
+      }
     }
+  };
+  const uint32_t qh = base + kTkOffQ + gq * 2 * kQBytes, ql = qh + kQBytes;
+  mbar_wait(bar(kTQFull), 0);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int s = t % kTkStages;
+    mbar_wait(bar(kTFull0 + s), (uint32_t)((t / kTkStages) & 1));
+    const uint32_t ih = base + kTkOffI + s * 2 * kIBytes, il = ih + kIBytes;
+    float d[2][32] = {};
+    wgmma_fence();
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+      for (int term = 0; term < 3; ++term) {  // lo * hi, hi * lo, hi * hi (small terms first)
+        const uint32_t a0 = (term == 0 ? ql : qh) + mh * 64 * 128;
+        const uint32_t b0 = term == 1 ? il : ih;
+#pragma unroll
+        for (int ks = 0; ks < kTkF / 16; ++ks)
+          wgmma_f16_m64n64k16(d[mh], wgmma_desc_k_sw128(a0 + ks * 32), wgmma_desc_k_sw128(b0 + ks * 32), term + ks > 0);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(d[0]);
+    wgmma_fence_operand(d[1]);
+    if (st == 0) mbar_arrive(bar(kTEmpty0 + s));
+    named_sync(1 + gq, 128);  // every row of the previous tile has been scanned
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+      for (int v = 0; v < 32; ++v) sc[(64 * mh + wgmma_row(st, v)) * kScLd + wgmma_col(st, v)] = d[mh][v];
+    named_sync(1 + gq, 128);
+    scan(my_row, t * kTkI);
+    scan(my_row + 32, t * kTkI + 32);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  if (live) {
+    // scores leave the scaled domain: exact multiplications by powers of two
+    const float inv_q = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_q)) << 23);
+    const float inv_i = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_i)) << 23);
+#pragma unroll
+    for (int j = 0; j < KMAX; ++j)
+      if (j < k && lc[j] >= 0) {  // the tail stays zero when fewer than k items qualified (topk.pyx:20-21)
+        out_ids[(int64_t)q * k + j] = lc[j];
+        out_scores[(int64_t)q * k + j] = ls[j] * inv_q * inv_i;
+      }
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // rows x 64 fp16 row-major (128-byte rows), boxes of `box_rows` rows, 128B swizzle, rows past the end read as zero
 int make_half_map(CUtensorMap *m, const void *ptr, int64_t rows, int box_rows) {
@@ -404,7 +302,7 @@ int64_t topk_tc_scratch_bytes(int64_t n_query, int64_t n_items) {
 }
 
 bool topk_tc_eligible(int ld, int64_t n_query, int64_t n_items, int k, bool has_norms) {
-  return ld == kTkF && k >= 1 && k <= 16 && !has_norms && n_query >= 1024 && n_items >= kTkI;
+  return ld == kTkF && k >= 1 && k <= 16 && !has_norms && n_query >= 1024 && n_items >= 256;
 }
 
 // out_ids / out_scores: device [n_query][k], zero-initialised by the caller; query_rows: device indices or nullptr

@@ -1,5 +1,5 @@
 /*
- * als_b200.h -- C-ABI of libals_b200.so: the B200 (sm_100a) ALS fit / recommend hot path.
+ * als_b200.h -- C-ABI of libals_b200.so: the H100 (sm_90a) ALS fit / recommend hot path.
  *
  * This is the drop-in boundary for benfred/implicit's ALS hot path.  Every entry point names the
  * reference interface it replaces (file:line relative to the reference repository).  The reference
@@ -145,7 +145,7 @@ int als_least_squares_with_gramian(als_ctx *ctx, const float *YtY_host, const al
                                    const als_factors *Y, double regularization, int64_t *bad_row);
 
 /* The per-half preprocessing of the short-row path, downloaded: W = Y P with Y^T Y + reg I = R^T R, P = R^-1
- * (whitened factors) and Z = Y (Y^T Y + reg I)^-1, both rows x factors floats.  Produced on the tcgen05
+ * (whitened factors) and Z = Y (Y^T Y + reg I)^-1, both rows x factors floats.  Produced on the wgmma
  * tensor cores for 64 padded factors (csrc/dense.cu).  Test / tooling entry: the reference has no
  * counterpart (it forms every row's F x F normal equations, implicit/cpu/_als.pyx:96-130). */
 int als_whitened_factors(als_ctx *ctx, const als_factors *Y, double regularization, float *W_host, float *Z_host);

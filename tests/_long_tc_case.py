@@ -1,5 +1,5 @@
 """Helper of tests/test_gpu_long_tc.py (run as a subprocess so that a hanging kernel cannot take the suite with it):
-one Cholesky half over rows of 0 ... 3500 nonzeros with the tcgen05 long-row kernel (knob long_tc) and with the
+one Cholesky half over rows of 0 ... 3500 nonzeros with the wgmma long-row kernel (knob long_tc) and with the
 mma.sync kernel, both against the oracle.  Prints one JSON line."""
 import json
 import os

@@ -54,21 +54,23 @@ def test_product_does_not_import_the_oracle():
 
 
 def test_graft_entry_build_runs():
-    """The driver's build check: compiles (or finds up to date) the library, the oracle port and, where the
-    reference is present, oracle/_ref -- and every header symbol resolves."""
+    """build() compiles (or finds up to date) the library, the oracle port and, where the reference is present,
+    oracle/_ref -- and every header symbol resolves."""
     import __graft_entry__ as entry
 
     assert entry.build() is None
     import oracle
+    from oracle import build_ref_gpu
 
-    if os.path.isdir("/root/reference"):
+    if os.path.isdir(build_ref_gpu.REFERENCE):
         assert oracle.have_ref() and oracle.have_ref_evaluation()
 
 
-def test_library_holds_the_blackwell_paths():
-    """The sm_100a-specific data paths are in the built library, kernel by kernel (cuobjdump, no GPU needed): tcgen05
-    MMAs with TMEM loads and TMA in the dense pre-pass, the Gramian and the top-k kernel; tcgen05 + setmaxnreg in the
-    opt-in long-row kernel.  A refactor that silently falls back to mma.sync everywhere fails here."""
+def test_library_holds_the_hopper_paths():
+    """The sm_90a-specific data paths are in the built library, kernel by kernel (cuobjdump, no GPU needed): wgmma
+    (HGMMA) fed by TMA loads in the dense pre-pass, the Gramian and the top-k kernel, and TMA stores in the dense
+    pre-pass; wgmma + setmaxnreg in the opt-in long-row kernel.  A refactor that silently falls back to mma.sync
+    everywhere fails here."""
     import shutil
     import subprocess
 
@@ -85,7 +87,7 @@ def test_library_holds_the_blackwell_paths():
             fn = line.split("Function :")[1].strip()
             per_kernel[fn] = set()
         elif fn is not None:
-            for m in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM", "USETMAXREG"):
+            for m in ("HGMMA", "UTMALDG", "UTMASTG", "USETMAXREG"):
                 if m in line:
                     per_kernel[fn].add(m)
 
@@ -93,7 +95,7 @@ def test_library_holds_the_blackwell_paths():
         hits = [ms for name, ms in per_kernel.items() if kernel in name]
         return bool(hits) and all(any(m in ms for ms in hits) for m in mnemonics)
 
-    assert has("dense_apply_kernel", "UTCHMMA", "UTMALDG", "UTMASTG", "LDTM")
-    assert has("gramian_tc_kernel", "UTCHMMA", "UTMALDG", "LDTM")
-    assert has("topk_tc_kernel", "UTCHMMA", "UTMALDG", "LDTM")
-    assert has("cholesky_tc_kernel", "UTCHMMA", "LDTM", "USETMAXREG")
+    assert has("dense_apply_kernel", "HGMMA", "UTMALDG", "UTMASTG")
+    assert has("gramian_tc_kernel", "HGMMA", "UTMALDG")
+    assert has("topk_tc_kernel", "HGMMA", "UTMALDG")
+    assert has("cholesky_tc_kernel", "HGMMA", "USETMAXREG")

@@ -1,5 +1,5 @@
 """Full-size parity (BASELINE.json configs C2, C3, C5) on the GPU against the CPU oracle: what bench.py times is
-what these tests check.  Every call goes Python -> ctypes -> C-ABI -> sm_100a kernels.
+what these tests check.  Every call goes Python -> ctypes -> C-ABI -> sm_90a kernels.
 
   C2  (360k x 300k, 17M nnz, f=64, Cholesky): a WARM user half (after one GPU iteration) on a row sample against
       the reference's _least_squares with the same Gramian, asserted at 1e-4; and the 3-iteration fit bench.py
@@ -233,10 +233,10 @@ def test_least_squares_with_gramian_matches_reference(lib, ctx, orc, f):
     assert e.max() < CHOL_MAX
 
 
-# ---------------------------------------------------------------------------------------- tcgen05 top-k at mid size
+# ---------------------------------------------------------------------------------------- tensor-core top-k at mid size
 @pytest.mark.parametrize("k", [1, 10, 16])
 def test_topk_tcgen05_path_matches_oracle_and_legacy_kernel(lib, ctx, orc, k):
-    """The tcgen05 kernel (csrc/topk_tc.cu: batches of >= 1024 queries, 64 factors, k <= 16) against the reference's
+    """The wgmma kernel (csrc/topk_tc.cu: batches of >= 1024 queries, 64 factors, k <= 16) against the reference's
     topk and against the mma.sync kernel (knob topk_legacy), with a liked CSR, a global filter list, a ragged last
     query tile and a ragged last item tile."""
     Q, I, f = 3000 + 37, 5000 + 113, 64
@@ -261,7 +261,7 @@ def test_topk_tcgen05_path_matches_oracle_and_legacy_kernel(lib, ctx, orc, k):
     same = ids == eids
     noise = 4 * np.finfo(np.float32).eps * np.linalg.norm(users, axis=1)[:, None] * np.linalg.norm(items, axis=1).max()
     bad = (~same) & (np.abs(sc - esc) > noise)
-    print(f"tcgen05 top-k k={k}: ids equal to the reference {same.mean():.6f} (true mismatches {bad.sum()}), to the mma.sync kernel "
+    print(f"wgmma top-k k={k}: ids equal to the reference {same.mean():.6f} (true mismatches {bad.sum()}), to the mma.sync kernel "
           f"{(ids == ids_old).mean():.6f}; score rel err {np.abs(sc - esc).max() / np.abs(esc).max():.2e}")
     assert bad.sum() == 0 and same.mean() > 0.999
     np.testing.assert_allclose(sc, esc, rtol=2e-5, atol=1e-6)

@@ -1,4 +1,4 @@
-"""The opt-in tcgen05 long-row kernel (csrc/cholesky_tc.cu, knob long_tc) against the oracle and against the default
+"""The opt-in wgmma long-row kernel (csrc/cholesky_tc.cu, knob long_tc) against the oracle and against the default
 mma.sync kernel.  Runs in a subprocess with a time limit: a synchronisation bug in a warp-specialised kernel shows up
 as a hang, and that must fail this test only."""
 import json

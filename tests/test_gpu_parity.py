@@ -1,4 +1,4 @@
-"""GPU parity tests proper: every call goes Python -> ctypes -> C-ABI (include/als_b200.h) -> sm_100a kernels,
+"""GPU parity tests proper: every call goes Python -> ctypes -> C-ABI (include/als_b200.h) -> sm_90a kernels,
 and is compared with the CPU oracle (the reference's own compiled Cython when oracle/_ref is present,
 else its C restatement) on the same seeded inputs, and with the committed golden vectors."""
 import numpy as np

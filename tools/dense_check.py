@@ -1,4 +1,4 @@
-"""tcgen05 apply (csrc/dense.cu) against an fp64 product: W = Y P and Z = Y G^-1 on C2-sized factor matrices,
+"""wgmma apply (csrc/dense.cu) against an fp64 product: W = Y P and Z = Y G^-1 on C2-sized factor matrices,
 with the fp32 FMA tiles (ALS_B200_WHITEN_FMA=1 in a second process) as the comparison point, and its timing."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,7 +22,7 @@ for rows, kind in ((1000, "normal"), (300000, "cold"), (360037, "normal")):
     ew, ez = err(W, Wt), err(Z, Zt)
     print(f"rows {rows} ({kind}): W max-rel {ew[0]:.2e} row-median {ew[1]:.2e} | Z max-rel {ez[0]:.2e} row-median {ez[1]:.2e} | cond(G) {np.linalg.cond(G):.1e}", flush=True)
     Gt = Y64.T @ Y64
-    for knob, name in ((0, "tcgen05"), (1, "fma")):
+    for knob, name in ((0, "wgmma"), (1, "fma")):
         ctx.set_knob("gramian_fma", knob)
         Gg = _lib.gramian(ctx, Y)
         ctx.profile(True); ctx.profile_read()

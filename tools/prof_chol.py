@@ -1,4 +1,4 @@
-"""Workload for ncu captures: a few C2 half-iterations (Cholesky by default, --cg for CG)."""
+"""Workload for profiler captures: a few C2 half-iterations (Cholesky by default, --cg for CG)."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Workload for ncu captures of the fused top-k: Q queries (default 2 waves of 128-row CTAs) x 1M items, f=64, k=10."""
+"""Workload for profiler captures of the fused top-k: Q queries (default 2 waves of 128-row CTAs) x 1M items, f=64, k=10."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
