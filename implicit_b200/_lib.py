@@ -164,7 +164,7 @@ class Context:
         check(self.lib.als_sync(self.h))
 
     def set_knob(self, name, value):
-        """Measurement knobs (short_max, short_serial, whiten_fma, gramian_mma, cg_nv); see include/als_b200.h."""
+        """Measurement knobs (short_max, short_serial, whiten_fma, gramian_fma, topk_legacy, cg_nv); see include/als_b200.h."""
         check(self.lib.als_ctx_set_knob(self.h, name.encode(), int(value)))
 
     def info(self):

@@ -301,7 +301,7 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   {
     struct { const char *env; const char *name; } table[] = {
         {"ALS_B200_SHORT_MAX", "short_max"}, {"ALS_B200_SHORT_SERIAL", "short_serial"}, {"ALS_B200_WHITEN_FMA", "whiten_fma"},
-        {"ALS_B200_GRAMIAN_MMA", "gramian_mma"}, {"ALS_B200_GRAMIAN_FMA", "gramian_fma"}, {"ALS_B200_TOPK_LEGACY", "topk_legacy"}, {"ALS_B200_LONG_TC", "long_tc"}, {"ALS_B200_CG_NV", "cg_nv"}};
+        {"ALS_B200_GRAMIAN_FMA", "gramian_fma"}, {"ALS_B200_TOPK_LEGACY", "topk_legacy"}, {"ALS_B200_LONG_TC", "long_tc"}, {"ALS_B200_CG_NV", "cg_nv"}};
     for (const auto &t : table) {
       const char *e = getenv(t.env);
       if (!e) continue;
@@ -360,7 +360,6 @@ ALS_API int als_ctx_set_knob(als_ctx *ctx, const char *name, int value) {
   if (!strcmp(name, "short_max")) k.short_max = value >= 48 ? 48 : value <= 0 ? 0 : value / 8 * 8;
   else if (!strcmp(name, "short_serial")) k.short_serial = value != 0;
   else if (!strcmp(name, "whiten_fma")) k.whiten_fma = value != 0;
-  else if (!strcmp(name, "gramian_mma")) k.gramian_mma = value != 0;
   else if (!strcmp(name, "gramian_fma")) k.gramian_fma = value != 0;
   else if (!strcmp(name, "topk_legacy")) k.topk_legacy = value != 0;
   else if (!strcmp(name, "long_tc")) k.long_tc = value != 0;
@@ -675,6 +674,8 @@ ALS_API int als_csr_destroy(als_csr *csr) {
       dev_free(ctx, csr->data);
     }
     dev_free(ctx, csr->wmax_dev);
+    dev_free(ctx, csr->sorted_indptr);
+    dev_free(ctx, csr->sorted_indices);
     dev_free(ctx, csr->work);
     dev_free(ctx, csr->finish);
     dev_free(ctx, csr->chunks);

@@ -56,7 +56,6 @@ struct als_knobs {
   int short_max = 48;         // ALS_B200_SHORT_MAX: longest row (nonzeros) of the n x n short-row path: 0, 8, ..., 48
   int short_serial = 0;       // ALS_B200_SHORT_SERIAL: short-row kernels on the compute stream instead of the aux stream
   int whiten_fma = 0;         // ALS_B200_WHITEN_FMA: fp32 FMA tiles for W = Y P, Z = Y G^-1 instead of the wgmma apply
-  int gramian_mma = 0;        // ALS_B200_GRAMIAN_MMA: legacy mma.sync Gramian
   int topk_legacy = 0;        // ALS_B200_TOPK_LEGACY: mma.sync top-k kernel for every call (no wgmma path)
   int gramian_fma = 0;        // ALS_B200_GRAMIAN_FMA: fp32 FMA Gramian instead of the wgmma one (64 padded factors)
   int long_tc = 0;            // ALS_B200_LONG_TC: experimental wgmma kernel for the long rows of a Cholesky half (cholesky_tc.cu)
@@ -155,6 +154,11 @@ struct als_csr {
   bool wmax_valid = false;
   bool neg_w_known = false, has_neg_w = false;  // host copy of wmax_dev[1]: weights |c| - 1 < 0 exist (then no wgmma long-row path)
   bool sched_pending = false;  // transposed on the device: the schedule is built at first use (ensure_schedule)
+  // as the liked lists of als_topk, whose fused kernels walk each row's columns in ascending order: checked once on
+  // the device at first use; a CSR with an unsorted row gets a sorted copy (indptr rebased to 0) kept for later calls
+  bool order_known = false;
+  int32_t *sorted_indptr = nullptr;
+  int32_t *sorted_indices = nullptr;
   als::WorkItem *finish = nullptr;  // finish pass: one per giant row (row, first slot, #slots)
   int64_t n_finish = 0;
   int64_t n_slots = 0;

@@ -4,10 +4,10 @@
 // Bandwidth-bound reduction over the rows of Y (f/2 flop per byte): every CTA streams rows through shared
 // memory and writes one F x F partial; a second tiny kernel sums the partials in a fixed order in fp64 so the
 // result is deterministic and independent of the grid size rounding.
-//   f <= 64:  gramian_mma_kernel -- each warp streams 8-row steps through a 4-deep cp.async ring and accumulates
-//             the upper-triangular 16x8 tiles with mma.sync 3xTF32 (the accumulation step of cholesky.cu with unit
-//             weights: fp32-faithful), the 8 warps of a CTA are summed in a fixed tree;
+//   64 padded factors: gramian_tc_kernel on wgmma (dense.cu), unless the gramian_fma knob is set;
 //   f <= 128: gramian_partial_kernel -- fp32 FMA register tiles (the CG configurations).
+// An mma.sync 3xTF32 variant (long fp32 accumulator chains on the tensor core) was removed: on one H100 it was
+// 8-11x outside |G - G64| <= 1e-6 |Y|^T|Y| at a million rows (tests/test_gpu_kernel_edges.py).
 #include <limits.h>
 
 #include "cholesky_device.cuh"
@@ -17,120 +17,6 @@ namespace als {
 namespace {
 
 constexpr int kGramRows = 32;  // rows of Y staged per step (FMA version)
-
-__device__ __forceinline__ void cp_async16_zfill(float *smem_dst, const float *gmem_src, bool valid) {
-  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem_dst);
-  const int n = valid ? 16 : 0;  // src-size 0: nothing is read, the 16 bytes are zero-filled
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "r"(n) : "memory");
-}
-
-constexpr int kGramWarps = 8;
-constexpr int kGramStages = 4;
-
-template <int NB>
-__global__ void __launch_bounds__(32 * kGramWarps, 1)
-gramian_mma_kernel(const float *__restrict__ Y, int64_t rows, float *__restrict__ partials) {
-  using C = Cfg<NB>;
-  constexpr int F = C::F, LDS = C::LDS, STAGE = 8 * LDS, NT8 = C::NT8, NTILES = C::NTILES;
-  extern __shared__ __align__(16) unsigned char gram_smem[];
-  float *smem = reinterpret_cast<float *>(gram_smem);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int g = lane >> 2, t = lane & 3;
-  float *ring = smem + warp * kGramStages * STAGE;
-  const int64_t nks = (rows + 7) >> 3;  // 8-row steps
-  const int64_t stride = (int64_t)gridDim.x * kGramWarps;
-
-  float acc[NTILES][4];
-#pragma unroll
-  for (int e = 0; e < NTILES; ++e) acc[e][0] = acc[e][1] = acc[e][2] = acc[e][3] = 0.f;
-
-  auto issue = [&](int64_t ks, int stage) {
-    if (ks < nks) {
-      float *st = ring + stage * STAGE;
-      constexpr int CH = F / 4;
-#pragma unroll
-      for (int q = 0; q < NB; ++q) {
-        const int id = q * 32 + lane, row = id / CH, ch = id % CH;
-        const int64_t r = ks * 8 + row;
-        const bool valid = r < rows;
-        cp_async16_zfill(st + row * LDS + ch * 4, Y + (valid ? r : 0) * F + ch * 4, valid);
-      }
-    }
-    cp_async_commit();
-  };
-
-  int64_t ks = (int64_t)blockIdx.x * kGramWarps + warp;
-  issue(ks, 0);
-  issue(ks + stride, 1);
-  issue(ks + 2 * stride, 2);
-  int stage = 0;
-  for (; ks < nks; ks += stride) {
-    cp_async_wait<2>();
-    __syncwarp();
-    issue(ks + 3 * stride, (stage + 3) & 3);
-    const float *st = ring + stage * STAGE;
-    uint32_t vh0[NT8], vl0[NT8], vh1[NT8], vl1[NT8];
-#pragma unroll
-    for (int c = 0; c < NT8; ++c) {
-      split_tf32(st[t * LDS + 8 * c + g], vh0[c], vl0[c]);
-      split_tf32(st[(t + 4) * LDS + 8 * c + g], vh1[c], vl1[c]);
-    }
-#pragma unroll
-    for (int term = 0; term < 3; ++term) {
-#pragma unroll
-      for (int i = 0; i < NB; ++i) {
-        const uint32_t a0 = term == 0 ? vl0[2 * i] : vh0[2 * i];
-        const uint32_t a1 = term == 0 ? vl0[2 * i + 1] : vh0[2 * i + 1];
-        const uint32_t a2 = term == 0 ? vl1[2 * i] : vh1[2 * i];
-        const uint32_t a3 = term == 0 ? vl1[2 * i + 1] : vh1[2 * i + 1];
-#pragma unroll
-        for (int j = 2 * i; j < NT8; ++j) {
-          float(&d)[4] = acc[C::tidx(i, j)];
-          if (term == 1) mma_tf32(d, a0, a1, a2, a3, vl0[j], vl1[j]);
-          else mma_tf32(d, a0, a1, a2, a3, vh0[j], vh1[j]);
-        }
-      }
-    }
-    stage = (stage + 1) & 3;
-  }
-  cp_async_wait<0>();
-  __syncthreads();
-  // fixed-order tree over the CTA's warps (through the now idle ring), then one partial per CTA
-  constexpr int SLOT = NTILES * 128;
-  for (int half = kGramWarps / 2; half >= 1; half >>= 1) {
-    if (warp >= half && warp < 2 * half) {
-      float *dst = smem + (warp - half) * SLOT;
-#pragma unroll
-      for (int e = 0; e < NTILES; ++e)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) dst[(e * 4 + v) * 32 + lane] = acc[e][v];
-    }
-    __syncthreads();
-    if (warp < half) {
-      const float *src = smem + warp * SLOT;
-#pragma unroll
-      for (int e = 0; e < NTILES; ++e)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) acc[e][v] += src[(e * 4 + v) * 32 + lane];
-    }
-    __syncthreads();
-  }
-  if (warp == 0) {
-    float *out = partials + (size_t)blockIdx.x * F * F;
-#pragma unroll
-    for (int i = 0; i < NB; ++i)
-#pragma unroll
-      for (int j = 2 * i; j < NT8; ++j)
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const int r = 16 * i + g + ((v & 2) ? 8 : 0), c = 8 * j + 2 * t + (v & 1);
-          const float val = acc[C::tidx(i, j)][v];
-          out[r * F + c] = val;
-          if ((r >> 3) < 2 * (c >> 4)) out[c * F + r] = val;  // the mirror position is in no computed tile
-        }
-  }
-}
-
 
 // fp32 FMA version (round-to-nearest accumulation).  Thread (ty, tx) of the 16 x 16 block owns the T x T
 // sub-block of G at rows T ty .. T ty + T - 1, columns T tx .. T tx + T - 1 (T = F / 16), so both of its operands
@@ -275,16 +161,6 @@ static int run_gramian(als_ctx *ctx, const als_factors *Y, int grid) {
   return ALS_OK;
 }
 
-template <int NB>
-static int run_gramian_mma(als_ctx *ctx, const als_factors *Y, int grid) {
-  const int smem = kGramWarps * kGramStages * 8 * Cfg<NB>::LDS * (int)sizeof(float);
-  static_assert(kGramWarps / 2 * Cfg<NB>::NTILES * 128 <= kGramWarps * kGramStages * 8 * Cfg<NB>::LDS, "tree does not fit");
-  auto kern = gramian_mma_kernel<NB>;
-  ALS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  kern<<<grid, 32 * kGramWarps, smem, ctx->stream>>>(Y->d, Y->rows, ctx->gram_partials);
-  return ALS_OK;
-}
-
 }  // namespace
 
 int launch_gramian(als_ctx *ctx, const als_factors *Y) {
@@ -317,16 +193,13 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
     ctx->launches += 2;
     return ALS_OK;
   }
-  // Other widths: the FMA version (round to nearest) is the default; the mma.sync one is kept behind a knob because a
-  // tensor core that truncates while accumulating biases the all-positive diagonal of G.
-  if (F == 64 && Y->rows >= 128 && !ctx->knobs.gramian_mma && !ctx->knobs.gramian_fma) {  // (a TMA box is 128 rows)
+  // Other widths: the FMA version (round to nearest).
+  if (F == 64 && Y->rows >= 128 && !ctx->knobs.gramian_fma) {  // (a TMA box is 128 rows)
     ProfScope prof(ctx, kProfGramian);
     return launch_gramian_tc(ctx, Y);  // wgmma + TMA (dense.cu)
   }
-  const bool mma = F <= 64 && ctx->knobs.gramian_mma;
-  const int64_t steps = mma ? ceil_div(std::max<int64_t>(Y->rows, 1), 8 * kGramWarps)
-                            : ceil_div(std::max<int64_t>(Y->rows, 1), kGramRows);
-  const int grid = (int)std::min<int64_t>(steps, (int64_t)ctx->sm_count * (mma ? 1 : 2));
+  const int64_t steps = ceil_div(std::max<int64_t>(Y->rows, 1), kGramRows);
+  const int grid = (int)std::min<int64_t>(steps, (int64_t)ctx->sm_count * 2);
   const int64_t need = (int64_t)grid * F * F;
   if (need > ctx->gram_partials_cap) {
     if (ctx->gram_partials) {
@@ -341,10 +214,10 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
   ProfScope prof(ctx, kProfGramian);
   int rc = ALS_OK;
   switch (F / 16) {
-    case 1: rc = mma ? run_gramian_mma<1>(ctx, Y, grid) : run_gramian<1>(ctx, Y, grid); break;
-    case 2: rc = mma ? run_gramian_mma<2>(ctx, Y, grid) : run_gramian<2>(ctx, Y, grid); break;
-    case 3: rc = mma ? run_gramian_mma<3>(ctx, Y, grid) : run_gramian<3>(ctx, Y, grid); break;
-    case 4: rc = mma ? run_gramian_mma<4>(ctx, Y, grid) : run_gramian<4>(ctx, Y, grid); break;
+    case 1: rc = run_gramian<1>(ctx, Y, grid); break;
+    case 2: rc = run_gramian<2>(ctx, Y, grid); break;
+    case 3: rc = run_gramian<3>(ctx, Y, grid); break;
+    case 4: rc = run_gramian<4>(ctx, Y, grid); break;
     case 5: run_gramian<5>(ctx, Y, grid); break;
     case 6: run_gramian<6>(ctx, Y, grid); break;
     case 7: run_gramian<7>(ctx, Y, grid); break;

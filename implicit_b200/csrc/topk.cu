@@ -251,7 +251,7 @@ topk_kernel(const float *__restrict__ items, int n_items, const float *__restric
         const int row = warp * C::ROWS_PER_WARP + rr;
         if (q0 + row >= n_query) break;
         float *srow = Ss + row * SLD;
-        if (liked_indptr && Nxt[row] < i0 + IT) {  // topk.pyx:51-53 (row indices sorted ascending by the host)
+        if (liked_indptr && Nxt[row] < i0 + IT) {  // topk.pyx:51-53 (rows in ascending column order: liked_in_order)
           const int end = liked_indptr[q0 + row + 1];
           int cur = Cur[row];
           for (;;) {
@@ -490,6 +490,64 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld, int32_t *ids_host, flo
   return rc;
 }
 
+// ---- liked lists in column order -------------------------------------------------------------------------------
+// Both fused kernels advance a cursor through a row's liked columns as the item tiles go by, so they need every row
+// sorted ascending.  The reference (topk.pyx:51-54) does not care about the order, and neither may the ABI: a CSR
+// is checked once, and one with an unsorted row gets a sorted copy that is kept with it.
+__global__ void __launch_bounds__(256) csr_unsorted_kernel(const int32_t *__restrict__ indptr, int64_t rows,
+                                                           const int32_t *__restrict__ indices, int *flag) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x)
+    for (int p = indptr[r] + 1; p < indptr[r + 1]; ++p)
+      if (indices[p - 1] > indices[p]) {
+        *flag = 1;
+        break;
+      }
+}
+
+__global__ void rebase_indptr_kernel(const int32_t *__restrict__ in, int64_t n, int32_t *__restrict__ out) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = in[i] - in[0];
+}
+
+// (indptr, indices) of `liked` with every row in ascending column order
+int liked_in_order(als_ctx *ctx, const als_csr *liked, const int32_t **indptr, const int32_t **indices) {
+  als_csr *c = const_cast<als_csr *>(liked);  // the check and the sorted copy are caches of the handle
+  if (!c->order_known && c->rows > 0 && c->nnz > 0) {
+    int *flag = nullptr;
+    int rc = dev_alloc(ctx, (void **)&flag, sizeof(int));
+    if (rc != ALS_OK) return rc;
+    ALS_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+    csr_unsorted_kernel<<<(unsigned)std::min<int64_t>(ceil_div(c->rows, 256), (int64_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+        c->indptr, c->rows, c->indices, flag);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    int unsorted = 0, base = 0;
+    ALS_CUDA(cudaMemcpyAsync(&unsorted, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    ALS_CUDA(cudaMemcpyAsync(&base, c->indptr, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    dev_free(ctx, flag);
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (unsorted) {
+      if ((rc = dev_alloc(ctx, (void **)&c->sorted_indptr, (c->rows + 1) * sizeof(int32_t))) != ALS_OK) return rc;
+      if ((rc = dev_alloc(ctx, (void **)&c->sorted_indices, c->nnz * sizeof(int32_t))) != ALS_OK) return rc;
+      rebase_indptr_kernel<<<(unsigned)ceil_div(c->rows + 1, 256), 256, 0, ctx->stream>>>(c->indptr, c->rows + 1, c->sorted_indptr);
+      ALS_CUDA(cudaGetLastError());
+      void *tmp = nullptr;
+      size_t tmp_bytes = 0;
+      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, c->indices + base, c->sorted_indices, (int)c->nnz,
+                                                       (int)c->rows, c->sorted_indptr, c->sorted_indptr + 1, 0, 32, ctx->stream));
+      if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(tmp, tmp_bytes, c->indices + base, c->sorted_indices, (int)c->nnz,
+                                                       (int)c->rows, c->sorted_indptr, c->sorted_indptr + 1, 0, 32, ctx->stream));
+      dev_free(ctx, tmp);
+      ctx->launches += 2;
+    }
+    c->order_known = true;
+  }
+  *indptr = c->sorted_indptr ? c->sorted_indptr : c->indptr;
+  *indices = c->sorted_indptr ? c->sorted_indices : c->indices;
+  return ALS_OK;
+}
+
 template <int F>
 int run_topk_f(als_ctx *ctx, const TopkArgs &a) {
   if (a.k <= 64) return run_topk<F, 4>(ctx, a);
@@ -572,8 +630,9 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
   a.k_out = k;
   a.norms = item_norms_host ? (const float *)(base + o_nrm) : nullptr;
   a.mask = n_filter ? (const uint8_t *)(base + o_mask) : nullptr;
-  a.liked_indptr = liked ? liked->indptr : nullptr;
-  a.liked_indices = liked ? liked->indices : nullptr;
+  a.liked_indptr = nullptr;
+  a.liked_indices = nullptr;
+  if (liked && (rc = liked_in_order(ctx, liked, &a.liked_indptr, &a.liked_indices)) != ALS_OK) return rc;
   a.ids = (int32_t *)(base + o_ids);
   a.scores = (float *)(base + o_sc);
 #define CALL(FF) run_topk_f<FF>(ctx, a)

@@ -3,8 +3,9 @@
 //
 // The score matrix  S = Q I^T  is the one large dense contraction of the hot path (C5: 1M x 1M x 64).  Here it runs
 // on wgmma with TMA-fed operands; the selection is the epilogue, so a score never leaves the SM:
-//   pre-pass   both factor matrices are split ONCE per call into fp16 hi / lo halves (x 2^e, e from the matrix's
-//              absolute maximum, so the halves carry 22 bits): scores = (Qh + Ql)(Ih + Il)^T ~ Ql Ih^T + Qh Il^T + Qh Ih^T,
+//   pre-pass   both factor matrices are split ONCE per call into fp16 hi / lo halves (x 2^e, e from each query row's
+//              own absolute maximum and from the item matrix's, so the halves carry 22 bits however small a query row
+//              is next to the others): scores = (Qh + Ql)(Ih + Il)^T ~ Ql Ih^T + Qh Il^T + Qh Ih^T,
 //              fp32-faithful like the 3xTF32 split of topk.cu at half the tensor work and half the operand bytes;
 //   CTA        2 x 128 query rows (hi and lo tiles resident in shared memory, K-major, 128B swizzle) sweep ALL items;
 //              every landed item tile is multiplied with BOTH query tiles (half the L2 -> SM operand traffic of one
@@ -83,17 +84,43 @@ __device__ __forceinline__ int scale_exp_field(unsigned absmax_bits) {
   return se < 1 ? 1 : se > 253 ? 253 : se;
 }
 
+// Splits rows of x into fp16 hi / lo halves.  absmax != nullptr: one scale for the whole matrix (the items: a score
+// is compared only with the scores of the same query, so the item side may share one exponent).  absmax == nullptr:
+// one scale per row, taken from that row's own absolute maximum and written to row_exp (the queries: a row far below
+// the matrix maximum would otherwise lose its low bits in fp16 subnormals).
 __global__ void __launch_bounds__(256) tk_split_kernel(const float *__restrict__ x, int ld, const int32_t *__restrict__ rows,
                                                        int64_t n_rows, const unsigned *__restrict__ absmax,
-                                                       uint4 *__restrict__ hi, uint4 *__restrict__ lo) {
-  const float scale = __uint_as_float((unsigned)scale_exp_field(*absmax) << 23);
-  const int64_t n = n_rows * (kTkF / 8);  // 8 values -> one 16-byte chunk of halves
-  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+                                                       int *__restrict__ row_exp, uint4 *__restrict__ hi,
+                                                       uint4 *__restrict__ lo) {
+  const float mscale = absmax ? __uint_as_float((unsigned)scale_exp_field(*absmax) << 23) : 1.f;
+  const int64_t n = n_rows * (kTkF / 8);  // 8 values -> one 16-byte chunk of halves; 8 consecutive lanes hold a row
+  const int64_t n_pad = (n + 31) & ~(int64_t)31;  // whole warps stay in the loop for the per-row shuffles
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n_pad; e += (int64_t)gridDim.x * blockDim.x) {
+    const bool in = e < n;
     const int64_t r = e / (kTkF / 8);
     const int c = (int)(e % (kTkF / 8));
-    const int64_t s = rows ? rows[r] : r;
-    const float4 a = __ldg(reinterpret_cast<const float4 *>(x + s * ld) + 2 * c);
-    const float4 b = __ldg(reinterpret_cast<const float4 *>(x + s * ld) + 2 * c + 1);
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+    if (in) {
+      const int64_t s = rows ? rows[r] : r;
+      a = __ldg(reinterpret_cast<const float4 *>(x + s * ld) + 2 * c);
+      b = __ldg(reinterpret_cast<const float4 *>(x + s * ld) + 2 * c + 1);
+    }
+    float scale = mscale;
+    if (!absmax) {
+      const float u[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+      unsigned m = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const unsigned bits = __float_as_uint(u[j]) & 0x7fffffffu;
+        if (bits < 0x7f800000u) m = max(m, bits);  // NaN / inf cannot be scaled (as in tk_absmax_kernel)
+      }
+#pragma unroll
+      for (int o = 4; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+      const int se = scale_exp_field(m);
+      scale = __uint_as_float((unsigned)se << 23);
+      if (in && c == 0) row_exp[r] = se;
+    }
+    if (!in) continue;
     const float v[8] = {a.x * scale, a.y * scale, a.z * scale, a.w * scale, b.x * scale, b.y * scale, b.z * scale, b.w * scale};
     uint32_t h[4], l[4];
 #pragma unroll
@@ -116,7 +143,7 @@ template <int KMAX>
 __global__ void __launch_bounds__(kTkThreads, 1)
 topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant__ CUtensorMap map_ql,
                const __grid_constant__ CUtensorMap map_ih, const __grid_constant__ CUtensorMap map_il, int n_items,
-               int n_query, int k, const unsigned *__restrict__ absmax_q, const unsigned *__restrict__ absmax_i,
+               int n_query, int k, const int *__restrict__ q_exp, const unsigned *__restrict__ absmax_i,
                const uint8_t *__restrict__ item_mask, const int32_t *__restrict__ liked_indptr,
                const int32_t *__restrict__ liked_indices, int32_t *__restrict__ out_ids, float *__restrict__ out_scores) {
   extern __shared__ unsigned char tk_smem_raw[];
@@ -181,7 +208,7 @@ topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   }
   auto consider = [&](float s, int id) {
     if (id >= n_items) return;
-    while (lnext < id) {  // both the candidates and the liked list come in increasing item order
+    while (lnext < id) {  // both the candidates and the liked list come in increasing item order (liked_in_order)
       ++lp;
       lnext = lp < lend ? liked_indices[lp] : INT_MAX;
     }
@@ -254,8 +281,8 @@ topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
     scan(my_row + 32, t * kTkI + 32);
   }
   if (live) {
-    // scores leave the scaled domain: exact multiplications by powers of two
-    const float inv_q = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_q)) << 23);
+    // scores leave the scaled domain: exact multiplications by powers of two (this query row's own, the items')
+    const float inv_q = __uint_as_float((unsigned)(254 - q_exp[q]) << 23);
     const float inv_i = __uint_as_float((unsigned)(254 - scale_exp_field(*absmax_i)) << 23);
 #pragma unroll
     for (int j = 0; j < KMAX; ++j)
@@ -298,7 +325,7 @@ int make_half_map(CUtensorMap *m, const void *ptr, int64_t rows, int box_rows) {
 
 // bytes of device scratch launch_topk_tc needs for `n_query` queries against `n_items` items
 int64_t topk_tc_scratch_bytes(int64_t n_query, int64_t n_items) {
-  return 256 + 2 * ((n_query * 128 + 255) / 256 * 256) + 2 * ((n_items * 128 + 255) / 256 * 256);
+  return 256 + (n_query * 4 + 255) / 256 * 256 + 2 * ((n_query * 128 + 255) / 256 * 256) + 2 * ((n_items * 128 + 255) / 256 * 256);
 }
 
 bool topk_tc_eligible(int ld, int64_t n_query, int64_t n_items, int k, bool has_norms) {
@@ -310,18 +337,19 @@ int launch_topk_tc(als_ctx *ctx, const float *items, int64_t n_items, const floa
                    int64_t n_query, int k, const uint8_t *mask, const int32_t *liked_indptr, const int32_t *liked_indices,
                    int32_t *out_ids, float *out_scores, void *scratch) {
   char *p = (char *)scratch;
-  unsigned *absmax = (unsigned *)p;  // [0] queries, [1] items
+  unsigned *absmax = (unsigned *)p;  // the items' absolute maximum
   p += 256;
+  int *q_exp = (int *)p;             // per query row: the exponent field of its scale
+  p += (n_query * 4 + 255) / 256 * 256;
   const int64_t qbytes = (n_query * 128 + 255) / 256 * 256, ibytes = (n_items * 128 + 255) / 256 * 256;
   void *qh = p, *ql = p + qbytes, *ih = p + 2 * qbytes, *il = p + 2 * qbytes + ibytes;
-  ALS_CUDA(cudaMemsetAsync(absmax, 0, 8, ctx->stream));
+  ALS_CUDA(cudaMemsetAsync(absmax, 0, 4, ctx->stream));
   const int g = ctx->sm_count * 8;
-  tk_absmax_kernel<<<g, 256, 0, ctx->stream>>>(queries, kTkF, query_rows, n_query, absmax);
-  tk_absmax_kernel<<<g, 256, 0, ctx->stream>>>(items, kTkF, nullptr, n_items, absmax + 1);
-  tk_split_kernel<<<g, 256, 0, ctx->stream>>>(queries, kTkF, query_rows, n_query, absmax, (uint4 *)qh, (uint4 *)ql);
-  tk_split_kernel<<<g, 256, 0, ctx->stream>>>(items, kTkF, nullptr, n_items, absmax + 1, (uint4 *)ih, (uint4 *)il);
+  tk_absmax_kernel<<<g, 256, 0, ctx->stream>>>(items, kTkF, nullptr, n_items, absmax);
+  tk_split_kernel<<<g, 256, 0, ctx->stream>>>(queries, kTkF, query_rows, n_query, nullptr, q_exp, (uint4 *)qh, (uint4 *)ql);
+  tk_split_kernel<<<g, 256, 0, ctx->stream>>>(items, kTkF, nullptr, n_items, absmax, nullptr, (uint4 *)ih, (uint4 *)il);
   ALS_CUDA(cudaGetLastError());
-  ctx->launches += 4;
+  ctx->launches += 3;
   CUtensorMap mqh, mql, mih, mil;
   int rc;
   if ((rc = make_half_map(&mqh, qh, n_query, kTkQ)) != ALS_OK) return rc;
@@ -333,7 +361,7 @@ int launch_topk_tc(als_ctx *ctx, const float *items, int64_t n_items, const floa
   const int grid = (int)ceil_div(n_query, kTkQ * kTkG);
   {
     ProfScope prof(ctx, kProfTopk);
-    kern<<<grid, kTkThreads, kTkSmem, ctx->stream>>>(mqh, mql, mih, mil, (int)n_items, (int)n_query, k, absmax, absmax + 1, mask,
+    kern<<<grid, kTkThreads, kTkSmem, ctx->stream>>>(mqh, mql, mih, mil, (int)n_items, (int)n_query, k, q_exp, absmax, mask,
                                                      liked_indptr, liked_indices, out_ids, out_scores);
   }
   ALS_CUDA(cudaGetLastError());

@@ -57,7 +57,7 @@ int als_device_count(void);
 int als_ctx_create(int device, als_ctx **out);
 int als_ctx_destroy(als_ctx *ctx);
 
-/* Measurement knobs ("short_max" 0/16/32/48, "short_serial", "whiten_fma", "gramian_mma", "gramian_fma", "topk_legacy", "cg_nv" 1/2/4).  The
+/* Measurement knobs ("short_max" 0/16/32/48, "short_serial", "whiten_fma", "gramian_fma", "topk_legacy", "cg_nv" 1/2/4).  The
  * environment variables ALS_B200_<KNOB> are read once, in als_ctx_create, and reported on stderr when set; this
  * call changes a knob afterwards (A/B tools).  Results do not depend on any knob beyond fp32 rounding.
  * (No reference equivalent.) */
@@ -187,6 +187,9 @@ int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors *X, con
  * filter_items set to -FLT_MAX first.  Queries are rows `query_rows[0..n_query)` of `queries`
  * (query_rows NULL = rows 0..n_query-1).  Outputs are host arrays [n_query, k], zero-initialised
  * by the callee like topk.pyx:20-21; tie-breaking follows implicit/cpu/select.h:12-39 exactly.
+ * `liked` has n_query rows; its columns may come in any order within a row and may repeat (like the reference's
+ * batch_distances[i, liked.indices] = -max).  The first call with a given `liked` checks the order on the device;
+ * if a row is unsorted, a sorted copy is built once and kept with the handle (its nnz int32s) until it is destroyed.
  * Replaces topk.topk(items, query, k, item_norms, filter_query_items, filter_items, num_threads),
  * implicit/cpu/topk.pyx:15-67, and KnnQuery::topk (implicit/gpu/knn.cu:131-265). */
 int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,

@@ -32,6 +32,46 @@ def row_err(a, b):
     return num / np.maximum(np.maximum(den, floor), 1e-30)
 
 
+def cholesky_truth(Cui, Y, reg, YtY=None):
+    """The Cholesky half in fp64: for every row u, x_u = (G + reg I + Y_u^T diag(|c| - 1) Y_u)^-1 Y_u^T c+ with
+    G = YtY (the caller's, cast to fp64) or the fp64 Y^T Y.  Every stored entry counts like _als.pyx:96-130: an
+    explicit zero subtracts y y^T, duplicates are not merged.  Empty rows are zero (_als.pyx:98-100)."""
+    Y64 = np.asarray(Y, dtype=np.float64)
+    f = Y64.shape[1]
+    G = Y64.T @ Y64 if YtY is None else np.asarray(YtY, dtype=np.float64)
+    G = G + reg * np.eye(f)
+    lens = np.diff(Cui.indptr)
+    rows = np.nonzero(lens)[0]
+    A = np.empty((len(rows), f, f))
+    b = np.empty((len(rows), f))
+    for n, u in enumerate(rows):
+        s, e = Cui.indptr[u], Cui.indptr[u + 1]
+        Yu, c = Y64[Cui.indices[s:e]], np.asarray(Cui.data[s:e], dtype=np.float64)
+        A[n] = G + (Yu.T * (np.abs(c) - 1.0)) @ Yu
+        b[n] = Yu.T @ np.maximum(c, 0.0)
+    X = np.zeros((Cui.shape[0], f))
+    if len(rows):
+        X[rows] = np.linalg.solve(A, b[:, :, None])[:, :, 0]
+    return X
+
+
+def topk_noise(queries, items):
+    """Per-row fp32 summation noise of a score q . i: 4 eps |q| max_i |i|, as an (n, 1) column.  The query side is
+    per row (a kernel must hold its accuracy however small a query is next to the others); the item side is the
+    largest item, because every item of a row competes for the same k slots."""
+    q = np.linalg.norm(np.asarray(queries, dtype=np.float64), axis=1)[:, None]
+    return 4 * np.finfo(np.float32).eps * q * np.linalg.norm(np.asarray(items, dtype=np.float64), axis=1).max()
+
+
+def topk_mismatches(ids, scores, ref_ids, ref_scores, noise):
+    """Near-tie classification of two top-k results (SURVEY.md section 8(d)): where the ids at a rank differ, the
+    two scores at that rank must agree within `noise` (a scalar or an (n, 1) column from topk_noise).
+    Returns (same, bad): the boolean arrays of equal ids and of true mismatches."""
+    same = ids == ref_ids
+    bad = (~same) & (np.abs(np.asarray(scores, np.float64) - np.asarray(ref_scores, np.float64)) > noise)
+    return same, bad
+
+
 def golden_cases():
     """The fit fixtures (chol_*, cg_*); eval_metrics.npz belongs to tests/test_evaluation.py."""
     return sorted(f[:-4] for f in os.listdir(GOLDEN) if f.endswith(".npz") and f.startswith(("chol_", "cg_")))

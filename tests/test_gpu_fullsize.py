@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 import oracle
-from helpers import CG_CONVERGED_MAX, CG_MEDIAN, CG_P99, CHOL_MAX, row_err
+from helpers import CG_CONVERGED_MAX, CG_MEDIAN, CG_P99, CHOL_MAX, row_err, topk_mismatches, topk_noise
 from implicit_b200 import synthetic
 
 pytestmark = pytest.mark.gpu
@@ -200,10 +200,8 @@ def test_c5_sampled_queries_match_oracle_topk(lib, ctx, orc):
     for h in (dl, dq, di):
         h.close()
     eids, esc = orc.topk(items, users[rows], k, filter_query_items=liked)
-    same = ids == eids
     # near-tie classification: where the ids differ, the scores at that rank must agree within summation noise
-    noise = 4 * np.finfo(np.float32).eps * np.linalg.norm(users[rows], axis=1)[:, None] * np.linalg.norm(items, axis=1).max()
-    bad = (~same) & (np.abs(sc - esc) > noise)
+    same, bad = topk_mismatches(ids, sc, eids, esc, topk_noise(users[rows], items))
     print(f"C5 sample: {nq} queries x {I} items, ids equal {same.mean():.6f}, near-tie swaps {(~same).sum() - bad.sum()}, "
           f"true mismatches {bad.sum()}; score rel err max {np.abs(sc - esc).max() / np.abs(esc).max():.2e}")
     assert bad.sum() == 0
@@ -258,9 +256,7 @@ def test_topk_tcgen05_path_matches_oracle_and_legacy_kernel(lib, ctx, orc, k):
     for h in (dl2, dl, dq, di):
         h.close()
     eids, esc = orc.topk(items, users, k, filter_query_items=liked, filter_items=flt)
-    same = ids == eids
-    noise = 4 * np.finfo(np.float32).eps * np.linalg.norm(users, axis=1)[:, None] * np.linalg.norm(items, axis=1).max()
-    bad = (~same) & (np.abs(sc - esc) > noise)
+    same, bad = topk_mismatches(ids, sc, eids, esc, topk_noise(users, items))
     print(f"wgmma top-k k={k}: ids equal to the reference {same.mean():.6f} (true mismatches {bad.sum()}), to the mma.sync kernel "
           f"{(ids == ids_old).mean():.6f}; score rel err {np.abs(sc - esc).max() / np.abs(esc).max():.2e}")
     assert bad.sum() == 0 and same.mean() > 0.999

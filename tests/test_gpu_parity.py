@@ -6,7 +6,7 @@ import pytest
 import scipy.sparse as sp
 
 import oracle
-from helpers import CHOL_MAX, golden_cases, load_golden, row_err
+from helpers import CHOL_MAX, cholesky_truth, golden_cases, load_golden, row_err
 from implicit_b200 import synthetic
 
 pytestmark = pytest.mark.gpu
@@ -387,15 +387,7 @@ def test_c2_full_size_sampled_rows_match_oracle(lib, ctx, orc):
     # (3) ground truth in fp64 for the sampled rows: at this cold start the normal equations have condition
     #     number ~2e2 (Y^T Y of all-positive factors is rank-1 dominated), so fp32 LAPACK itself is ~1e-4 off
     #     on the worst rows; the GPU result must be no further from the truth than the reference is.
-    Y64 = Y0.astype(np.float64)
-    truth = np.zeros((len(sample), 64))
-    for n, u in enumerate(sample):
-        s, t = Cui.indptr[u], Cui.indptr[u + 1]
-        if s == t:
-            continue
-        Yu, c = Y64[Cui.indices[s:t]], Cui.data[s:t].astype(np.float64)
-        A = G64 + 0.01 * np.eye(64) + (Yu.T * (np.abs(c) - 1.0)) @ Yu
-        truth[n] = np.linalg.solve(A, Yu.T @ np.where(c > 0, c, 0.0))
+    truth = cholesky_truth(sub, Y0, 0.01, YtY=G64)
     e_gpu_truth, e_ref_truth = row_err(got[sample], truth), row_err(exp, truth)
     print(f"vs fp64 truth: gpu max {e_gpu_truth.max():.2e} median {np.median(e_gpu_truth):.2e}; "
           f"reference max {e_ref_truth.max():.2e} median {np.median(e_ref_truth):.2e}")

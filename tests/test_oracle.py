@@ -11,7 +11,7 @@ import pytest
 from scipy.sparse import csr_matrix
 
 import oracle
-from helpers import CHOL_MAX, GOLDEN, golden_cases, load_golden, row_err
+from helpers import CHOL_MAX, GOLDEN, cholesky_truth, golden_cases, load_golden, row_err
 
 sys.path.insert(0, GOLDEN)
 import make_golden_ref  # noqa: E402
@@ -59,6 +59,41 @@ def test_port_loss_and_topk_match_golden(name):
     diff = ids != z["topk_ids"]
     if diff.any():
         assert np.abs(scores[diff] - z["topk_scores"][diff]).max() < 1e-6
+
+
+@pytest.mark.parametrize("name", [n for n in golden_cases() if n.startswith("chol")])
+def test_cholesky_truth_matches_golden_half(name):
+    """tests/helpers.cholesky_truth, the fp64 yardstick of the GPU kernel tests, against the reference's own fp32 half
+    (golden Xh) from the stored warm state, with its own fp64 Gramian and with a caller-supplied one (_least_squares)."""
+    rc, Cui, _, _, z = load_golden(name)
+    Y = z["Y"]
+    truth = cholesky_truth(Cui, Y, 0.01)
+    e = row_err(z["Xh"], truth)
+    YtY = (Y.astype(np.float64).T @ Y.astype(np.float64) * 0.5).astype(np.float32)  # any SPD Gramian will do
+    got = np.zeros_like(z["X"])
+    PORT._least_squares(YtY, Cui.indptr, Cui.indices, Cui.data.astype(np.float32), got, Y, 0.01)
+    e_g = row_err(got, cholesky_truth(Cui, Y, 0.01, YtY=YtY))
+    print(f"{name}: fp32 reference vs cholesky_truth max {e.max():.2e}; with a supplied Gramian max {e_g.max():.2e}")
+    assert e.max() < 1e-5 and e_g.max() < 1e-5
+
+
+def test_cholesky_truth_counts_zeros_duplicates_and_negatives():
+    """Stored zeros subtract y y^T, duplicates are not merged, negative confidences weigh |c| - 1 with no right-hand
+    side, empty rows are zero: the same as the oracle's fp32 solve of _als.pyx:96-130."""
+    rng = np.random.default_rng(12)
+    indptr = np.array([0, 5, 9, 9, 12], dtype=np.int32)
+    indices = np.array([1, 1, 3, 7, 2, 0, 4, 4, 6, 5, 2, 5], dtype=np.int32)
+    data = np.array([2.0, 3.0, 0.0, -1.5, 1.0, 4.0, 0.0, 2.5, -0.5, 3.0, 0.5, 3.0], dtype=np.float32)
+    Cui = csr_matrix((data, indices, indptr), shape=(4, 8))
+    Y = (rng.standard_normal((8, 16)) * 0.4).astype(np.float32)
+    exp = np.zeros((4, 16), dtype=np.float32)
+    PORT.least_squares(Cui, exp, Y, 0.5)
+    truth = cholesky_truth(Cui, Y, 0.5)
+    assert np.all(truth[2] == 0)
+    assert row_err(exp, truth).max() < 1e-5
+    merged = Cui.copy()
+    merged.sum_duplicates()
+    assert row_err(cholesky_truth(merged, Y, 0.5), truth).max() > 1e-3  # merging duplicates is a different problem
 
 
 @pytest.mark.parametrize("use_cg", [False, True])

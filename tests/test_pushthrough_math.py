@@ -10,7 +10,7 @@ import pytest
 import scipy.linalg as sl
 
 import oracle
-from helpers import row_err
+from helpers import cholesky_truth, row_err
 from implicit_b200 import synthetic
 
 
@@ -50,15 +50,7 @@ def test_pushthrough_matches_reference_solve(warm, neg):
     orc.least_squares(Cui, exp, Y, 0.01)
     got = pushthrough_rows_fp32(Cui, Y, 0.01)
     # fp64 truth, to show the two fp32 routes are equally far from it
-    Y64 = Y.astype(np.float64)
-    G64 = Y64.T @ Y64 + 0.01 * np.eye(64)
-    truth = np.zeros_like(exp, dtype=np.float64)
-    for u in range(Cui.shape[0]):
-        s, e = Cui.indptr[u], Cui.indptr[u + 1]
-        if s == e:
-            continue
-        Yu, c = Y64[Cui.indices[s:e]], Cui.data[s:e].astype(np.float64)
-        truth[u] = np.linalg.solve(G64 + (Yu.T * (np.abs(c) - 1)) @ Yu, Yu.T @ np.where(c > 0, c, 0))
+    truth = cholesky_truth(Cui, Y, 0.01)
     e_ref, e_new = row_err(exp, truth), row_err(got, truth)
     print(f"warm={warm} neg={neg}: reference vs fp64 max {e_ref.max():.2e}; push-through vs fp64 max {e_new.max():.2e}; "
           f"push-through vs reference max {row_err(got, exp).max():.2e}")
