@@ -194,12 +194,15 @@ __device__ __forceinline__ void split_f16_pair(float x0, float x1, uint32_t &hi,
   lo = *reinterpret_cast<const uint32_t *>(&l);
 }
 
-// biased exponent field of the power of two that scales a positive maximum p to just below 2^14 (see topk_tc.cu)
+// the power of two sigma that scales a positive maximum p to just below 2^14 (see topk_tc.cu).  Its exponent is clamped
+// to [-63, 63] so that sigma^2 and 1 / sigma^2 stay normal fp32 numbers (the kernels multiply by both): sigma is exact
+// for p in [2^-50, 2^77); a smaller p leaves the operands below 2^14 (p < 2^-50: factors of order 1e-16), a larger one
+// is past any Gramian that fits in fp32.
 __device__ __forceinline__ float pow2_scale_below_2_14(float p) {
   const unsigned b = __float_as_uint(p);
   const int E = (int)(b >> 23) & 0xff;
   int se = (b & 0x7fffffffu) ? 267 - E : 127;
-  se = se < 1 ? 1 : se > 253 ? 253 : se;
+  se = se < 127 - 63 ? 127 - 63 : se > 127 + 63 ? 127 + 63 : se;
   return __uint_as_float((unsigned)se << 23);
 }
 

@@ -3,8 +3,10 @@ import os
 import sys
 
 import numpy as np
+import pytest
+import scipy.sparse as sp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+ROOT =os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
@@ -41,18 +43,129 @@ def cholesky_truth(Cui, Y, reg, YtY=None):
     G = Y64.T @ Y64 if YtY is None else np.asarray(YtY, dtype=np.float64)
     G = G + reg * np.eye(f)
     lens = np.diff(Cui.indptr)
-    rows = np.nonzero(lens)[0]
-    A = np.empty((len(rows), f, f))
-    b = np.empty((len(rows), f))
-    for n, u in enumerate(rows):
-        s, e = Cui.indptr[u], Cui.indptr[u + 1]
-        Yu, c = Y64[Cui.indices[s:e]], np.asarray(Cui.data[s:e], dtype=np.float64)
-        A[n] = G + (Yu.T * (np.abs(c) - 1.0)) @ Yu
-        b[n] = Yu.T @ np.maximum(c, 0.0)
     X = np.zeros((Cui.shape[0], f))
-    if len(rows):
+    nonempty = np.nonzero(lens)[0]
+    for r0 in range(0, len(nonempty), 1024):  # blocks of rows: A stays small at 128 factors and many rows
+        rows = nonempty[r0:r0 + 1024]
+        A = np.empty((len(rows), f, f))
+        b = np.empty((len(rows), f))
+        for n, u in enumerate(rows):
+            s, e = Cui.indptr[u], Cui.indptr[u + 1]
+            Yu, c = Y64[Cui.indices[s:e]], np.asarray(Cui.data[s:e], dtype=np.float64)
+            A[n] = G + (Yu.T * (np.abs(c) - 1.0)) @ Yu
+            b[n] = Yu.T @ np.maximum(c, 0.0)
         X[rows] = np.linalg.solve(A, b[:, :, None])[:, :, 0]
     return X
+
+
+#: every knob of als_ctx_set_knob and its default (include/als_b200.h, csrc/common.h)
+KNOB_DEFAULTS = dict(short_max=48, short_serial=0, whiten_fma=0, gramian_fma=0, topk_legacy=0,
+                     long_tc=0, cg_nv=2)
+
+
+# ----------------------------------------------------------------------------- fixtures of the kernel-path modules
+# A GPU module that compares kernel paths imports these by name: one context per module, every knob at its default
+# before and after each test, and a failure at once when a knob is set in the environment.
+@pytest.fixture(scope="module")
+def lib():
+    set_in_env = sorted(f"ALS_B200_{k.upper()}" for k in KNOB_DEFAULTS if f"ALS_B200_{k.upper()}" in os.environ)
+    if set_in_env:  # a "default path" test would silently run another path
+        pytest.fail(f"knob environment variables are set: {', '.join(set_in_env)}; unset them to run these tests")
+    from implicit_b200 import _lib
+
+    return _lib
+
+
+@pytest.fixture(scope="module")
+def ctx(lib):
+    c = lib.Context(0)
+    yield c
+    c.close()
+
+
+@pytest.fixture(autouse=True)
+def default_knobs(ctx):
+    """Every test starts and ends with every knob at its default."""
+    for k, v in KNOB_DEFAULTS.items():
+        ctx.set_knob(k, v)
+    yield
+    for k, v in KNOB_DEFAULTS.items():
+        ctx.set_knob(k, v)
+
+
+@pytest.fixture(scope="module")
+def orc():
+    import oracle
+
+    return oracle.get("auto")
+
+
+@pytest.fixture(scope="module")
+def sm(ctx):
+    return ctx.info()["sm_count"]
+
+
+def factors_of(kind, rows, f, seed):
+    rng = np.random.default_rng(seed)
+    if kind == "mixed":
+        return rng.standard_normal((rows, f), dtype=np.float32)
+    if kind == "cold":  # the all-positive initialisation (implicit/cpu/als.py:144-147)
+        return rng.random((rows, f), dtype=np.float32) * np.float32(0.01)
+    if kind == "decades":  # row norms spread over six decades
+        Y = rng.standard_normal((rows, f), dtype=np.float32)
+        return (Y * (10.0 ** rng.uniform(-6, 0, size=(rows, 1)))).astype(np.float32)
+    if kind == "zero_rows":
+        Y = rng.standard_normal((rows, f), dtype=np.float32)
+        Y[rng.random(rows) < 0.3] = 0
+        Y[-1] = 0
+        return Y
+    raise ValueError(kind)
+
+
+def worst_ratio(err, bar):
+    """max(err / bar); entries with bar == 0 must have err == 0."""
+    err, bar = np.asarray(err, np.float64), np.asarray(bar, np.float64)
+    if np.any((bar == 0) & (err != 0)):
+        return np.inf
+    return float(np.max(np.where(bar > 0, err / np.where(bar > 0, bar, 1), 0.0), initial=0.0))
+
+
+def mixed_csr(users, items, seed, giants=(3073, 3500, 4100), duplicates=False):
+    """Rows at every short-row class boundary, giant rows past the split threshold (> 3072; rows 3, 50, 97, ...
+    get the lengths `giants`, sampled with repeats where a length exceeds `items`), negative confidences, weights
+    |c| - 1 below zero and stored zeros.  duplicates=True repeats the first column of every ninth row at its end."""
+    rng = np.random.default_rng(seed)
+    lengths = [0, 1, 8, 9, 15, 16, 17, 24, 25, 31, 32, 33, 40, 41, 47, 48, 49, 64, 65, 200]
+    lens = [lengths[u % len(lengths)] for u in range(users)]
+    for i, n in enumerate(giants):
+        lens[3 + 47 * i] = n
+    rows, cols, vals = [], [], []
+    for u, n in enumerate(lens):
+        c = rng.choice(items, n, replace=n > items)
+        v = 1 + 4 * rng.random(n)
+        kind = u % 9
+        if n and kind == 1:
+            v[0] = 0.5      # weight below zero
+        elif n and kind == 2:
+            v[0] = 0.0      # stored zero
+        elif n and kind == 3:
+            v[: n // 2 + 1] *= -1
+        elif n and kind == 4:
+            v[0] = -0.25
+        rows += [u] * n
+        cols += c.tolist()
+        vals += v.tolist()
+    if not duplicates:
+        Cui = sp.csr_matrix((np.array(vals, dtype=np.float32), (rows, cols)), shape=(users, items))
+    else:  # built from indptr so that nothing merges the repeats
+        indptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+        for u in range(5, users, 9):
+            if lens[u] >= 2:
+                cols[indptr[u + 1] - 1] = cols[indptr[u]]
+        Cui = sp.csr_matrix((np.array(vals, dtype=np.float32), np.array(cols, dtype=np.int32), indptr),
+                            shape=(users, items))
+    assert (Cui.data == 0).sum() > 0
+    return Cui
 
 
 def topk_noise(queries, items):

@@ -5,58 +5,17 @@ a plain fp64 computation of the same operation.  Shapes come from the device's S
 two and three-plus tiles, ragged last tiles and ring wrap-arounds.  Each bar is an error model stated next to it, and
 the measured worst ratio (error / bar) is printed beside it.
 """
-import os
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 
 import oracle
-from helpers import CG_MEDIAN, cholesky_truth, row_err, topk_mismatches, topk_noise
+from helpers import (CG_MEDIAN, KNOB_DEFAULTS, cholesky_truth, factors_of, mixed_csr, row_err, topk_mismatches,
+                     topk_noise, worst_ratio)
+from helpers import ctx, default_knobs, lib, orc, sm  # noqa: F401  (fixtures)
 from implicit_b200 import synthetic
 
 pytestmark = pytest.mark.gpu
-
-#: every knob of als_ctx_set_knob and its default (include/als_b200.h, csrc/common.h)
-KNOB_DEFAULTS = dict(short_max=48, short_serial=0, whiten_fma=0, gramian_fma=0, topk_legacy=0,
-                     long_tc=0, cg_nv=2)
-
-
-@pytest.fixture(scope="module")
-def lib():
-    set_in_env = sorted(f"ALS_B200_{k.upper()}" for k in KNOB_DEFAULTS if f"ALS_B200_{k.upper()}" in os.environ)
-    if set_in_env:  # a "default path" test would silently run another path
-        pytest.fail(f"knob environment variables are set: {', '.join(set_in_env)}; unset them to run these tests")
-    from implicit_b200 import _lib
-
-    return _lib
-
-
-@pytest.fixture(scope="module")
-def ctx(lib):
-    c = lib.Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(autouse=True)
-def default_knobs(ctx):
-    """Every test starts and ends with every knob at its default."""
-    for k, v in KNOB_DEFAULTS.items():
-        ctx.set_knob(k, v)
-    yield
-    for k, v in KNOB_DEFAULTS.items():
-        ctx.set_knob(k, v)
-
-
-@pytest.fixture(scope="module")
-def orc():
-    return oracle.get("auto")
-
-
-@pytest.fixture(scope="module")
-def sm(ctx):
-    return ctx.info()["sm_count"]
 
 
 def row_counts(sm):
@@ -64,43 +23,18 @@ def row_counts(sm):
     return [1, 127, 128, 129, 128 * sm, 128 * (2 * sm + 1) + 37, (1 << 20) + 5]
 
 
-def factors_of(kind, rows, f, seed):
-    rng = np.random.default_rng(seed)
-    if kind == "mixed":
-        return rng.standard_normal((rows, f), dtype=np.float32)
-    if kind == "cold":  # the all-positive initialisation (implicit/cpu/als.py:144-147)
-        return rng.random((rows, f), dtype=np.float32) * np.float32(0.01)
-    if kind == "decades":  # row norms spread over six decades
-        Y = rng.standard_normal((rows, f), dtype=np.float32)
-        return (Y * (10.0 ** rng.uniform(-6, 0, size=(rows, 1)))).astype(np.float32)
-    if kind == "zero_rows":
-        Y = rng.standard_normal((rows, f), dtype=np.float32)
-        Y[rng.random(rows) < 0.3] = 0
-        Y[-1] = 0
-        return Y
-    raise ValueError(kind)
-
-
 KINDS = ["mixed", "cold", "decades", "zero_rows"]
-
-
-def worst_ratio(err, bar):
-    """max(err / bar); entries with bar == 0 must have err == 0."""
-    err, bar = np.asarray(err, np.float64), np.asarray(bar, np.float64)
-    if np.any((bar == 0) & (err != 0)):
-        return np.inf
-    return float(np.max(np.where(bar > 0, err / np.where(bar > 0, bar, 1), 0.0), initial=0.0))
 
 
 # ---------------------------------------------------------------------------------------- Gramian
 def gramian_paths(f):
-    if f == 64:
+    if (f + 15) // 16 * 16 == 64:  # the path follows the padded width: 49..63 factors run the wgmma kernel too
         return {"wgmma": {}, "gramian_fma": {"gramian_fma": 1}}
     return {"fma": {}}
 
 
 @pytest.mark.parametrize("kind", KINDS)
-@pytest.mark.parametrize("f", [16, 40, 64, 100, 128])
+@pytest.mark.parametrize("f", [16, 40, 49, 63, 64, 100, 128])
 def test_gramian_elementwise_against_fp64(lib, ctx, sm, f, kind):
     """Error model: an fp32-faithful Gramian is the fp64 one up to a few ulps of the sum of |terms| per entry, so
     |G - G64| <= 1e-6 (|Y|^T |Y|) elementwise -- the normwise 1e-6 of C2 applied entry by entry, which a wrong
@@ -188,10 +122,10 @@ def chunked_ratios(Y, W, Z, P, Ginv, chunk=1 << 17):
 
 
 @pytest.mark.parametrize("kind", KINDS)
-@pytest.mark.parametrize("f", [33, 48, 64])
+@pytest.mark.parametrize("f", [33, 48, 49, 63, 64])
 def test_whitened_factors_against_fp64(lib, ctx, sm, f, kind):
     """W = Y P and Z = Y G^-1 of the short-row path (als_whitened_factors): the wgmma apply (64 padded factors,
-    at least 128 rows) and the fp32 FMA tiles (whiten_fma, and every other width).
+    49..64 real ones, at least 128 rows) and the fp32 FMA tiles (whiten_fma, and every other width).
     Error model: |Z - Zt| <= e |Y||G^-1| and |W - Wt| <= e |Y||P| + 2^-38 elementwise, e = max(1e-6, (f + 2) 2^-24):
     the textbook bound of a length-f fp32 dot product plus the fp32 rounding of P or G^-1 and of the result (measured
     on one H100: Z reaches 1.2e-6 relative at a million rows, where 64M entries sample the tail).  2^-38 is the
@@ -226,34 +160,6 @@ KNOB_SETTINGS = {
     "whiten_fma": {"whiten_fma": 1},
     "gramian_fma": {"gramian_fma": 1},
 }
-
-
-def mixed_csr(users, items, seed):
-    """Rows at every short-row class boundary, giant rows past the split threshold (> 3072), negative confidences,
-    weights |c| - 1 below zero and stored zeros."""
-    rng = np.random.default_rng(seed)
-    lengths = [0, 1, 8, 9, 15, 16, 17, 24, 25, 31, 32, 33, 40, 41, 47, 48, 49, 64, 65, 200]
-    lens = [lengths[u % len(lengths)] for u in range(users)]
-    lens[3], lens[50], lens[97] = 3073, 3500, 4100
-    rows, cols, vals = [], [], []
-    for u, n in enumerate(lens):
-        c = rng.choice(items, n, replace=False)
-        v = 1 + 4 * rng.random(n)
-        kind = u % 9
-        if n and kind == 1:
-            v[0] = 0.5      # weight below zero
-        elif n and kind == 2:
-            v[0] = 0.0      # stored zero
-        elif n and kind == 3:
-            v[: n // 2 + 1] *= -1
-        elif n and kind == 4:
-            v[0] = -0.25
-        rows += [u] * n
-        cols += c.tolist()
-        vals += v.tolist()
-    Cui = sp.csr_matrix((np.array(vals, dtype=np.float32), (rows, cols)), shape=(users, items))
-    assert (Cui.data == 0).sum() > 0
-    return Cui
 
 
 @pytest.mark.parametrize("state", ["cold", "warm"])
@@ -371,14 +277,18 @@ def _check_ids(ids, sc, eids, esc, noise, what):
     return same
 
 
-@pytest.mark.parametrize("n_items", [256, 257, 64 * 40 + 1])
-@pytest.mark.parametrize("n_query", [1024, 1025, 256 * 5 + 1, 256 * 5 + 128, 256 * 6 + 129])
-def test_topk_wgmma_tile_edges(lib, ctx, orc, n_query, n_items):
+TILE_EDGE_SHAPES = [(q, i, 64) for q in (1024, 1025, 256 * 5 + 1, 256 * 5 + 128, 256 * 6 + 129)
+                    for i in (256, 257, 64 * 40 + 1)] + [(1025, 257, 50), (256 * 6 + 129, 64 * 40 + 1, 50)]
+
+
+@pytest.mark.parametrize("n_query,n_items,f", TILE_EDGE_SHAPES,
+                         ids=[f"{q}-{i}" + ("" if f == 64 else f"-f{f}") for q, i, f in TILE_EDGE_SHAPES])
+def test_topk_wgmma_tile_edges(lib, ctx, orc, n_query, n_items, f):
     """Query counts that leave a CTA's second warpgroup without queries or with one; 256 items (four tiles, no ring
     wrap), 257 and 64 m + 1 (a one-item last tile); k = 1 and 16 on the wgmma kernel and k = 17 on the mma.sync
-    kernel; a liked CSR and a global filter list.  Ids must equal the reference's away from near-ties (noise per
-    row: 4 eps |q| max|i|) and the mma.sync kernel's, scores to rtol 2e-5."""
-    f = 64
+    kernel; a liked CSR and a global filter list; 64 factors, and 50 (64 padded, 14 zero columns) at two shapes.
+    Ids must equal the reference's away from near-ties (noise per row: 4 eps |q| max|i|) and the mma.sync kernel's,
+    scores to rtol 2e-5."""
     rng = np.random.default_rng(n_query * 7 + n_items)
     users = (rng.standard_normal((n_query, f)) * 0.3).astype(np.float32)
     items = (rng.standard_normal((n_items, f)) * 0.3).astype(np.float32)
@@ -452,14 +362,14 @@ def test_topk_wgmma_query_rows_with_repeats(lib, ctx, orc):
         first.setdefault(r, n)
 
 
-@pytest.mark.parametrize("k", [1, 16])
-def test_topk_wgmma_small_query_norms_against_fp64(lib, ctx, k):
-    """Query rows at 10^U(-6, 0) of the largest one.  Error model: the score of every returned id is the fp64
-    product to within 4 eps |q| max|i| (per query row: the kernel must keep its relative accuracy however small a
-    query is next to the others; the item side is absolute, DESIGN.md section 4.3); ids equal the fp64 top-k and the
-    mma.sync kernel's away from near-ties."""
-    f, Q, I = 64, 1500, 2000
-    rng = np.random.default_rng(79 + k)
+@pytest.mark.parametrize("k,f", [(1, 64), (16, 64), (1, 50), (16, 50)], ids=["1", "16", "1-f50", "16-f50"])
+def test_topk_wgmma_small_query_norms_against_fp64(lib, ctx, k, f):
+    """Query rows at 10^U(-6, 0) of the largest one, at 64 factors and at 50 (64 padded).  Error model: the score of
+    every returned id is the fp64 product to within 4 eps |q| max|i| (per query row: the kernel must keep its
+    relative accuracy however small a query is next to the others; the item side is absolute, DESIGN.md section 4.3);
+    ids equal the fp64 top-k and the mma.sync kernel's away from near-ties."""
+    Q, I = 1500, 2000
+    rng = np.random.default_rng(79 + k + f)
     users = rng.standard_normal((Q, f)).astype(np.float32)
     users = (users * 10.0 ** rng.uniform(-6, 0, size=(Q, 1))).astype(np.float32)
     items = rng.standard_normal((I, f)).astype(np.float32)
