@@ -395,7 +395,8 @@ int launch_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_fa
     case 3: return run_cholesky<3>(ctx, C, X, Y);
     case 4: return run_cholesky<4>(ctx, C, X, Y);
     default:
-      return launch_cholesky_wide(ctx, C, X, Y);  // 64 < padded factors <= 128: cholesky_wide.cu
+      if (Y->ld <= 128) return launch_cholesky_wide(ctx, C, X, Y);  // 64 < padded factors <= 128: cholesky_wide.cu
+      return launch_cholesky_xwide(ctx, C, X, Y);                    // 256 ... 1024: cholesky_xwide.cu
   }
 }
 

@@ -216,10 +216,7 @@ int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const a
     case 5: return run_wide<5>(ctx, C, X, Y);
     case 6: return run_wide<6>(ctx, C, X, Y);
     case 7: return run_wide<7>(ctx, C, X, Y);
-    case 8: return run_wide<8>(ctx, C, X, Y);
-    default:
-      set_error("cholesky: factors=%d (padded %d) is not supported: the Cholesky solver covers factors <= 128, wider models use CG", Y->f, Y->ld);
-      return ALS_E_UNSUPPORTED;
+    default: return run_wide<8>(ctx, C, X, Y);  // launch_cholesky sends only padded factors 80 ... 128 here
   }
 }
 

@@ -208,7 +208,8 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y);                  // -> c
 int comm_allreduce_gramian(als_ctx *ctx, int n_floats);                   // sum ctx->G over ranks (comm.cu)
 int launch_regularize(als_ctx *ctx, int f, int ld, float lambda);         // ctx->G -> ctx->Greg
 int launch_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);
-int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);
+int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);   // 64 < ld <= 128
+int launch_cholesky_xwide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);  // 128 < ld <= 1024
 // long rows on the wgmma tensor cores (cholesky_tc.cu): 64 padded factors, no weights |c| - 1 < 0
 bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld);
 int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items, cudaStream_t stream);

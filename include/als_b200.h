@@ -115,7 +115,7 @@ int als_csr_destroy(als_csr *csr);
 /* ---- dense factor matrices ------------------------------------------------------------------- */
 /* Replaces Matrix::Matrix(rows, cols, data), implicit/gpu/matrix.cu:66-104.  1 <= factors <= 1024 (the bound of the
  * reference's CUDA solver, implicit/gpu/als.cu:177-178); the device row stride is the width rounded up to 16 (<= 128) or
- * to 128 (wider: CG solver only). */
+ * to 128 (wider).  Both solvers cover every width. */
 int als_factors_create(als_ctx *ctx, int64_t rows, int factors, als_factors **out);
 /* host[nrows, factors] (row-major, unpadded) <-> device rows [row0, row0 + nrows). */
 int als_factors_upload(als_ctx *ctx, als_factors *f, const float *host, int64_t row0, int64_t nrows);
