@@ -43,6 +43,9 @@ SIGNATURES = {
     "als_host_alloc": (c_int, [P(c_void_p), c_i64]),
     "als_host_free": (c_int, [c_void_p]),
     "als_csr_upload": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_void_p, c_i64, P(c_void_p)]),
+    "als_csr_upload64": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_int, c_void_p, c_i64, P(c_void_p)]),
+    "als_csr_segment_count": (c_int, [c_void_p, P(c_i64)]),
+    "als_csr_download64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "als_csr_transpose": (c_int, [c_void_p, c_void_p, P(c_void_p)]),
     "als_csr_generate": (c_int, [c_void_p, c_i64, c_i64, c_i64, ctypes.c_uint64, P(c_void_p)]),
     "als_factors_fill_uniform": (c_int, [c_void_p, c_void_p, ctypes.c_uint64, ctypes.c_float]),
@@ -284,8 +287,19 @@ def comm_unique_id():
     return buf.tobytes()
 
 
+#: the largest nnz als_csr_upload takes (int32 positions); above it, als_csr_upload64 stores the CSR as row-block segments
+INT32_CSR_MAX_NNZ = 2**31 - 2
+
+
+def csr_upload_route(nnz):
+    """Which upload a CSR of `nnz` nonzeros takes: "int32" (als_csr_upload, int32 host arrays) or "int64"
+    (als_csr_upload64: the scipy arrays as they are, int32 or int64, narrowed while they are staged)."""
+    return "int32" if nnz <= INT32_CSR_MAX_NNZ else "int64"
+
+
 class DeviceCSR:
-    """als_csr: a CSR (or a row shard of one) resident on the device with its launch schedule."""
+    """als_csr: a CSR (or a row shard of one) resident on the device with its launch schedule.  A CSR with more
+    nonzeros than the segment cap is held as row-block segments of int32 positions; every call takes it as it is."""
 
     def __init__(self, ctx, handle, parent=None):
         self.ctx, self.h, self._parent = ctx, handle, parent
@@ -293,18 +307,31 @@ class DeviceCSR:
     @classmethod
     def upload(cls, ctx, m, row_offset=0, rows=None):
         """m: scipy.sparse.csr_matrix (any float dtype; values are cast to float32)."""
+        data = np.ascontiguousarray(m.data, dtype=np.float32)
+        h = c_void_p()
+        if csr_upload_route(m.nnz) == "int64":
+            indptr = np.ascontiguousarray(m.indptr, dtype=np.int64)
+            indices = m.indices
+            if indices.dtype not in (np.int32, np.int64) or not indices.flags.c_contiguous:
+                indices = np.ascontiguousarray(indices, dtype=np.int64)
+            check(ctx.lib.als_csr_upload64(ctx.h, m.shape[0], m.shape[1], m.nnz, ptr(indptr), ptr(indices),
+                                           indices.dtype.itemsize, ptr(data), int(row_offset), ctypes.byref(h)))
+            return cls(ctx, h)
         indptr = m.indptr
         if indptr.dtype != np.int32:
-            if m.nnz >= 2**31:
-                raise ValueError("int32 CSR only: nnz must be < 2^31")
             indptr = indptr.astype(np.int32)
         indices = np.ascontiguousarray(m.indices, dtype=np.int32)
-        data = np.ascontiguousarray(m.data, dtype=np.float32)
         indptr = np.ascontiguousarray(indptr)
-        h = c_void_p()
         check(ctx.lib.als_csr_upload(ctx.h, m.shape[0], m.shape[1], m.nnz, ptr(indptr), ptr(indices), ptr(data),
                                      int(row_offset), ctypes.byref(h)))
         return cls(ctx, h)
+
+    @property
+    def segment_count(self):
+        """Row-block segments of the device layout (1 unless nnz exceeds the segment cap)."""
+        n = c_i64()
+        check(self.ctx.lib.als_csr_segment_count(self.h, ctypes.byref(n)))
+        return n.value
 
     def transpose(self):
         h = c_void_p()
@@ -336,14 +363,20 @@ class DeviceCSR:
         import scipy.sparse as sp
 
         rows, cols, nnz = self.shape3
-        indptr = np.zeros(rows + 1, dtype=np.int32)
+        indptr = self.indptr_host()
         indices = np.zeros(nnz, dtype=np.int32)
         data = np.zeros(nnz, dtype=np.float32)
-        check(self.ctx.lib.als_csr_download(self.ctx.h, self.h, ptr(indptr), ptr(indices), ptr(data)))
+        download = self.ctx.lib.als_csr_download64 if indptr.dtype == np.int64 else self.ctx.lib.als_csr_download
+        check(download(self.ctx.h, self.h, None, ptr(indices), ptr(data)))
         return sp.csr_matrix((data, indices, indptr), shape=(rows, cols))
 
     def indptr_host(self):
-        rows, _, _ = self.shape3
+        """int32, or int64 when nnz >= 2^31 (like scipy)."""
+        rows, _, nnz = self.shape3
+        if nnz >= 2**31:
+            indptr = np.zeros(rows + 1, dtype=np.int64)
+            check(self.ctx.lib.als_csr_download64(self.ctx.h, self.h, ptr(indptr), None, None))
+            return indptr
         indptr = np.zeros(rows + 1, dtype=np.int32)
         check(self.ctx.lib.als_csr_download(self.ctx.h, self.h, ptr(indptr), None, None))
         return indptr

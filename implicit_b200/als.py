@@ -19,6 +19,26 @@ from .utils import ModelFitError, check_csr, check_random_state, nnz_balanced_sp
 
 log = logging.getLogger("implicit")
 
+#: nonzeros of the filter CSR ("already liked") that one top-k call takes: its kernels walk int32 positions
+_LIKED_NNZ_MAX = _lib.INT32_CSR_MAX_NNZ
+
+
+def liked_batches(indptr, limit):
+    """Consecutive query ranges [(start, end), ...] covering every row of a CSR with this `indptr`, each holding at
+    most `limit` nonzeros (recommend splits its top-k call along them)."""
+    indptr = np.asarray(indptr, dtype=np.int64)
+    n = len(indptr) - 1
+    out = []
+    start = 0
+    while start < n:
+        end = min(int(np.searchsorted(indptr, indptr[start] + limit, side="right")) - 1, n)
+        if end <= start:
+            raise ValueError(f"row {start} of user_items holds {int(indptr[start + 1] - indptr[start])} nonzeros, "
+                             f"more than one top-k call takes ({limit})")
+        out.append((start, end))
+        start = end
+    return out
+
 
 class AlternatingLeastSquares:
     """Alternating Least Squares (Hu, Koren & Volinsky 2008; CG variant Takacs et al. 2011) on one or more H100s.
@@ -407,15 +427,16 @@ class AlternatingLeastSquares:
                 item_handle = _lib.DeviceFactors.from_host(ctx, self.item_factors[items])
                 tmp.append(item_handle)
 
-            liked = None
+            fq = None
+            batches = [(0, n_query)]
             if filter_already_liked_items:
                 fq = user_items
                 if items is not None:
                     fq = _filter_items_from_sparse_matrix(items, fq)
                 if not fq.has_sorted_indices:
                     fq = fq.sorted_indices()
-                liked = _lib.DeviceCSR.upload(ctx, fq)
-                tmp.append(liked)
+                if fq.nnz > _LIKED_NNZ_MAX:
+                    batches = liked_batches(fq.indptr, _LIKED_NNZ_MAX)
 
             fl = None
             if filter_items is not None:
@@ -423,8 +444,21 @@ class AlternatingLeastSquares:
                 if fl.size and (fl.min() < 0 or fl.max() >= item_handle.rows):
                     raise IndexError("filter_items contains ids that are not in the model")
 
-            ids, scores = _lib.topk(ctx, item_handle, queries, int(N), query_rows=query_rows, n_query=n_query,
-                                    liked=liked, filter_items=fl)
+            parts = []
+            for b0, b1 in batches:
+                qr = query_rows
+                if len(batches) > 1:
+                    qr = query_rows[b0:b1] if query_rows is not None else np.arange(b0, b1)
+                liked = None
+                if fq is not None:
+                    liked = _lib.DeviceCSR.upload(ctx, fq if len(batches) == 1 else fq[b0:b1])
+                    tmp.append(liked)
+                parts.append(_lib.topk(ctx, item_handle, queries, int(N), query_rows=qr, n_query=b1 - b0,
+                                       liked=liked, filter_items=fl))
+                if liked is not None:
+                    liked.close()
+            ids, scores = parts[0] if len(parts) == 1 else (np.concatenate([p[0] for p in parts]),
+                                                             np.concatenate([p[1] for p in parts]))
         finally:
             for t in tmp:
                 t.close()

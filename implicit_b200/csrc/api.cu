@@ -6,6 +6,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
+#include <functional>
 #include <thread>
 
 #include "common.h"
@@ -95,15 +97,11 @@ int ensure_pinned(als_ctx *ctx, int64_t bytes) {
 static constexpr int kStageThreads = 4;
 static constexpr size_t kStageChunk = 4u << 20;
 
-static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
-  if (bytes == 0) return ALS_OK;
-  cudaPointerAttributes at;
-  const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-  cudaGetLastError();  // an unregistered host pointer may leave an error behind on older drivers
-  if (pinned || bytes < 2 * kStageChunk * kStageThreads) {
-    ALS_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    return ALS_OK;
-  }
+// fill(stage, off, len): writes the `len` bytes that go to dst + off into the staging buffer; false stops the copy
+// (the caller's input is bad, ALS_E_INVALID)
+using StageFill = std::function<bool(char *stage, size_t off, size_t len)>;
+
+static int staged_h2d(als_ctx *ctx, void *dst, size_t bytes, const StageFill &fill) {
   if (!ctx->stage_buf) {
     ALS_CUDA(cudaMallocHost(&ctx->stage_buf, kStageThreads * 2 * kStageChunk));
     for (int t = 0; t < kStageThreads; ++t) {
@@ -117,9 +115,10 @@ static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
   for (int t = 0; t < kStageThreads; ++t) ALS_CUDA(cudaStreamWaitEvent(ctx->stage_stream[t], ctx->stage_ready, 0));
   const size_t nchunks = (bytes + kStageChunk - 1) / kStageChunk;
   std::vector<int> status(kStageThreads, (int)cudaSuccess);
+  std::atomic<bool> refused{false};
   std::vector<std::thread> pool;
   for (int t = 0; t < kStageThreads; ++t) {
-    pool.emplace_back([=, &status]() {
+    pool.emplace_back([=, &status, &refused, &fill]() {
       cudaSetDevice(ctx->device);
       // the staging buffers are shared by consecutive calls: a previous call's last DMAs may still be reading them
       cudaError_t e = cudaStreamSynchronize(ctx->stage_stream[t]);
@@ -129,7 +128,10 @@ static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
         char *stage = (char *)ctx->stage_buf + ((size_t)t * 2 + b) * kStageChunk;
         if (use >= 2) e = cudaEventSynchronize(ctx->stage_ev[t][b]);  // the DMA out of this buffer has finished
         const size_t off = c * kStageChunk, len = std::min(kStageChunk, bytes - off);
-        memcpy(stage, (const char *)src + off, len);
+        if (!fill(stage, off, len)) {
+          refused = true;
+          break;
+        }
         if (e == cudaSuccess) e = cudaMemcpyAsync((char *)dst + off, stage, len, cudaMemcpyHostToDevice, ctx->stage_stream[t]);
         if (e == cudaSuccess) e = cudaEventRecord(ctx->stage_ev[t][b], ctx->stage_stream[t]);
       }
@@ -143,7 +145,59 @@ static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
     ALS_CUDA(cudaEventRecord(ctx->stage_ev[t][0], ctx->stage_stream[t]));
     ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[t][0], 0));
   }
-  return ALS_OK;
+  return refused ? ALS_E_INVALID : ALS_OK;
+}
+
+static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
+  if (bytes == 0) return ALS_OK;
+  cudaPointerAttributes at;
+  const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
+  cudaGetLastError();  // an unregistered host pointer may leave an error behind on older drivers
+  if (pinned || bytes < 2 * kStageChunk * kStageThreads) {
+    ALS_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    return ALS_OK;
+  }
+  return staged_h2d(ctx, dst, bytes, [src](char *stage, size_t off, size_t len) {
+    memcpy(stage, (const char *)src + off, len);
+    return true;
+  });
+}
+
+// n column indices (int32 or int64 on the host) -> int32 on the device, narrowed chunk by chunk in the staging threads
+// (no host-side int32 copy of the whole array, half the PCIe bytes of int64).  Every index must lie in [0, cols): the
+// first one that does not is reported in *bad_at (else -1) and the call returns ALS_E_INVALID.
+static int h2d_indices(als_ctx *ctx, int32_t *dst, const void *src, int index_bytes, int64_t n, int64_t cols, int64_t *bad_at) {
+  *bad_at = -1;
+  if (n == 0) return ALS_OK;
+  std::atomic<int64_t> bad{INT64_MAX};
+  auto narrow = [&](char *stage, size_t off, size_t len) -> bool {
+    int32_t *o = reinterpret_cast<int32_t *>(stage);
+    const int64_t i0 = (int64_t)(off / 4), m = (int64_t)(len / 4);
+    int64_t first = -1;
+    if (index_bytes == 8) {
+      const int64_t *in = static_cast<const int64_t *>(src) + i0;
+      for (int64_t k = 0; k < m; ++k) {
+        const int64_t v = in[k];
+        if ((uint64_t)v >= (uint64_t)cols && first < 0) first = k;
+        o[k] = (int32_t)v;
+      }
+    } else {
+      const int32_t *in = static_cast<const int32_t *>(src) + i0;
+      for (int64_t k = 0; k < m; ++k) {
+        const int32_t v = in[k];
+        if ((uint64_t)(int64_t)v >= (uint64_t)cols && first < 0) first = k;
+        o[k] = v;
+      }
+    }
+    if (first < 0) return true;
+    int64_t cur = bad.load();
+    while (i0 + first < cur && !bad.compare_exchange_weak(cur, i0 + first)) {
+    }
+    return false;
+  };
+  const int rc = staged_h2d(ctx, dst, (size_t)n * sizeof(int32_t), narrow);
+  if (rc == ALS_E_INVALID) *bad_at = bad.load();
+  return rc;
 }
 
 // Longest-first schedule.  Rows with more than kSplitNnz nonzeros are cut into chunks of kChunkNnz
@@ -301,7 +355,8 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   {
     struct { const char *env; const char *name; } table[] = {
         {"ALS_B200_SHORT_MAX", "short_max"}, {"ALS_B200_SHORT_SERIAL", "short_serial"}, {"ALS_B200_WHITEN_FMA", "whiten_fma"},
-        {"ALS_B200_GRAMIAN_FMA", "gramian_fma"}, {"ALS_B200_TOPK_LEGACY", "topk_legacy"}, {"ALS_B200_LONG_TC", "long_tc"}, {"ALS_B200_CG_NV", "cg_nv"}};
+        {"ALS_B200_GRAMIAN_FMA", "gramian_fma"}, {"ALS_B200_TOPK_LEGACY", "topk_legacy"}, {"ALS_B200_LONG_TC", "long_tc"}, {"ALS_B200_CG_NV", "cg_nv"},
+        {"ALS_B200_SEGMENT_NNZ", "segment_nnz"}};
     for (const auto &t : table) {
       const char *e = getenv(t.env);
       if (!e) continue;
@@ -366,6 +421,9 @@ ALS_API int als_ctx_set_knob(als_ctx *ctx, const char *name, int value) {
   else if (!strcmp(name, "cg_nv")) {
     ALS_REQUIRE(value == 1 || value == 2 || value == 4, "als_ctx_set_knob: cg_nv must be 1, 2 or 4");
     k.cg_nv = value;
+  } else if (!strcmp(name, "segment_nnz")) {
+    ALS_REQUIRE(value >= 0 && value < INT32_MAX, "als_ctx_set_knob: segment_nnz must be in [0, 2^31 - 1)");
+    k.segment_nnz = value;
   } else {
     set_error("als_ctx_set_knob: unknown knob '%s'", name);
     return ALS_E_INVALID;
@@ -546,6 +604,19 @@ ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz
     }
   }
   int arc;
+  if (needs_segments(ctx, nnz)) {  // a cap set by the segment_nnz knob: the same layout as als_csr_upload64's
+    std::vector<int64_t> ip64(ip, ip + rows + 1);
+    if ((arc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * nnz)) != ALS_OK ||
+        (arc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * nnz)) != ALS_OK ||
+        (arc = h2d_copy(ctx, c->indices, indices + base, sizeof(int32_t) * nnz)) != ALS_OK ||
+        (arc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz)) != ALS_OK ||
+        (arc = make_segments(ctx, c, ip64.data())) != ALS_OK) {
+      als_csr_destroy(c);
+      return arc;
+    }
+    *out = c;
+    return ALS_OK;
+  }
   if ((arc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (rows + 1))) != ALS_OK ||
       (arc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
       (arc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK) {
@@ -567,6 +638,66 @@ ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz
     return rc;
   }
   *out = c;
+  return ALS_OK;
+}
+
+ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
+                             const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+  ALS_REQUIRE(ctx && out && indptr, "als_csr_upload64: NULL argument");
+  ALS_REQUIRE(index_bytes == 4 || index_bytes == 8, "als_csr_upload64: index_bytes must be 4 or 8, got %d", index_bytes);
+  ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "als_csr_upload64: negative shape");
+  ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "als_csr_upload64: rows and cols must be < 2^31 - 1");
+  ALS_REQUIRE(indptr[0] >= 0 && indptr[rows] - indptr[0] == nnz, "als_csr_upload64: indptr[rows] - indptr[0] = %lld != nnz = %lld",
+              (long long)(indptr[rows] - indptr[0]), (long long)nnz);
+  ALS_REQUIRE(nnz == 0 || (indices && data), "als_csr_upload64: indices/data NULL with nnz > 0");
+  for (int64_t r = 0; r < rows; ++r)
+    ALS_REQUIRE(indptr[r + 1] >= indptr[r], "als_csr_upload64: indptr is not monotone at row %lld", (long long)r);
+  *out = nullptr;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  als_csr *c = new als_csr();
+  c->ctx = ctx;
+  c->rows = rows;
+  c->cols = cols;
+  c->nnz = nnz;
+  c->row_offset = row_offset;
+  const int64_t base = indptr[0];  // a row shard arrives with indptr[0] != 0
+  int rc;
+  int64_t bad = -1;
+  if ((rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+      (rc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+      (rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad)) != ALS_OK ||
+      (rc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz)) != ALS_OK) {
+    if (bad >= 0) {
+      const int64_t v = index_bytes == 8 ? ((const int64_t *)indices)[base + bad] : ((const int32_t *)indices)[base + bad];
+      set_error("als_csr_upload64: indices[%lld] = %lld is outside [0, %lld)", (long long)(base + bad), (long long)v, (long long)cols);
+    }
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    als_csr_destroy(c);
+    return rc;
+  }
+  std::vector<int64_t> ip((size_t)rows + 1);
+  for (int64_t r = 0; r <= rows; ++r) ip[r] = indptr[r] - base;
+  if (needs_segments(ctx, nnz)) {
+    rc = make_segments(ctx, c, ip.data());
+  } else {
+    std::vector<int32_t> ip32(ip.begin(), ip.end());
+    if ((rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (rows + 1))) == ALS_OK) {
+      ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * (rows + 1), cudaMemcpyHostToDevice, ctx->stream));
+      rc = build_schedule(ctx, c, ip32.data());
+      ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+  }
+  if (rc != ALS_OK) {
+    als_csr_destroy(c);
+    return rc;
+  }
+  *out = c;
+  return ALS_OK;
+}
+
+ALS_API int als_csr_segment_count(const als_csr *csr, int64_t *n) {
+  ALS_REQUIRE(csr && n, "als_csr_segment_count: NULL argument");
+  *n = csr->segs.empty() ? 1 : (int64_t)csr->segs.size();
   return ALS_OK;
 }
 
@@ -596,6 +727,26 @@ ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int6
   ALS_REQUIRE(in->row_offset == 0, "als_csr_slice_rows: cannot slice a shard");
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
+  if (!in->segs.empty()) {  // a shard of a segmented CSR can itself exceed 2^31 nonzeros: a segmented view
+    std::vector<int64_t> ip64;
+    int rc = csr_indptr64(ctx, in, ip64);
+    if (rc != ALS_OK) return rc;
+    als_csr *c = new als_csr();
+    c->ctx = ctx;
+    c->rows = r1 - r0;
+    c->cols = in->cols;
+    c->nnz = ip64[r1] - ip64[r0];
+    c->row_offset = r0;
+    c->owns = false;
+    c->indices = in->indices;
+    c->data = in->data;
+    if ((rc = make_segments(ctx, c, ip64.data() + r0)) != ALS_OK) {
+      als_csr_destroy(c);
+      return rc;
+    }
+    *out = c;
+    return ALS_OK;
+  }
   const int64_t rows = r1 - r0;
   std::vector<int32_t> ip((size_t)rows + 1);
   ALS_CUDA(cudaMemcpyAsync(ip.data(), in->indptr + r0, sizeof(int32_t) * (rows + 1), cudaMemcpyDeviceToHost, ctx->stream));
@@ -624,7 +775,9 @@ ALS_API int als_csr_scale(als_ctx *ctx, als_csr *csr, float alpha) {
   if (csr->nnz == 0) return ALS_OK;
   ALS_CUDA(cudaSetDevice(ctx->device));
   csr->wmax_valid = false;
-  scale_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(csr->data, csr->nnz, alpha);
+  // segments are consecutive blocks of one array: the first one starts the CSR's values
+  float *data = csr->segs.empty() ? csr->data : csr->segs[0]->data;
+  scale_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(data, csr->nnz, alpha);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   return ALS_OK;
@@ -640,7 +793,17 @@ ALS_API int als_csr_shape(const als_csr *csr, int64_t *rows, int64_t *cols, int6
 
 ALS_API int als_csr_download(als_ctx *ctx, const als_csr *csr, int32_t *indptr, int32_t *indices, float *data) {
   ALS_REQUIRE(ctx && csr, "als_csr_download: NULL argument");
+  ALS_REQUIRE(csr->nnz < (int64_t)INT32_MAX, "als_csr_download: %lld nonzeros need a 64-bit indptr: use als_csr_download64",
+              (long long)csr->nnz);
   ALS_CUDA(cudaSetDevice(ctx->device));
+  if (!csr->segs.empty()) {
+    std::vector<int64_t> ip64((size_t)csr->rows + 1);
+    int rc = als_csr_download64(ctx, csr, indptr ? ip64.data() : nullptr, indices, data);
+    if (rc != ALS_OK) return rc;
+    if (indptr)
+      for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] = (int32_t)ip64[r];
+    return ALS_OK;
+  }
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   // a row-slice view keeps absolute positions into its parent's arrays: rebase on the way out
   int32_t base = 0;
@@ -650,6 +813,22 @@ ALS_API int als_csr_download(als_ctx *ctx, const als_csr *csr, int32_t *indptr, 
     if (base)
       for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] -= base;
   }
+  if (indices && csr->nnz)
+    ALS_CUDA(cudaMemcpy(indices, csr->indices + base, sizeof(int32_t) * csr->nnz, cudaMemcpyDeviceToHost));
+  if (data && csr->nnz)
+    ALS_CUDA(cudaMemcpy(data, csr->data + base, sizeof(float) * csr->nnz, cudaMemcpyDeviceToHost));
+  return ALS_OK;
+}
+
+ALS_API int als_csr_download64(als_ctx *ctx, const als_csr *csr, int64_t *indptr, int32_t *indices, float *data) {
+  ALS_REQUIRE(ctx && csr, "als_csr_download64: NULL argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  std::vector<int64_t> ip;
+  int rc = csr_indptr64(ctx, csr, ip);
+  if (rc != ALS_OK) return rc;
+  const int64_t base = ip[0];  // a row-slice view keeps absolute positions into its parent's arrays: rebase
+  if (indptr)
+    for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] = ip[r] - base;
   if (indices && csr->nnz)
     ALS_CUDA(cudaMemcpy(indices, csr->indices + base, sizeof(int32_t) * csr->nnz, cudaMemcpyDeviceToHost));
   if (data && csr->nnz)
@@ -680,6 +859,8 @@ ALS_API int als_csr_destroy(als_csr *csr) {
     dev_free(ctx, csr->finish);
     dev_free(ctx, csr->chunks);
     dev_free(ctx, csr->chunk_owner);
+    for (als_csr *seg : csr->segs) als_csr_destroy(seg);
+    dev_free(ctx, csr->seg_indptr);
   }
   delete csr;
   return ALS_OK;
@@ -1055,9 +1236,17 @@ ALS_API int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors
   int rc = check_half("als_calculate_loss", ctx, C, const_cast<als_factors *>(X), Y);
   if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaSetDevice(ctx->device));
-  rc = launch_gramian(ctx, Y);
-  if (rc != ALS_OK) return rc;
-  return launch_loss(ctx, C, X, Y, regularization, loss);
+  // per segment (launch_loss leaves X^T X of the segment's rows in the Gramian buffer): the terms are shard sums
+  double sum[3] = {0.0, 0.0, 0.0};
+  for (const als_csr *S : segments_of(C)) {
+    double t[3];
+    if ((rc = launch_gramian(ctx, Y)) != ALS_OK || (rc = launch_loss(ctx, S, X, Y, regularization, t)) != ALS_OK) return rc;
+    sum[0] += t[0];
+    sum[1] += t[1];
+    sum[2] = t[2];  // reg ||Y||^2: once
+  }
+  for (int i = 0; i < 3; ++i) loss[i] = sum[i];
+  return ALS_OK;
 }
 
 ALS_API int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
@@ -1068,6 +1257,8 @@ ALS_API int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *
   ALS_REQUIRE(k >= 0 && n_query >= 0, "als_topk: negative k or n_query");
   ALS_REQUIRE(!liked || liked->rows == n_query, "als_topk: liked has %lld rows for %lld queries",
               liked ? (long long)liked->rows : 0LL, (long long)n_query);
+  ALS_REQUIRE(!liked || liked->segs.empty(), "als_topk: the liked CSR (%lld nonzeros) is held as segments; split the queries "
+              "into calls whose liked rows hold fewer than 2^31 - 1 nonzeros", liked ? (long long)liked->nnz : 0LL);
   ALS_REQUIRE(!liked || liked->cols == items->rows, "als_topk: liked has %lld columns for %lld items",
               liked ? (long long)liked->cols : 0LL, (long long)items->rows);
   ALS_CUDA(cudaSetDevice(ctx->device));

@@ -382,9 +382,7 @@ int run_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
   return ALS_OK;
 }
 
-}  // namespace
-
-int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int cg_steps) {
+int launch_cg_segment(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int cg_steps) {
   if (X->ld != Y->ld) {
     set_error("cg: X and Y strides differ (%d vs %d)", X->ld, Y->ld);
     return ALS_E_INVALID;
@@ -426,6 +424,17 @@ int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors 
       return ALS_E_UNSUPPORTED;
   }
 #undef ALS_CG_CASE
+}
+
+}  // namespace
+
+// rows are independent: a CSR of row-block segments is solved one segment after the other with the same Greg
+int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int cg_steps) {
+  for (const als_csr *S : segments_of(C)) {
+    int rc = launch_cg_segment(ctx, S, X, Y, cg_steps);
+    if (rc != ALS_OK) return rc;
+  }
+  return ALS_OK;
 }
 
 }  // namespace als

@@ -254,6 +254,16 @@ static int debug_flags() {
 #endif
 }
 
+// zeroes the per-segment work counters between the segments of one half: the whitening flag and max |y| of the half
+// (kCtrWhitenOk, kCtrYAbsMax) stay
+__global__ void reset_segment_counters(int32_t *counters) {
+  const int t = threadIdx.x;
+  if (t < 16 && t != kCtrWhitenOk && t != kCtrHasNan && t != kCtrYAbsMax) counters[t] = 0;
+}
+
+// One half over C, which may be a list of row-block segments.  Everything that affects rounding is decided once for the
+// whole matrix (bad_row reset, max |y|, max ||c| - 1|, the long-row kernel, whether short rows take the whitened path,
+// the whitening itself); the deferred list, its counters and the giant-row slots are per segment.
 template <int NB>
 int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_factors *Y) {
   using C = Cfg<NB>;
@@ -267,9 +277,12 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     set_error("cholesky: kernel does not fit on an SM (smem %d bytes)", smem);
     return ALS_E_CUDA;
   }
+  const std::vector<const als_csr *> segs = segments_of(Cm);
+  int64_t max_slots = 0;
+  for (const als_csr *S : segs) max_slots = std::max(max_slots, S->n_slots);
   float *slots = nullptr;
-  if (Cm->n_slots) {
-    int rc = ensure_scratch(ctx, (int64_t)Cm->n_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
+  if (max_slots) {
+    int rc = ensure_scratch(ctx, max_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
     if (rc != ALS_OK) return rc;
     slots = (float *)ctx->scratch;
   }
@@ -290,9 +303,11 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
   }
   if (!Cmut->wmax_valid) {
     ALS_CUDA(cudaMemsetAsync(Cmut->wmax_dev, 0, 2 * sizeof(unsigned), ctx->stream));
-    csr_wmax_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(Cm->indptr, Cm->rows, Cm->data, Cmut->wmax_dev);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    for (const als_csr *S : segs) {
+      csr_wmax_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(S->indptr, S->rows, S->data, Cmut->wmax_dev);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
     Cmut->wmax_valid = true;
     Cmut->neg_w_known = false;
   }
@@ -304,80 +319,93 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     Cmut->has_neg_w = flag != 0;
     Cmut->neg_w_known = true;
   }
+  const bool long_tc = NB == 4 && cholesky_tc_eligible(ctx, Cm, Y->ld);
   // Items of at most `short_max` nonzeros (a suffix of the length-sorted work list) go through the n x n
   // push-through system of cholesky_short.cu when there are enough of them to pay for whitening Y.
   int short_max = std::min(ctx->knobs.short_max, 16 * (NB - 1));  // a multiple of 8; a system of NS unknowns needs NS < F
-  int64_t n_main = Cm->n_work;
+  const int short_class = (48 - std::max(short_max, 0)) / 8;      // kShortThresholds: 48, 40, ..., 8
   if (short_max > 0) {
-    const int64_t begin = Cm->le_begin[(48 - short_max) / 8];  // kShortThresholds: 48, 40, ..., 8
+    int64_t n_short = 0;
+    for (const als_csr *S : segs) n_short += S->n_work - S->le_begin[short_class];
     // worth it when the short rows outweigh whitening all of Y: one short row saves roughly what whitening 16 rows
     // of Y costs
-    if ((Cm->n_work - begin) * 16 >= Y->rows) n_main = begin;
-    else short_max = 0;
+    if (n_short * 16 < Y->rows) short_max = 0;
   }
-  if (Cm->n_work) {
-    ProfScope prof(ctx, kProfCholesky);
-    const int max_grid = ctx->sm_count * ctas_per_sm;
-    // The short-row side (whitening, the short-row kernels, the second pass of the full-size kernel over what they
-    // hand back) runs on the aux stream.  The single-CTA factorisation of G is launched first and hides behind the
-    // full-size kernel; the rest moves in as that kernel's persistent CTAs run out of long rows.
-    const bool overlap = short_max > 0 && n_main > 0 && !ctx->knobs.short_serial;
-    cudaStream_t side = overlap ? ctx->aux : ctx->stream;
-    if (short_max > 0) {
-      if (overlap) {
-        ALS_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        ALS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
-      }
-      int rc = short_rows_prepare(ctx, Y, side);
-      if (rc != ALS_OK) return rc;
+  const int max_grid = ctx->sm_count * ctas_per_sm;
+  for (size_t s = 0; s < segs.size(); ++s) {
+    const als_csr *S = segs[s];
+    if (s > 0) {
+      reset_segment_counters<<<1, 32, 0, ctx->stream>>>(ctx->counters);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
     }
-    if (n_main && NB == 4 && cholesky_tc_eligible(ctx, Cm, Y->ld)) {
-      // whole rows: normal equations on the wgmma tensor cores; chunks of giant rows: the mma.sync kernel
-      int rc = launch_cholesky_tc(ctx, Cm, X, Y, n_main, ctx->stream);
-      if (rc != ALS_OK) return rc;
-      if (Cm->n_slots) {
-        const int grid = (int)std::min<int64_t>(ceil_div(Cm->n_slots, kWarpsPerCta), max_grid);
-        kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg, Cm->chunks,
-                                                       (int)Cm->n_slots, nullptr, ctx->counters + kCtrChunks, slots, ctx->bad_row,
-                                                       0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+    const int64_t n_main = short_max > 0 ? S->le_begin[short_class] : S->n_work;
+    const bool seg_short = short_max > 0 && S->n_work > n_main;
+    if (S->n_work) {
+      ProfScope prof(ctx, kProfCholesky);
+      // The short-row side (whitening, the short-row kernels, the second pass of the full-size kernel over what they
+      // hand back) runs on the aux stream.  The single-CTA factorisation of G is launched first and hides behind the
+      // full-size kernel; the rest moves in as that kernel's persistent CTAs run out of long rows.
+      const bool overlap = seg_short && n_main > 0 && !ctx->knobs.short_serial;
+      cudaStream_t side = overlap ? ctx->aux : ctx->stream;
+      if (short_max > 0) {
+        if (overlap) {
+          ALS_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+          ALS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
+        }
+        if (s == 0) {  // once per half: the later segments find W and Z in place
+          int rc = short_rows_prepare(ctx, Y, side);
+          if (rc != ALS_OK) return rc;
+        }
+      }
+      if (n_main && long_tc) {
+        // whole rows: normal equations on the wgmma tensor cores; chunks of giant rows: the mma.sync kernel
+        int rc = launch_cholesky_tc(ctx, S, X, Y, n_main, Cm->wmax_dev, ctx->stream);
+        if (rc != ALS_OK) return rc;
+        if (S->n_slots) {
+          const int grid = (int)std::min<int64_t>(ceil_div(S->n_slots, kWarpsPerCta), max_grid);
+          kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg, S->chunks,
+                                                         (int)S->n_slots, nullptr, ctx->counters + kCtrChunks, slots, ctx->bad_row,
+                                                         0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+          ALS_CUDA(cudaGetLastError());
+          ctx->launches++;
+        }
+      } else if (n_main) {
+        const int grid = (int)std::min<int64_t>(ceil_div(n_main, kWarpsPerCta), max_grid);
+        kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
+                                                              S->work, (int)n_main, nullptr, ctx->counters + kCtrMain,
+                                                              slots, ctx->bad_row, 0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
         ALS_CUDA(cudaGetLastError());
         ctx->launches++;
       }
-    } else if (n_main) {
-      const int grid = (int)std::min<int64_t>(ceil_div(n_main, kWarpsPerCta), max_grid);
-      kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
-                                                            Cm->work, (int)n_main, nullptr, ctx->counters + kCtrMain,
-                                                            slots, ctx->bad_row, 0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches++;
-    }
-    if (short_max > 0) {
-      int rc = short_rows_launch(ctx, Cm, X, Y, n_main, short_max, side);
-      if (rc != ALS_OK) return rc;
-      // whatever the short-row kernels handed back (negative weights, chunks of giant rows, G not PD)
-      const int grid = (int)std::min<int64_t>(ceil_div(Cm->n_work - n_main, kWarpsPerCta), max_grid);
-      kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
-                                                     ctx->deferred, 0, ctx->counters + kCtrDeferredCount,
-                                                     ctx->counters + kCtrDeferredWork, slots, ctx->bad_row, 0, dbg,
-                                                     X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches++;
-      if (overlap) {
-        ALS_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
-        ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+      if (seg_short) {
+        int rc = short_rows_launch(ctx, S, X, Y, n_main, short_max, side);
+        if (rc != ALS_OK) return rc;
+        // whatever the short-row kernels handed back (negative weights, chunks of giant rows, G not PD)
+        const int grid = (int)std::min<int64_t>(ceil_div(S->n_work - n_main, kWarpsPerCta), max_grid);
+        kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
+                                                       ctx->deferred, 0, ctx->counters + kCtrDeferredCount,
+                                                       ctx->counters + kCtrDeferredWork, slots, ctx->bad_row, 0, dbg,
+                                                       X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+        ALS_CUDA(cudaGetLastError());
+        ctx->launches++;
+        if (overlap) {
+          ALS_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
+          ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+        }
       }
     }
-  }
-  if (Cm->n_finish) {
-    const int64_t want = ceil_div(Cm->n_finish, kWarpsPerCta);
-    const int grid = (int)std::min<int64_t>(want, (int64_t)ctx->sm_count * ctas_per_sm);
-    ProfScope prof(ctx, kProfCholFinish);
-    kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
-                                                          Cm->finish, (int)Cm->n_finish, nullptr,
-                                                          ctx->counters + kCtrFinish, slots,
-                                                          ctx->bad_row, 1, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
+    if (S->n_finish) {
+      const int64_t want = ceil_div(S->n_finish, kWarpsPerCta);
+      const int grid = (int)std::min<int64_t>(want, (int64_t)max_grid);
+      ProfScope prof(ctx, kProfCholFinish);
+      kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
+                                                            S->finish, (int)S->n_finish, nullptr,
+                                                            ctx->counters + kCtrFinish, slots,
+                                                            ctx->bad_row, 1, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
   }
   return ALS_OK;
 }

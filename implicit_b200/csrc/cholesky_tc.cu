@@ -359,8 +359,10 @@ bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld) {
 }
 
 // items [0, n_items) of C->work that are whole rows (chunk items of giant rows are skipped: the caller runs the mma.sync
-// kernel over C->chunks); needs ctx->Greg, the cached weight range of C and max |y| in counters[kCtrYAbsMax]
-int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items, cudaStream_t stream) {
+// kernel over C->chunks); needs ctx->Greg, the weight range of the whole matrix (wmax_dev: C is one of its segments) and
+// max |y| in counters[kCtrYAbsMax]
+int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items,
+                       const unsigned *wmax_dev, cudaStream_t stream) {
   if (n_items <= 0) return ALS_OK;
   static bool attr_done = false;
   if (!attr_done) {
@@ -370,7 +372,7 @@ int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als
   const int grid = (int)std::min<int64_t>(n_items, ctx->sm_count);
   cholesky_tc_kernel<<<grid, kTcThreads, kTcSmem, stream>>>(
       C->indices, C->data, Y->d, X->d, C->row_offset, ctx->Greg, C->work, (int)n_items, ctx->bad_row, X->peers_dev, X->n_peers,
-      C->wmax_dev, reinterpret_cast<const unsigned *>(ctx->counters + kCtrYAbsMax));
+      wmax_dev, reinterpret_cast<const unsigned *>(ctx->counters + kCtrYAbsMax));
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   return ALS_OK;

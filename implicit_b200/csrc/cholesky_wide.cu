@@ -175,14 +175,17 @@ cholesky_wide_kernel(const int32_t *__restrict__ indices, const float *__restric
 __global__ void init_bad_row(long long *bad_row) { bad_row[0] = LLONG_MAX; }
 
 template <int T>
-int run_wide(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_factors *Y) {
+int run_wide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const als_factors *Y) {
   using C = WideCfg<T>;
   const int smem = C::SMEM_FLOATS * (int)sizeof(float);
   auto kern = cholesky_wide_kernel<T>;
   ALS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const std::vector<const als_csr *> segs = segments_of(Cw);  // row-block segments: bad_row is reset once per half
+  int64_t max_slots = 0;
+  for (const als_csr *S : segs) max_slots = std::max(max_slots, S->n_slots);
   float *slots = nullptr;
-  if (Cm->n_slots) {
-    int rc = ensure_scratch(ctx, (int64_t)Cm->n_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
+  if (max_slots) {
+    int rc = ensure_scratch(ctx, max_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
     if (rc != ALS_OK) return rc;
     slots = (float *)ctx->scratch;
   }
@@ -190,21 +193,23 @@ int run_wide(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_factors 
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   const int per_sm = std::max(1, (227 * 1024) / (smem + 1024));
-  if (Cm->n_work) {
-    const int grid = (int)std::min<int64_t>(Cm->n_work, (int64_t)ctx->sm_count * per_sm);
-    ProfScope prof(ctx, kProfCholesky);
-    kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg, Cm->work,
-                                                    (int)Cm->n_work, slots, ctx->bad_row, 0, X->peers_dev, X->n_peers);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  if (Cm->n_finish) {
-    const int grid = (int)std::min<int64_t>(Cm->n_finish, (int64_t)ctx->sm_count * per_sm);
-    ProfScope prof(ctx, kProfCholFinish);
-    kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
-                                                    Cm->finish, (int)Cm->n_finish, slots, ctx->bad_row, 1, X->peers_dev, X->n_peers);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
+  for (const als_csr *Cm : segs) {
+    if (Cm->n_work) {
+      const int grid = (int)std::min<int64_t>(Cm->n_work, (int64_t)ctx->sm_count * per_sm);
+      ProfScope prof(ctx, kProfCholesky);
+      kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg, Cm->work,
+                                                      (int)Cm->n_work, slots, ctx->bad_row, 0, X->peers_dev, X->n_peers);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
+    if (Cm->n_finish) {
+      const int grid = (int)std::min<int64_t>(Cm->n_finish, (int64_t)ctx->sm_count * per_sm);
+      ProfScope prof(ctx, kProfCholFinish);
+      kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
+                                                      Cm->finish, (int)Cm->n_finish, slots, ctx->bad_row, 1, X->peers_dev, X->n_peers);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
   }
   return ALS_OK;
 }

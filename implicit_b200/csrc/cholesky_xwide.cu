@@ -368,7 +368,7 @@ __global__ void xwide_init_bad_row(long long *bad_row) {
 
 }  // namespace
 
-int launch_cholesky_xwide(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_factors *Y) {
+int launch_cholesky_xwide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const als_factors *Y) {
   if (Y->ld > 1024 || Y->ld % 64) {
     set_error("cholesky: padded factors %d out of range", Y->ld);
     return ALS_E_INVALID;
@@ -385,39 +385,47 @@ int launch_cholesky_xwide(als_ctx *ctx, const als_csr *Cm, als_factors *X, const
     return ALS_E_CUDA;
   }
   const int64_t max_grid = (int64_t)ctx->sm_count * per_sm;
-  const int grid0 = (int)std::min<int64_t>(Cm->n_work, max_grid);
-  const int grid1 = (int)std::min<int64_t>(Cm->n_finish, max_grid);
-  // one scratch block: the giant-row slots, then one workspace per resident CTA
-  const int64_t n_ws = std::max(grid0, grid1);
+  // row-block segments run one after the other: the scratch covers the largest, bad_row is reset once per half
+  const std::vector<const als_csr *> segs = segments_of(Cw);
+  int64_t max_slots = 0, n_ws = 0;
+  for (const als_csr *S : segs) {
+    max_slots = std::max(max_slots, S->n_slots);
+    // one scratch block: the giant-row slots, then one workspace per resident CTA
+    n_ws = std::max(n_ws, std::min<int64_t>(std::max(S->n_work, S->n_finish), max_grid));
+  }
   // (n_slots + n_ws) * wsf floats: 2.2 MB per giant-row chunk and per workspace at 1024 factors
-  const int64_t bytes = (Cm->n_slots + n_ws) * wsf * (int64_t)sizeof(float);
+  const int64_t bytes = (max_slots + n_ws) * wsf * (int64_t)sizeof(float);
   int rc = ensure_scratch(ctx, bytes);
   if (rc != ALS_OK) {
     set_error("cholesky: factors=%d needs %.2f GB of device scratch (%lld giant-row chunks and %lld workspaces of %.2f MB "
               "each) and the allocation failed; split the rows into smaller calls or use the CG solver",
-              Y->f, bytes / 1e9, (long long)Cm->n_slots, (long long)n_ws, wsf * 4 / 1e6);
+              Y->f, bytes / 1e9, (long long)max_slots, (long long)n_ws, wsf * 4 / 1e6);
     return rc;
   }
   float *slots = (float *)ctx->scratch;
-  float *workspaces = slots + Cm->n_slots * wsf;
+  float *workspaces = slots + max_slots * wsf;
   xwide_init_bad_row<<<1, 1, 0, ctx->stream>>>(ctx->bad_row);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
-  if (Cm->n_work) {
-    ProfScope prof(ctx, kProfCholesky);
-    kern<<<grid0, kXwThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Y->ld, nt, Cm->row_offset, ctx->Greg,
-                                                   Cm->work, (int)Cm->n_work, slots, workspaces, ctx->bad_row, 0,
-                                                   X->peers_dev, X->n_peers);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  if (Cm->n_finish) {
-    ProfScope prof(ctx, kProfCholFinish);
-    kern<<<grid1, kXwThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Y->ld, nt, Cm->row_offset, ctx->Greg,
-                                                   Cm->finish, (int)Cm->n_finish, slots, workspaces, ctx->bad_row, 1,
-                                                   X->peers_dev, X->n_peers);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
+  for (const als_csr *Cm : segs) {
+    const int grid0 = (int)std::min<int64_t>(Cm->n_work, max_grid);
+    const int grid1 = (int)std::min<int64_t>(Cm->n_finish, max_grid);
+    if (Cm->n_work) {
+      ProfScope prof(ctx, kProfCholesky);
+      kern<<<grid0, kXwThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Y->ld, nt, Cm->row_offset, ctx->Greg,
+                                                     Cm->work, (int)Cm->n_work, slots, workspaces, ctx->bad_row, 0,
+                                                     X->peers_dev, X->n_peers);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
+    if (Cm->n_finish) {
+      ProfScope prof(ctx, kProfCholFinish);
+      kern<<<grid1, kXwThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Y->ld, nt, Cm->row_offset, ctx->Greg,
+                                                     Cm->finish, (int)Cm->n_finish, slots, workspaces, ctx->bad_row, 1,
+                                                     X->peers_dev, X->n_peers);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
   }
   return ALS_OK;
 }

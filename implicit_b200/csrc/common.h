@@ -1,6 +1,7 @@
 // Internal declarations shared by the translation units of libals_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -60,6 +61,8 @@ struct als_knobs {
   int gramian_fma = 0;        // ALS_B200_GRAMIAN_FMA: fp32 FMA Gramian instead of the wgmma one (64 padded factors)
   int long_tc = 0;            // ALS_B200_LONG_TC: experimental wgmma kernel for the long rows of a Cholesky half (cholesky_tc.cu)
   int cg_nv = 2;              // ALS_B200_CG_NV: float4 words per lane of the CG kernel (1 / 2 / 4)
+  int64_t segment_nnz = 0;    // ALS_B200_SEGMENT_NNZ: nonzeros per row-block segment of a device CSR; 0: automatic (one
+                              // segment below 2^31 - 1 nonzeros, else segments of at most 2^30).  Changes no bit.
 };
 
 struct als_ctx {
@@ -164,6 +167,12 @@ struct als_csr {
   int64_t n_slots = 0;
   als::WorkItem *chunks = nullptr;  // the n_slots chunk items in slot order (CG walks them pass by pass)
   int32_t *chunk_owner = nullptr;   // chunk -> index of its row in `finish`
+  // A CSR above the segment cap is a list of row-block segments, each an ordinary int32 CSR of whole rows: its own
+  // rebased indptr (in seg_indptr), indices / data offset into this CSR's arrays, its own schedule, row_offset = its
+  // first row.  The segments are non-owning children destroyed with this CSR; its own indptr and schedule stay empty,
+  // and wmax_dev, has_neg_w and max_row_nnz cover all segments.  Empty: one segment, the CSR itself.
+  std::vector<als_csr *> segs;
+  int32_t *seg_indptr = nullptr;  // the segments' indptrs, concatenated (rows + segs.size() entries)
 };
 
 namespace als {
@@ -198,6 +207,22 @@ int ensure_scratch(als_ctx *ctx, int64_t bytes);
 int ensure_device_buffer(als_ctx *ctx, void **buf, int64_t *cap, int64_t bytes);
 int ensure_pinned(als_ctx *ctx, int64_t bytes);
 int build_schedule(als_ctx *ctx, als_csr *csr, const int32_t *indptr_host);
+// the segments a solve walks: the CSR itself, or its row-block segments in row order
+static inline std::vector<const als_csr *> segments_of(const als_csr *c) {
+  if (c->segs.empty()) return {c};
+  return std::vector<const als_csr *>(c->segs.begin(), c->segs.end());
+}
+// the largest segment: the knob, else 2^30 (2x headroom on the kernels' int32 positions)
+static inline int64_t segment_cap(const als_ctx *ctx) { return ctx->knobs.segment_nnz > 0 ? ctx->knobs.segment_nnz : (int64_t)1 << 30; }
+// a CSR of nnz nonzeros is held as segments: above the knob when it is set, else from 2^31 - 1 nonzeros on
+static inline bool needs_segments(const als_ctx *ctx, int64_t nnz) {
+  return ctx->knobs.segment_nnz > 0 ? nnz > ctx->knobs.segment_nnz : nnz >= (int64_t)INT32_MAX;
+}
+// Cuts `p` (rows, cols, nnz, row_offset, indices and data set) into segments of at most segment_cap nonzeros.
+// ip[0 .. rows]: the host indptr as positions into p->indices / p->data.  Builds every segment's schedule.
+int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip);
+// the indptr of any CSR as 64-bit positions relative to its first nonzero (synchronises)
+int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out);
 int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
 // synthetic inputs generated on the device (gen.cu)
 int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t nnz_target, uint64_t seed, als_csr **out);
@@ -212,7 +237,8 @@ int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const a
 int launch_cholesky_xwide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);  // 128 < ld <= 1024
 // long rows on the wgmma tensor cores (cholesky_tc.cu): 64 padded factors, no weights |c| - 1 < 0
 bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld);
-int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items, cudaStream_t stream);
+int launch_cholesky_tc(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int64_t n_items,
+                       const unsigned *wmax_dev, cudaStream_t stream);
 // short-row path (cholesky_short.cu).  prepare: P and W from ctx->Greg and Y.  launch: items [begin, n_work) of
 // C->work, all of at most `max_len` nonzeros; whatever it cannot take lands in ctx->deferred / counters[kCtrDeferredCount].
 int short_rows_prepare(als_ctx *ctx, const als_factors *Y, cudaStream_t stream);

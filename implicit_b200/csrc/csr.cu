@@ -7,6 +7,9 @@
 // exactly scipy's canonical result, deterministically.  The radix sort is CUB's (toolkit library
 // code; this is one-time input preparation, not the per-iteration hot path).
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include <algorithm>
 
 #include "common.h"
 
@@ -50,7 +53,200 @@ __global__ void indptr_from_sorted_kernel(const int32_t *__restrict__ sorted_col
   out_indptr[c] = (int32_t)lo;
 }
 
+// ---- the transpose of a CSR held as row-block segments -----------------------------------------------------------
+// Peak memory: input + output + O(piece).  Output positions are 64-bit: a column histogram over all segments, scanned
+// into the output indptr, gives every column its range; the input is then sorted in row pieces of bounded nnz, in row
+// order, each piece stably by column, and every entry goes to out_indptr[c] + (entries of column c in earlier pieces)
+// + (its rank within the piece's column c).  Pieces in row order and stable sorts keep scipy's order exactly.
+constexpr int64_t kPieceNnz = int64_t(1) << 28;
+
+__global__ void column_histogram_kernel(const int32_t *__restrict__ indices, int64_t n, unsigned long long *count) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) atomicAdd(count + indices[i], 1ull);
+}
+
+__device__ __forceinline__ int64_t first_of_key(const int32_t *__restrict__ keys, int64_t n, int32_t c) {
+  int64_t lo = 0, hi = n;  // first j with keys[j] >= c
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (keys[mid] < c) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// sorted entry j of a piece (perm[j]: its position after the piece's first nonzero, keys[j]: its column) -> its place
+// in the output.  indptr: the piece's rows in the segment's indptr (indptr[0] is the piece's first nonzero).
+__global__ void scatter_piece_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ keys, int64_t n,
+                                     const int32_t *__restrict__ indptr, int rows, int64_t row0,
+                                     const float *__restrict__ data, const long long *__restrict__ next,
+                                     int32_t *__restrict__ out_indices, float *__restrict__ out_data) {
+  int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int32_t base = indptr[0];
+  for (; j < n; j += stride) {
+    const int32_t e = perm[j], c = keys[j];
+    int lo = 0, hi = rows;  // largest r with indptr[r] - base <= e
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (indptr[mid] - base <= e) lo = mid; else hi = mid;
+    }
+    const int64_t dst = next[c] + (j - first_of_key(keys, n, c));
+    out_indices[dst] = (int32_t)(row0 + lo);
+    out_data[dst] = data[e];
+  }
+}
+
+// after a piece: next[c] += its entries of column c (the last entry of each run of equal keys adds the run length)
+__global__ void advance_columns_kernel(const int32_t *__restrict__ keys, int64_t n, long long *next) {
+  int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; j < n; j += stride) {
+    const int32_t c = keys[j];
+    if (j + 1 < n && keys[j + 1] == c) continue;
+    next[c] += j - first_of_key(keys, n, c) + 1;
+  }
+}
+
+int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
+  const int64_t cols = in->cols;
+  int end_bit = 1;
+  while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
+  long long *count = nullptr, *out_ip = nullptr;
+  int rc;
+  if ((rc = dev_alloc(ctx, (void **)&count, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
+  if ((rc = dev_alloc(ctx, (void **)&out_ip, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
+  ALS_CUDA(cudaMemsetAsync(count, 0, sizeof(long long) * (cols + 1), ctx->stream));
+  const std::vector<const als_csr *> segs = segments_of(in);
+  for (const als_csr *S : segs) {
+    if (!S->nnz) continue;
+    column_histogram_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(S->indices, S->nnz, (unsigned long long *)count);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  {
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    ALS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count, out_ip, (int)(cols + 1), ctx->stream));
+    if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+    ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, count, out_ip, (int)(cols + 1), ctx->stream));
+    dev_free(ctx, tmp);
+  }
+  std::vector<int64_t> ip((size_t)cols + 1);
+  ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaMemcpyAsync(count, out_ip, sizeof(long long) * (cols + 1), cudaMemcpyDeviceToDevice, ctx->stream));  // next[c]
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  dev_free(ctx, out_ip);
+  // pieces: whole rows of one segment, at most kPieceNnz nonzeros unless a single row is longer
+  struct Piece { const als_csr *S; int64_t r0, r1, b0, n; };
+  std::vector<Piece> pieces;
+  int64_t max_piece = 0;
+  for (const als_csr *S : segs) {
+    std::vector<int32_t> sip((size_t)S->rows + 1);
+    ALS_CUDA(cudaMemcpy(sip.data(), S->indptr, sizeof(int32_t) * (S->rows + 1), cudaMemcpyDeviceToHost));
+    for (int64_t a = 0; a < S->rows;) {
+      int64_t b = std::upper_bound(sip.begin() + a + 1, sip.end(), (int64_t)sip[a] + kPieceNnz) - sip.begin() - 1;
+      b = std::max(b, a + 1);
+      pieces.push_back(Piece{S, a, b, sip[a], (int64_t)sip[b] - sip[a]});
+      max_piece = std::max(max_piece, pieces.back().n);
+      a = b;
+    }
+  }
+  if (max_piece > 0) {
+    int32_t *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, segs[0]->indices, keys_out, vals_in, vals_out, (int)max_piece,
+                                             0, end_bit, ctx->stream));
+    if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
+        (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * max_piece)) != ALS_OK ||
+        (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
+        (rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK)
+      return rc;
+    iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, max_piece);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    for (const Piece &pc : pieces) {
+      const int64_t b0 = pc.b0, n = pc.n;
+      if (n == 0) continue;
+      ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pc.S->indices + b0, keys_out, vals_in, vals_out, (int)n, 0,
+                                               end_bit, ctx->stream));
+      scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
+          vals_out, keys_out, n, pc.S->indptr + pc.r0, (int)(pc.r1 - pc.r0), pc.S->row_offset - in->row_offset + pc.r0,
+          pc.S->data + b0, count, t->indices, t->data);
+      ALS_CUDA(cudaGetLastError());
+      advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, n, count);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches += 2;
+    }
+    dev_free(ctx, keys_out);  // stream ordered: after the kernels above
+    dev_free(ctx, vals_in);
+    dev_free(ctx, vals_out);
+    dev_free(ctx, tmp);
+  }
+  dev_free(ctx, count);
+  // the output's segments and their schedules are built right away (no lazy schedule for a segmented transpose)
+  return make_segments(ctx, t, ip.data());
+}
+
 }  // namespace
+
+int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip) {
+  const int64_t cap = segment_cap(ctx), rows = p->rows;
+  std::vector<int64_t> starts;
+  for (int64_t a = 0; a < rows || starts.empty();) {
+    starts.push_back(a);
+    if (a >= rows) break;
+    // the most whole rows that fit the cap, and at least one
+    int64_t b = std::upper_bound(ip + a + 1, ip + rows + 1, ip[a] + cap) - ip - 1;
+    b = std::max(b, a + 1);
+    if (ip[b] - ip[a] >= (int64_t)INT32_MAX) {
+      set_error("CSR row %lld holds %lld nonzeros: a row is limited to 2^31 - 2", (long long)a, (long long)(ip[b] - ip[a]));
+      return ALS_E_INVALID;
+    }
+    a = b;
+  }
+  const int64_t nseg = (int64_t)starts.size();
+  starts.push_back(rows);
+  std::vector<int32_t> cat((size_t)(rows + nseg));
+  for (int64_t s = 0; s < nseg; ++s)
+    for (int64_t r = starts[s]; r <= starts[s + 1]; ++r) cat[r + s] = (int32_t)(ip[r] - ip[starts[s]]);
+  int rc = dev_alloc(ctx, (void **)&p->seg_indptr, sizeof(int32_t) * (rows + nseg));
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(p->seg_indptr, cat.data(), sizeof(int32_t) * cat.size(), cudaMemcpyHostToDevice, ctx->stream));
+  p->max_row_nnz = 0;
+  for (int64_t s = 0; s < nseg; ++s) {
+    const int64_t a = starts[s], b = starts[s + 1];
+    als_csr *c = new als_csr();
+    c->ctx = ctx;
+    c->rows = b - a;
+    c->cols = p->cols;
+    c->nnz = ip[b] - ip[a];
+    c->row_offset = p->row_offset + a;
+    c->owns = false;
+    c->indptr = p->seg_indptr + a + s;
+    c->indices = p->indices + ip[a];
+    c->data = p->data + ip[a];
+    p->segs.push_back(c);
+    if ((rc = build_schedule(ctx, c, cat.data() + a + s)) != ALS_OK) return rc;
+    p->max_row_nnz = std::max(p->max_row_nnz, c->max_row_nnz);
+  }
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `cat` dies here
+  return ALS_OK;
+}
+
+int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out) {
+  out.assign((size_t)c->rows + 1, 0);
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  std::vector<int32_t> ip;
+  for (const als_csr *S : segments_of(c)) {
+    ip.resize((size_t)S->rows + 1);
+    ALS_CUDA(cudaMemcpy(ip.data(), S->indptr, sizeof(int32_t) * ip.size(), cudaMemcpyDeviceToHost));
+    const int64_t r0 = S->row_offset - c->row_offset, base = S->indices - c->indices;
+    for (int64_t r = 0; r <= S->rows; ++r) out[r0 + r] = base + ip[r];
+  }
+  return ALS_OK;
+}
 
 int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   *out = nullptr;
@@ -67,6 +263,16 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   t->cols = rows;
   t->nnz = nnz;
   int rc;
+  if (!in->segs.empty() || needs_segments(ctx, nnz)) {
+    if ((rc = dev_alloc(ctx, (void **)&t->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+        (rc = dev_alloc(ctx, (void **)&t->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+        (rc = transpose_segmented(ctx, in, t)) != ALS_OK) {
+      als_csr_destroy(t);
+      return rc;
+    }
+    *out = t;
+    return ALS_OK;
+  }
   if ((rc = dev_alloc(ctx, (void **)&t->indptr, sizeof(int32_t) * ((int64_t)cols + 1))) != ALS_OK ||
       (rc = dev_alloc(ctx, (void **)&t->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
       (rc = dev_alloc(ctx, (void **)&t->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK) {

@@ -49,6 +49,24 @@ def power_law_csr(users, items, nnz_target, seed, negative_fraction=0.0):
     return sp.csr_matrix((data, col, indptr), shape=(users, items))
 
 
+def block_diagonal_tiling(base, R):
+    """R copies of `base` on the diagonal: block r holds users r U_b ... and items r I_b ....  Index arrays are int64
+    once the result passes 2^31 nonzeros, as scipy builds them; filled block by block without temporaries of the
+    whole size (the large-CSR test and tools/large_csr_bench.py: beyond 2^31 nonzeros at a few minutes of host time)."""
+    Ub, Ib = base.shape
+    nb = base.nnz
+    idx = np.int64 if R * nb >= 2**31 else np.int32
+    indices = np.empty(R * nb, dtype=idx)
+    indptr = np.empty(R * Ub + 1, dtype=idx)
+    ip = base.indptr.astype(np.int64)
+    for r in range(R):
+        indices[r * nb:(r + 1) * nb] = base.indices
+        indices[r * nb:(r + 1) * nb] += r * Ib
+        indptr[r * Ub:(r + 1) * Ub] = ip[:-1] + r * nb
+    indptr[-1] = R * nb
+    return sp.csr_matrix((np.tile(base.data, R), indices, indptr), shape=(R * Ub, R * Ib))
+
+
 def initial_factors(users, items, factors, seed=42):
     """Same distribution as implicit/cpu/als.py:144-147: rng.random((n, f), float32) * 0.01."""
     rng = np.random.default_rng(seed)
