@@ -44,6 +44,11 @@ SIGNATURES = {
     "als_host_free": (c_int, [c_void_p]),
     "als_csr_upload": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_void_p, c_i64, P(c_void_p)]),
     "als_csr_upload64": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_int, c_void_p, c_i64, P(c_void_p)]),
+    "als_csr_upload_host64": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_int, c_void_p, c_i64,
+                                      P(c_void_p)]),
+    "als_csr_is_host": (c_int, [c_void_p, P(c_int)]),
+    "als_mem_info": (c_int, [c_void_p, P(c_i64), P(c_i64)]),
+    "als_ctx_get_knob": (c_int, [c_void_p, ctypes.c_char_p, P(c_int)]),
     "als_csr_segment_count": (c_int, [c_void_p, P(c_i64)]),
     "als_csr_download64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "als_csr_transpose": (c_int, [c_void_p, c_void_p, P(c_void_p)]),
@@ -167,8 +172,20 @@ class Context:
         check(self.lib.als_sync(self.h))
 
     def set_knob(self, name, value):
-        """Measurement knobs (short_max, short_serial, whiten_fma, gramian_fma, topk_legacy, cg_nv); see include/als_b200.h."""
+        """Measurement knobs (short_max, short_serial, whiten_fma, gramian_fma, topk_legacy, cg_nv, segment_nnz,
+        host_csr); see include/als_b200.h."""
         check(self.lib.als_ctx_set_knob(self.h, name.encode(), int(value)))
+
+    def get_knob(self, name):
+        v = c_int()
+        check(self.lib.als_ctx_get_knob(self.h, name.encode(), ctypes.byref(v)))
+        return v.value
+
+    def mem_info(self):
+        """(free, total) device bytes; blocks the context's memory pool keeps for reuse count as free."""
+        free, total = c_i64(), c_i64()
+        check(self.lib.als_mem_info(self.h, ctypes.byref(free), ctypes.byref(total)))
+        return free.value, total.value
 
     def info(self):
         name = ctypes.create_string_buffer(256)
@@ -297,25 +314,57 @@ def csr_upload_route(nnz):
     return "int32" if nnz <= INT32_CSR_MAX_NNZ else "int64"
 
 
+#: the segment cap of a host-resident CSR (the default of als_csr_upload_host64): its two-slot device ring takes 4 GB
+HOST_SEGMENT_NNZ = 2**28
+
+
+def _padded_factors(factors):
+    return -(-factors // 16) * 16 if factors <= 128 else -(-factors // 128) * 128
+
+
+def csr_residency(users, items, nnz, factors, free_bytes):
+    """Where fit() keeps the pair Cui / Ciu: "device" when everything a device-resident fit allocates fits in
+    `free_bytes` of device memory, else "host" (page-locked host memory, streamed through the device per segment).
+
+    Counted: both orientations (int32 index + fp32 value per nonzero, each), the transpose's temporaries (three int32
+    arrays and the radix sort's two alternate buffers over the whole matrix, or over one 2^28-nonzero piece when it is
+    segmented), the indptrs and launch schedules of both (20 bytes per row, 16 per column count), the factor matrices
+    X and Y and the solver's two whitened copies of the larger one, plus 1 GiB for scratch and the pool's
+    fragmentation."""
+    users, items, nnz, factors = int(users), int(items), int(nnz), int(factors)
+    ld = _padded_factors(factors)
+    both = 2 * 8 * nnz
+    piece = nnz if nnz <= INT32_CSR_MAX_NNZ else min(nnz, HOST_SEGMENT_NNZ)
+    transpose = 20 * piece + 16 * (items + 1) * 2
+    rows = 20 * (users + items)
+    dense = 4 * ld * (users + items) + 2 * 4 * ld * max(users, items)
+    need = both + transpose + rows + dense + (1 << 30)
+    return "device" if need <= int(free_bytes) else "host"
+
+
 class DeviceCSR:
     """als_csr: a CSR (or a row shard of one) resident on the device with its launch schedule.  A CSR with more
-    nonzeros than the segment cap is held as row-block segments of int32 positions; every call takes it as it is."""
+    nonzeros than the segment cap is held as row-block segments of int32 positions; every call takes it as it is.
+    A host-resident CSR (upload(..., host=True)) keeps its indices / values in page-locked host memory and streams
+    them through the device segment by segment, with bitwise the results of the device layout of the same cap."""
 
     def __init__(self, ctx, handle, parent=None):
         self.ctx, self.h, self._parent = ctx, handle, parent
 
     @classmethod
-    def upload(cls, ctx, m, row_offset=0, rows=None):
-        """m: scipy.sparse.csr_matrix (any float dtype; values are cast to float32)."""
+    def upload(cls, ctx, m, row_offset=0, rows=None, host=False):
+        """m: scipy.sparse.csr_matrix (any float dtype; values are cast to float32).  host: keep it host-resident
+        (als_csr_upload_host64)."""
         data = np.ascontiguousarray(m.data, dtype=np.float32)
         h = c_void_p()
-        if csr_upload_route(m.nnz) == "int64":
+        if host or csr_upload_route(m.nnz) == "int64":
             indptr = np.ascontiguousarray(m.indptr, dtype=np.int64)
             indices = m.indices
             if indices.dtype not in (np.int32, np.int64) or not indices.flags.c_contiguous:
                 indices = np.ascontiguousarray(indices, dtype=np.int64)
-            check(ctx.lib.als_csr_upload64(ctx.h, m.shape[0], m.shape[1], m.nnz, ptr(indptr), ptr(indices),
-                                           indices.dtype.itemsize, ptr(data), int(row_offset), ctypes.byref(h)))
+            upload = ctx.lib.als_csr_upload_host64 if host else ctx.lib.als_csr_upload64
+            check(upload(ctx.h, m.shape[0], m.shape[1], m.nnz, ptr(indptr), ptr(indices), indices.dtype.itemsize,
+                         ptr(data), int(row_offset), ctypes.byref(h)))
             return cls(ctx, h)
         indptr = m.indptr
         if indptr.dtype != np.int32:
@@ -332,6 +381,13 @@ class DeviceCSR:
         n = c_i64()
         check(self.ctx.lib.als_csr_segment_count(self.h, ctypes.byref(n)))
         return n.value
+
+    @property
+    def host_resident(self):
+        """True when indices / values live in page-locked host memory (als_csr_upload_host64 or its transpose)."""
+        v = c_int()
+        check(self.ctx.lib.als_csr_is_host(self.h, ctypes.byref(v)))
+        return bool(v.value)
 
     def transpose(self):
         h = c_void_p()

@@ -173,7 +173,13 @@ class AlternatingLeastSquares:
         ctx = self.ctx
 
         s = time.time()
-        Cui = _lib.DeviceCSR.upload(ctx, Cui_host)
+        # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a single-GPU
+        # fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise the same
+        host = False
+        if self.process_group is None:
+            host = bool(ctx.get_knob("host_csr")) or \
+                _lib.csr_residency(users, items, Cui_host.nnz, self.factors, ctx.mem_info()[0]) == "host"
+        Cui = _lib.DeviceCSR.upload(ctx, Cui_host, host=host)
         if self.alpha != 1.0:
             Cui.scale(self.alpha)  # cpu/als.py:133-134, on device
         Ciu = Cui.transpose()      # cpu/als.py:137, on device

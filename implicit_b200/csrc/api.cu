@@ -163,10 +163,30 @@ static int h2d_copy(als_ctx *ctx, void *dst, const void *src, size_t bytes) {
   });
 }
 
+// The staging threads of staged_h2d writing straight into a page-locked host array instead (a host-resident CSR): the
+// same chunks, the same fill, no DMA.
+static int staged_fill_host(void *dst, size_t bytes, const StageFill &fill) {
+  const size_t nchunks = (bytes + kStageChunk - 1) / kStageChunk;
+  std::atomic<bool> refused{false};
+  std::vector<std::thread> pool;
+  for (int t = 0; t < kStageThreads; ++t) {
+    pool.emplace_back([=, &refused, &fill]() {
+      for (size_t c = t; c < nchunks && !refused; c += kStageThreads) {
+        const size_t off = c * kStageChunk, len = std::min(kStageChunk, bytes - off);
+        if (!fill((char *)dst + off, off, len)) refused = true;
+      }
+    });
+  }
+  for (auto &th : pool) th.join();
+  return refused ? ALS_E_INVALID : ALS_OK;
+}
+
 // n column indices (int32 or int64 on the host) -> int32 on the device, narrowed chunk by chunk in the staging threads
 // (no host-side int32 copy of the whole array, half the PCIe bytes of int64).  Every index must lie in [0, cols): the
-// first one that does not is reported in *bad_at (else -1) and the call returns ALS_E_INVALID.
-static int h2d_indices(als_ctx *ctx, int32_t *dst, const void *src, int index_bytes, int64_t n, int64_t cols, int64_t *bad_at) {
+// first one that does not is reported in *bad_at (else -1) and the call returns ALS_E_INVALID.  host: dst is a
+// page-locked host array (a host-resident CSR), written by the same threads.
+static int h2d_indices(als_ctx *ctx, int32_t *dst, const void *src, int index_bytes, int64_t n, int64_t cols, int64_t *bad_at,
+                       bool host = false) {
   *bad_at = -1;
   if (n == 0) return ALS_OK;
   std::atomic<int64_t> bad{INT64_MAX};
@@ -195,8 +215,30 @@ static int h2d_indices(als_ctx *ctx, int32_t *dst, const void *src, int index_by
     }
     return false;
   };
-  const int rc = staged_h2d(ctx, dst, (size_t)n * sizeof(int32_t), narrow);
+  const int rc = host ? staged_fill_host(dst, (size_t)n * sizeof(int32_t), narrow)
+                      : staged_h2d(ctx, dst, (size_t)n * sizeof(int32_t), narrow);
   if (rc == ALS_E_INVALID) *bad_at = bad.load();
+  return rc;
+}
+
+// n values -> a page-locked host array in the staging threads, folding the weight range of csr_wmax_kernel on the way
+static int fill_host_values(float *dst, const float *src, int64_t n, unsigned *wmax_bits, bool *neg) {
+  std::atomic<unsigned> m{0};
+  std::atomic<bool> ng{false};
+  const int rc = staged_fill_host(dst, (size_t)n * sizeof(float), [&](char *out, size_t off, size_t len) {
+    const float *in = src + off / 4;
+    memcpy(out, in, len);
+    unsigned cm;
+    bool cn;
+    host_wmax(in, (int64_t)(len / 4), &cm, &cn);
+    unsigned cur = m.load();
+    while (cm > cur && !m.compare_exchange_weak(cur, cm)) {
+    }
+    if (cn) ng = true;
+    return true;
+  });
+  *wmax_bits = m.load();
+  *neg = ng.load();
   return rc;
 }
 
@@ -356,7 +398,7 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
     struct { const char *env; const char *name; } table[] = {
         {"ALS_B200_SHORT_MAX", "short_max"}, {"ALS_B200_SHORT_SERIAL", "short_serial"}, {"ALS_B200_WHITEN_FMA", "whiten_fma"},
         {"ALS_B200_GRAMIAN_FMA", "gramian_fma"}, {"ALS_B200_TOPK_LEGACY", "topk_legacy"}, {"ALS_B200_LONG_TC", "long_tc"}, {"ALS_B200_CG_NV", "cg_nv"},
-        {"ALS_B200_SEGMENT_NNZ", "segment_nnz"}};
+        {"ALS_B200_SEGMENT_NNZ", "segment_nnz"}, {"ALS_B200_HOST_CSR", "host_csr"}};
     for (const auto &t : table) {
       const char *e = getenv(t.env);
       if (!e) continue;
@@ -383,6 +425,10 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->sched_ev, cudaEventDisableTiming));
+  for (int k = 0; k < 2; ++k) {
+    ALS_CUDA(cudaEventCreateWithFlags(&ctx->ring_loaded[k], cudaEventDisableTiming));
+    ALS_CUDA(cudaEventCreateWithFlags(&ctx->ring_free[k], cudaEventDisableTiming));
+  }
   {
     cudaMemPool_t pool;
     ALS_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
@@ -424,8 +470,28 @@ ALS_API int als_ctx_set_knob(als_ctx *ctx, const char *name, int value) {
   } else if (!strcmp(name, "segment_nnz")) {
     ALS_REQUIRE(value >= 0 && value < INT32_MAX, "als_ctx_set_knob: segment_nnz must be in [0, 2^31 - 1)");
     k.segment_nnz = value;
-  } else {
+  } else if (!strcmp(name, "host_csr")) k.host_csr = value != 0;
+  else {
     set_error("als_ctx_set_knob: unknown knob '%s'", name);
+    return ALS_E_INVALID;
+  }
+  return ALS_OK;
+}
+
+ALS_API int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value) {
+  ALS_REQUIRE(ctx && name && value, "als_ctx_get_knob: NULL argument");
+  const als_knobs &k = ctx->knobs;
+  if (!strcmp(name, "short_max")) *value = k.short_max;
+  else if (!strcmp(name, "short_serial")) *value = k.short_serial;
+  else if (!strcmp(name, "whiten_fma")) *value = k.whiten_fma;
+  else if (!strcmp(name, "gramian_fma")) *value = k.gramian_fma;
+  else if (!strcmp(name, "topk_legacy")) *value = k.topk_legacy;
+  else if (!strcmp(name, "long_tc")) *value = k.long_tc;
+  else if (!strcmp(name, "cg_nv")) *value = k.cg_nv;
+  else if (!strcmp(name, "segment_nnz")) *value = (int)k.segment_nnz;
+  else if (!strcmp(name, "host_csr")) *value = k.host_csr;
+  else {
+    set_error("als_ctx_get_knob: unknown knob '%s'", name);
     return ALS_E_INVALID;
   }
   return ALS_OK;
@@ -463,6 +529,10 @@ ALS_API int als_ctx_destroy(als_ctx *ctx) {
   }
   if (ctx->sched_pinned) cudaFreeHost(ctx->sched_pinned);
   cudaEventDestroy(ctx->sched_ev);
+  for (int k = 0; k < 2; ++k) {
+    cudaEventDestroy(ctx->ring_loaded[k]);
+    cudaEventDestroy(ctx->ring_free[k]);
+  }
   for (int i = 0; i < 5; ++i) {
     if (ctx->class_stream[i]) cudaStreamDestroy(ctx->class_stream[i]);
     if (ctx->class_join[i]) cudaEventDestroy(ctx->class_join[i]);
@@ -498,6 +568,26 @@ ALS_API int als_device_info(als_ctx *ctx, char *name, int *sm_count, int64_t *l2
   if (l2_bytes) *l2_bytes = ctx->l2_bytes;
   if (mem_bytes) *mem_bytes = ctx->mem_bytes;
   return ALS_OK;
+}
+
+int als::mem_info(als_ctx *ctx, int64_t *free_bytes, int64_t *total_bytes) {
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // stream-ordered frees land in the pool
+  size_t fr = 0, tot = 0;
+  ALS_CUDA(cudaMemGetInfo(&fr, &tot));
+  cudaMemPool_t pool;
+  ALS_CUDA(cudaDeviceGetDefaultMemPool(&pool, ctx->device));
+  uint64_t reserved = 0, used = 0;
+  ALS_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved));
+  ALS_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used));
+  *free_bytes = (int64_t)fr + (int64_t)(reserved > used ? reserved - used : 0);
+  *total_bytes = (int64_t)tot;
+  return ALS_OK;
+}
+
+ALS_API int als_mem_info(als_ctx *ctx, int64_t *free_bytes, int64_t *total_bytes) {
+  ALS_REQUIRE(ctx && free_bytes && total_bytes, "als_mem_info: NULL argument");
+  return als::mem_info(ctx, free_bytes, total_bytes);
 }
 
 ALS_API int64_t als_launch_count(als_ctx *ctx) { return ctx ? ctx->launches : 0; }
@@ -641,17 +731,19 @@ ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz
   return ALS_OK;
 }
 
-ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
-                             const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  ALS_REQUIRE(ctx && out && indptr, "als_csr_upload64: NULL argument");
-  ALS_REQUIRE(index_bytes == 4 || index_bytes == 8, "als_csr_upload64: index_bytes must be 4 or 8, got %d", index_bytes);
-  ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "als_csr_upload64: negative shape");
-  ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "als_csr_upload64: rows and cols must be < 2^31 - 1");
-  ALS_REQUIRE(indptr[0] >= 0 && indptr[rows] - indptr[0] == nnz, "als_csr_upload64: indptr[rows] - indptr[0] = %lld != nnz = %lld",
+// als_csr_upload64 and als_csr_upload_host64: the same checks and refusals; host keeps indices / data in page-locked host
+// memory (always segmented) instead of uploading them
+static int csr_upload64(const char *who, bool host, als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
+                        const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+  ALS_REQUIRE(ctx && out && indptr, "%s: NULL argument", who);
+  ALS_REQUIRE(index_bytes == 4 || index_bytes == 8, "%s: index_bytes must be 4 or 8, got %d", who, index_bytes);
+  ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "%s: negative shape", who);
+  ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "%s: rows and cols must be < 2^31 - 1", who);
+  ALS_REQUIRE(indptr[0] >= 0 && indptr[rows] - indptr[0] == nnz, "%s: indptr[rows] - indptr[0] = %lld != nnz = %lld", who,
               (long long)(indptr[rows] - indptr[0]), (long long)nnz);
-  ALS_REQUIRE(nnz == 0 || (indices && data), "als_csr_upload64: indices/data NULL with nnz > 0");
+  ALS_REQUIRE(nnz == 0 || (indices && data), "%s: indices/data NULL with nnz > 0", who);
   for (int64_t r = 0; r < rows; ++r)
-    ALS_REQUIRE(indptr[r + 1] >= indptr[r], "als_csr_upload64: indptr is not monotone at row %lld", (long long)r);
+    ALS_REQUIRE(indptr[r + 1] >= indptr[r], "%s: indptr is not monotone at row %lld", who, (long long)r);
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
   als_csr *c = new als_csr();
@@ -660,16 +752,31 @@ ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t n
   c->cols = cols;
   c->nnz = nnz;
   c->row_offset = row_offset;
+  c->host = host;
   const int64_t base = indptr[0];  // a row shard arrives with indptr[0] != 0
   int rc;
   int64_t bad = -1;
-  if ((rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-      (rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad)) != ALS_OK ||
-      (rc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz)) != ALS_OK) {
+  unsigned wmax_bits = 0;
+  bool neg = false;
+  if (host) {
+    const size_t bytes = sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1);
+    cudaError_t e = cudaMallocHost((void **)&c->indices, bytes);
+    if (e == cudaSuccess) e = cudaMallocHost((void **)&c->data, bytes);
+    if (e != cudaSuccess) {
+      als_csr_destroy(c);
+      return cuda_fail(e, "cudaMallocHost (host-resident CSR)", __FILE__, __LINE__);
+    }
+    rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad, true);
+    if (rc == ALS_OK) rc = fill_host_values(c->data, data + base, nnz, &wmax_bits, &neg);
+  } else if ((rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) == ALS_OK &&
+             (rc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) == ALS_OK &&
+             (rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad)) == ALS_OK) {
+    rc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz);
+  }
+  if (rc != ALS_OK) {
     if (bad >= 0) {
       const int64_t v = index_bytes == 8 ? ((const int64_t *)indices)[base + bad] : ((const int32_t *)indices)[base + bad];
-      set_error("als_csr_upload64: indices[%lld] = %lld is outside [0, %lld)", (long long)(base + bad), (long long)v, (long long)cols);
+      set_error("%s: indices[%lld] = %lld is outside [0, %lld)", who, (long long)(base + bad), (long long)v, (long long)cols);
     }
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
     als_csr_destroy(c);
@@ -677,7 +784,9 @@ ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t n
   }
   std::vector<int64_t> ip((size_t)rows + 1);
   for (int64_t r = 0; r <= rows; ++r) ip[r] = indptr[r] - base;
-  if (needs_segments(ctx, nnz)) {
+  if (host) {
+    if ((rc = set_host_wmax(ctx, c, wmax_bits, neg)) == ALS_OK) rc = make_segments(ctx, c, ip.data());
+  } else if (needs_segments(ctx, nnz)) {
     rc = make_segments(ctx, c, ip.data());
   } else {
     std::vector<int32_t> ip32(ip.begin(), ip.end());
@@ -692,6 +801,22 @@ ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t n
     return rc;
   }
   *out = c;
+  return ALS_OK;
+}
+
+ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
+                             const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+  return csr_upload64("als_csr_upload64", false, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+}
+
+ALS_API int als_csr_upload_host64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
+                                  const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+  return csr_upload64("als_csr_upload_host64", true, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+}
+
+ALS_API int als_csr_is_host(const als_csr *csr, int *host) {
+  ALS_REQUIRE(csr && host, "als_csr_is_host: NULL argument");
+  *host = csr->host ? 1 : 0;
   return ALS_OK;
 }
 
@@ -726,6 +851,11 @@ ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int6
               (long long)r1);
   ALS_REQUIRE(in->row_offset == 0, "als_csr_slice_rows: cannot slice a shard");
   *out = nullptr;
+  if (in->host) {
+    set_error("als_csr_slice_rows: a host-resident CSR cannot be sliced into shards; upload it with als_csr_upload64 for a "
+              "multi-GPU fit");
+    return ALS_E_UNSUPPORTED;
+  }
   ALS_CUDA(cudaSetDevice(ctx->device));
   if (!in->segs.empty()) {  // a shard of a segmented CSR can itself exceed 2^31 nonzeros: a segmented view
     std::vector<int64_t> ip64;
@@ -774,9 +904,31 @@ ALS_API int als_csr_scale(als_ctx *ctx, als_csr *csr, float alpha) {
   ALS_REQUIRE(ctx && csr, "als_csr_scale: NULL argument");
   if (csr->nnz == 0) return ALS_OK;
   ALS_CUDA(cudaSetDevice(ctx->device));
-  csr->wmax_valid = false;
   // segments are consecutive blocks of one array: the first one starts the CSR's values
   float *data = csr->segs.empty() ? csr->data : csr->segs[0]->data;
+  if (csr->host) {
+    // the same single fp32 rounding as scale_kernel, in the page-locked array, once no queued copy reads it any more;
+    // the weight range is folded on the way
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    ALS_CUDA(cudaStreamSynchronize(ctx->copy));
+    std::atomic<unsigned> m{0};
+    std::atomic<bool> ng{false};
+    staged_fill_host(data, sizeof(float) * (size_t)csr->nnz, [&](char *out, size_t, size_t len) {
+      float *v = reinterpret_cast<float *>(out);
+      const int64_t n = (int64_t)(len / 4);
+      for (int64_t i = 0; i < n; ++i) v[i] *= alpha;
+      unsigned cm;
+      bool cn;
+      host_wmax(v, n, &cm, &cn);
+      unsigned cur = m.load();
+      while (cm > cur && !m.compare_exchange_weak(cur, cm)) {
+      }
+      if (cn) ng = true;
+      return true;
+    });
+    return set_host_wmax(ctx, csr, m.load(), ng.load());
+  }
+  csr->wmax_valid = false;
   scale_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(data, csr->nnz, alpha);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
@@ -829,6 +981,11 @@ ALS_API int als_csr_download64(als_ctx *ctx, const als_csr *csr, int64_t *indptr
   const int64_t base = ip[0];  // a row-slice view keeps absolute positions into its parent's arrays: rebase
   if (indptr)
     for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] = ip[r] - base;
+  if (csr->host) {  // the page-locked arrays themselves (csr_indptr64 synchronised the compute stream)
+    if (indices && csr->nnz) memcpy(indices, csr->indices + base, sizeof(int32_t) * csr->nnz);
+    if (data && csr->nnz) memcpy(data, csr->data + base, sizeof(float) * csr->nnz);
+    return ALS_OK;
+  }
   if (indices && csr->nnz)
     ALS_CUDA(cudaMemcpy(indices, csr->indices + base, sizeof(int32_t) * csr->nnz, cudaMemcpyDeviceToHost));
   if (data && csr->nnz)
@@ -847,7 +1004,13 @@ ALS_API int als_csr_destroy(als_csr *csr) {
     }
     // stream-ordered frees: everything queued so far on the compute stream (which every other stream is joined
     // into before an entry point returns) still sees the arrays
-    if (csr->owns) {
+    if (csr->owns && csr->host) {
+      // page-locked arrays: every copy out of them is queued on the copy stream and waited for by the compute stream
+      cudaStreamSynchronize(ctx->stream);
+      cudaStreamSynchronize(ctx->copy);
+      cudaFreeHost(csr->indices);
+      cudaFreeHost(csr->data);
+    } else if (csr->owns) {
       dev_free(ctx, csr->indptr);
       dev_free(ctx, csr->indices);
       dev_free(ctx, csr->data);
@@ -1238,13 +1401,16 @@ ALS_API int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors
   ALS_CUDA(cudaSetDevice(ctx->device));
   // per segment (launch_loss leaves X^T X of the segment's rows in the Gramian buffer): the terms are shard sums
   double sum[3] = {0.0, 0.0, 0.0};
-  for (const als_csr *S : segments_of(C)) {
+  rc = for_each_segment(ctx, C, [&](size_t, const als_csr *S) -> int {
     double t[3];
-    if ((rc = launch_gramian(ctx, Y)) != ALS_OK || (rc = launch_loss(ctx, S, X, Y, regularization, t)) != ALS_OK) return rc;
+    int lrc;
+    if ((lrc = launch_gramian(ctx, Y)) != ALS_OK || (lrc = launch_loss(ctx, S, X, Y, regularization, t)) != ALS_OK) return lrc;
     sum[0] += t[0];
     sum[1] += t[1];
     sum[2] = t[2];  // reg ||Y||^2: once
-  }
+    return ALS_OK;
+  });
+  if (rc != ALS_OK) return rc;
   for (int i = 0; i < 3; ++i) loss[i] = sum[i];
   return ALS_OK;
 }
@@ -1257,8 +1423,12 @@ ALS_API int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *
   ALS_REQUIRE(k >= 0 && n_query >= 0, "als_topk: negative k or n_query");
   ALS_REQUIRE(!liked || liked->rows == n_query, "als_topk: liked has %lld rows for %lld queries",
               liked ? (long long)liked->rows : 0LL, (long long)n_query);
-  ALS_REQUIRE(!liked || liked->segs.empty(), "als_topk: the liked CSR (%lld nonzeros) is held as segments; split the queries "
+  ALS_REQUIRE(!liked || liked->host || liked->segs.empty(), "als_topk: the liked CSR (%lld nonzeros) is held as segments; split the queries "
               "into calls whose liked rows hold fewer than 2^31 - 1 nonzeros", liked ? (long long)liked->nnz : 0LL);
+  if (liked && liked->host) {
+    set_error("als_topk: the liked CSR is host-resident; upload the filter with als_csr_upload or als_csr_upload64");
+    return ALS_E_UNSUPPORTED;
+  }
   ALS_REQUIRE(!liked || liked->cols == items->rows, "als_topk: liked has %lld columns for %lld items",
               liked ? (long long)liked->cols : 0LL, (long long)items->rows);
   ALS_CUDA(cudaSetDevice(ctx->device));

@@ -428,13 +428,10 @@ int launch_cg_segment(als_ctx *ctx, const als_csr *C, als_factors *X, const als_
 
 }  // namespace
 
-// rows are independent: a CSR of row-block segments is solved one segment after the other with the same Greg
+// rows are independent: a CSR of row-block segments is solved one segment after the other with the same Greg (streamed
+// through the device ring when C is host-resident; every CG launch is on ctx->stream)
 int launch_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, int cg_steps) {
-  for (const als_csr *S : segments_of(C)) {
-    int rc = launch_cg_segment(ctx, S, X, Y, cg_steps);
-    if (rc != ALS_OK) return rc;
-  }
-  return ALS_OK;
+  return for_each_segment(ctx, C, [&](size_t, const als_csr *S) { return launch_cg_segment(ctx, S, X, Y, cg_steps); });
 }
 
 }  // namespace als

@@ -302,6 +302,10 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     if (arc != ALS_OK) return arc;
   }
   if (!Cmut->wmax_valid) {
+    if (Cm->host) {  // kept valid on the host from the upload on: the segments' values are not on the device here
+      set_error("cholesky: host-resident CSR without its weight range");
+      return ALS_E_INVALID;
+    }
     ALS_CUDA(cudaMemsetAsync(Cmut->wmax_dev, 0, 2 * sizeof(unsigned), ctx->stream));
     for (const als_csr *S : segs) {
       csr_wmax_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(S->indptr, S->rows, S->data, Cmut->wmax_dev);
@@ -332,8 +336,9 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     if (n_short * 16 < Y->rows) short_max = 0;
   }
   const int max_grid = ctx->sm_count * ctas_per_sm;
-  for (size_t s = 0; s < segs.size(); ++s) {
-    const als_csr *S = segs[s];
+  // every launch below reads S on ctx->stream, or on aux / the class streams joined back into it by ev_join before the
+  // segment ends, which is what for_each_segment needs to reuse a ring slot of a host-resident C
+  return for_each_segment(ctx, Cm, [&](size_t s, const als_csr *S) -> int {
     if (s > 0) {
       reset_segment_counters<<<1, 32, 0, ctx->stream>>>(ctx->counters);
       ALS_CUDA(cudaGetLastError());
@@ -406,8 +411,8 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
       ALS_CUDA(cudaGetLastError());
       ctx->launches++;
     }
-  }
-  return ALS_OK;
+    return ALS_OK;
+  });
 }
 
 }  // namespace

@@ -193,7 +193,7 @@ int run_wide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const als_factors 
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   const int per_sm = std::max(1, (227 * 1024) / (smem + 1024));
-  for (const als_csr *Cm : segs) {
+  return for_each_segment(ctx, Cw, [&](size_t, const als_csr *Cm) -> int {
     if (Cm->n_work) {
       const int grid = (int)std::min<int64_t>(Cm->n_work, (int64_t)ctx->sm_count * per_sm);
       ProfScope prof(ctx, kProfCholesky);
@@ -210,8 +210,8 @@ int run_wide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const als_factors 
       ALS_CUDA(cudaGetLastError());
       ctx->launches++;
     }
-  }
-  return ALS_OK;
+    return ALS_OK;
+  });
 }
 
 }  // namespace

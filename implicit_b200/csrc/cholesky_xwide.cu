@@ -407,7 +407,7 @@ int launch_cholesky_xwide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const
   xwide_init_bad_row<<<1, 1, 0, ctx->stream>>>(ctx->bad_row);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
-  for (const als_csr *Cm : segs) {
+  return for_each_segment(ctx, Cw, [&](size_t, const als_csr *Cm) -> int {
     const int grid0 = (int)std::min<int64_t>(Cm->n_work, max_grid);
     const int grid1 = (int)std::min<int64_t>(Cm->n_finish, max_grid);
     if (Cm->n_work) {
@@ -426,8 +426,8 @@ int launch_cholesky_xwide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const
       ALS_CUDA(cudaGetLastError());
       ctx->launches++;
     }
-  }
-  return ALS_OK;
+    return ALS_OK;
+  });
 }
 
 }  // namespace als

@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -62,7 +63,10 @@ struct als_knobs {
   int long_tc = 0;            // ALS_B200_LONG_TC: experimental wgmma kernel for the long rows of a Cholesky half (cholesky_tc.cu)
   int cg_nv = 2;              // ALS_B200_CG_NV: float4 words per lane of the CG kernel (1 / 2 / 4)
   int64_t segment_nnz = 0;    // ALS_B200_SEGMENT_NNZ: nonzeros per row-block segment of a device CSR; 0: automatic (one
-                              // segment below 2^31 - 1 nonzeros, else segments of at most 2^30).  Changes no bit.
+                              // segment below 2^31 - 1 nonzeros, else segments of at most 2^30; 2^28 for a host-resident
+                              // CSR).  Changes no bit.
+  int host_csr = 0;           // ALS_B200_HOST_CSR: fit() keeps Cui / Ciu in page-locked host memory and streams their
+                              // segments through the device even when they fit in device memory.  Changes no bit.
 };
 
 struct als_ctx {
@@ -118,6 +122,9 @@ struct als_ctx {
   int32_t *sched_pinned = nullptr;
   int64_t sched_pinned_cap = 0;
   cudaEvent_t sched_ev = nullptr;
+  // the two-slot device ring that streams the segments of a host-resident CSR (csr.cu for_each_segment): a slot is
+  // loaded (ring_loaded, on the copy stream) and free again once every launch that read it has finished (ring_free)
+  cudaEvent_t ring_loaded[2] = {nullptr, nullptr}, ring_free[2] = {nullptr, nullptr};
   // per-kernel profiling (als_profile_*)
   bool profiling = false;
   std::vector<cudaEvent_t> prof_events[8];  // pairs (start, stop) per category
@@ -173,6 +180,10 @@ struct als_csr {
   // and wmax_dev, has_neg_w and max_row_nnz cover all segments.  Empty: one segment, the CSR itself.
   std::vector<als_csr *> segs;
   int32_t *seg_indptr = nullptr;  // the segments' indptrs, concatenated (rows + segs.size() entries)
+  // Host-resident (als_csr_upload_host64, or the transpose of such a CSR): indices / data are page-locked host arrays and
+  // always segmented; seg_indptr, the schedules and wmax_dev stay on the device.  Every solve streams the segments through
+  // a device ring (for_each_segment); wmax_dev is computed on the host, so it is always valid.
+  bool host = false;
 };
 
 namespace als {
@@ -212,8 +223,20 @@ static inline std::vector<const als_csr *> segments_of(const als_csr *c) {
   if (c->segs.empty()) return {c};
   return std::vector<const als_csr *>(c->segs.begin(), c->segs.end());
 }
-// the largest segment: the knob, else 2^30 (2x headroom on the kernels' int32 positions)
-static inline int64_t segment_cap(const als_ctx *ctx) { return ctx->knobs.segment_nnz > 0 ? ctx->knobs.segment_nnz : (int64_t)1 << 30; }
+// the largest segment: the knob, else 2^30 (2x headroom on the kernels' int32 positions); 2^28 for a host-resident CSR,
+// whose two-slot device ring then takes 4 GB
+static inline int64_t segment_cap(const als_ctx *ctx, bool host = false) {
+  return ctx->knobs.segment_nnz > 0 ? ctx->knobs.segment_nnz : (int64_t)1 << (host ? 28 : 30);
+}
+// Runs launch(s, S) for every segment of C in row order.  For a host-resident C, segment s + 1 is copied into a two-slot
+// device ring on ctx->copy while segment s computes, and S is a view of segment s whose indices / data point into its
+// slot.  launch must queue its work on ctx->stream, or join every other stream it uses back into ctx->stream before it
+// returns: a slot is refilled only after ctx->stream has passed that point.
+// with_data = false stages the indices only (launch must not read S->data).
+using SegmentLaunch = std::function<int(size_t s, const als_csr *S)>;
+int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch, bool with_data = true);
+// free device memory, counting the blocks the stream-ordered pool keeps for reuse as free (synchronises ctx->stream)
+int mem_info(als_ctx *ctx, int64_t *free_bytes, int64_t *total_bytes);
 // a CSR of nnz nonzeros is held as segments: above the knob when it is set, else from 2^31 - 1 nonzeros on
 static inline bool needs_segments(const als_ctx *ctx, int64_t nnz) {
   return ctx->knobs.segment_nnz > 0 ? nnz > ctx->knobs.segment_nnz : nnz >= (int64_t)INT32_MAX;
@@ -224,6 +247,11 @@ int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip);
 // the indptr of any CSR as 64-bit positions relative to its first nonzero (synchronises)
 int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out);
 int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
+// the weight range of a host-resident CSR, computed on the host (bits of max | |c| - 1 | without NaN / inf, and whether
+// some |c| < 1: exactly what csr_wmax_kernel finds) -> c->wmax_dev, marked valid
+int set_host_wmax(als_ctx *ctx, als_csr *c, unsigned wmax_bits, bool neg);
+// the same range folded over n values on the host
+void host_wmax(const float *v, int64_t n, unsigned *wmax_bits, bool *neg);
 // synthetic inputs generated on the device (gen.cu)
 int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t nnz_target, uint64_t seed, als_csr **out);
 int factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale);

@@ -60,11 +60,17 @@ int als_ctx_create(int device, als_ctx **out);
 int als_ctx_destroy(als_ctx *ctx);
 
 /* Measurement knobs ("short_max" 0/16/32/48, "short_serial", "whiten_fma", "gramian_fma", "topk_legacy", "cg_nv" 1/2/4,
- * "segment_nnz": 0 = automatic, else the most nonzeros of one row-block segment of a device CSR).  The
+ * "segment_nnz": 0 = automatic, else the most nonzeros of one row-block segment of a device CSR; "host_csr": the Python
+ * fit() keeps Cui / Ciu host-resident even when they fit in device memory).  The
  * environment variables ALS_B200_<KNOB> are read once, in als_ctx_create, and reported on stderr when set; this
- * call changes a knob afterwards (A/B tools).  Results do not depend on any knob beyond fp32 rounding.
+ * call changes a knob afterwards (A/B tools).  Results do not depend on any knob beyond fp32 rounding; segment_nnz and
+ * host_csr change no bit.  als_ctx_get_knob reads one back.
  * (No reference equivalent.) */
 int als_ctx_set_knob(als_ctx *ctx, const char *name, int value);
+int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value);
+/* Free and total device memory in bytes.  Blocks the context's stream-ordered pool keeps for reuse count as free
+ * (cudaMemGetInfo alone under-reports after a fit has freed its arrays).  Synchronises the compute stream. */
+int als_mem_info(als_ctx *ctx, int64_t *free_bytes, int64_t *total_bytes);
 
 /* Join the ctx streams (replaces the cudaDeviceSynchronize after every call, implicit/gpu/als.cu:147,151,196). */
 int als_sync(als_ctx *ctx);
@@ -100,6 +106,17 @@ int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const 
  * the segment cap the CSR is stored as row-block segments of at most 2^30 nonzeros (or segment_nnz). */
 int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                      const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out);
+/* The same arguments and refusals, for a CSR larger than device memory: indices / data stay in page-locked host memory
+ * (indices narrowed to int32 while they are copied there) and the CSR is always held as row-block segments of at most
+ * 2^28 nonzeros (or segment_nnz).  The segment indptrs, schedules and weight range live on the device.  Every solve,
+ * the loss and als_csr_transpose stream the segments through a two-slot device ring, the copy of one segment under the
+ * compute of the one before it, with bitwise the factors of the device-resident CSR of the same segment cap.
+ * als_csr_transpose of it is host-resident too, built in column windows bounded by free device memory.
+ * als_csr_slice_rows and als_topk's `liked` refuse it (ALS_E_UNSUPPORTED). */
+int als_csr_upload_host64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
+                          const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out);
+/* *host = 1 for a host-resident CSR (als_csr_upload_host64 or its transpose), else 0. */
+int als_csr_is_host(const als_csr *csr, int *host);
 /* Number of row-block segments of the device layout (1 for a CSR within the segment cap). */
 int als_csr_segment_count(const als_csr *csr, int64_t *n);
 /* Synthetic inputs generated on the device (BASELINE.json configs too large to build on the host, e.g. C4:
