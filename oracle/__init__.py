@@ -145,6 +145,17 @@ def _port_least_squares_cg(Cui, X, Y, regularization, num_threads=0, cg_steps=3)
                                         X.shape[0], N, int(cg_steps), int(num_threads))
 
 
+def _port_least_squares_cg_with_gramian(YtY, Cui, X, Y, regularization, num_threads=0, cg_steps=3):
+    """_port_least_squares_cg with the caller's fp32 Gramian in place of Y^T Y (a shard's Gramian, as
+    als_least_squares_cg_pregram takes it): YtY + reg I is formed in fp32 like :164."""
+    _check(X), _check(Y)
+    N = X.shape[1]
+    YtY = np.ascontiguousarray(np.asarray(YtY, dtype=np.float32) + np.float32(regularization) * np.eye(N, dtype=np.float32))
+    indptr, indices, data = _csr_parts(Cui)
+    _port_lib().oracle_least_squares_cg(_f32(YtY), _i32(indptr), _i32(indices), _f32(data), _f32(X), _f32(Y),
+                                        X.shape[0], N, int(cg_steps), int(num_threads))
+
+
 def _port_calculate_loss(Cui, X, Y, regularization, num_threads=0):
     """implicit/cpu/_als.pyx:251-308"""
     _check(X), _check(Y)
@@ -180,8 +191,8 @@ def _port_topk(items, query, k, item_norms=None, filter_query_items=None, filter
 
 port = types.SimpleNamespace(
     name="port", least_squares=_port_least_squares, _least_squares=_port__least_squares,
-    least_squares_cg=_port_least_squares_cg, calculate_loss=_port_calculate_loss, topk=_port_topk,
-    gramian=_port_gramian,
+    least_squares_cg=_port_least_squares_cg, least_squares_cg_with_gramian=_port_least_squares_cg_with_gramian,
+    calculate_loss=_port_calculate_loss, topk=_port_topk, gramian=_port_gramian,
 )
 
 

@@ -58,6 +58,104 @@ def cholesky_truth(Cui, Y, reg, YtY=None):
     return X
 
 
+def _nnz_dots(Y64, V, indices, owner, out=None):
+    """d_k = y_k . v_owner(k) for every stored entry, in blocks of ~4M products (bounded memory at 1024 factors)."""
+    d = np.empty(len(indices)) if out is None else out
+    block = max(1, (1 << 22) // max(1, Y64.shape[1]))
+    for k0 in range(0, len(indices), block):
+        k1 = min(len(indices), k0 + block)
+        d[k0:k1] = np.einsum("kf,kf->k", Y64[indices[k0:k1]], V[owner[k0:k1]])
+    return d
+
+
+def _csr_parts64(Cui, r0=0, r1=None):
+    """(indptr rebased to 0, indices, data as fp64, owner row of every entry) of rows [r0, r1), duplicates kept."""
+    r1 = Cui.shape[0] if r1 is None else r1
+    indptr = np.asarray(Cui.indptr[r0:r1 + 1], dtype=np.int64)
+    s, e = int(indptr[0]), int(indptr[-1])
+    indptr = indptr - s
+    owner = np.repeat(np.arange(r1 - r0), np.diff(indptr))
+    return indptr, np.asarray(Cui.indices[s:e]), np.asarray(Cui.data[s:e], dtype=np.float64), owner
+
+
+def _rows_times_Y(coef, indices, indptr, Y64):
+    """sum_k coef_k y_k per row: the sparse matrix (coef, indices, indptr) times Y (duplicates add, as in the loop)."""
+    M = sp.csr_matrix((coef, indices, indptr), shape=(len(indptr) - 1, Y64.shape[0]))
+    return np.asarray(M @ Y64)
+
+
+def cg_truth(Cui, X0, Y, reg, cg_steps, YtY=None):
+    """The CG half in fp64: _least_squares_cg (_als.pyx:154-248, oracle_least_squares_cg) with the same recurrences
+    and the same 1e-20 thresholds on rsold (skip the row, x unchanged) and rsnew (stop after that step), vectorised
+    over rows.  A = G + reg I with G = YtY (the caller's, cast to fp64) or the fp64 Y^T Y.  Every stored entry counts:
+    a stored zero weighs |c| - 1 = -1, duplicates are not merged.  Empty rows are zero (:182-184).
+    Returns (X, rs0, stop, rs_last): rs0 the initial r.r of every row (0 for empty rows), stop the number of CG steps
+    applied to the row (0 for empty rows and rows skipped on rsold), rs_last its r.r after the last of those steps
+    (rs0 where none ran), so that rows which broke on rsnew are those with rs_last < 1e-20."""
+    Y64 = np.asarray(Y, dtype=np.float64)
+    n, f = Cui.shape[0], Y64.shape[1]
+    A = (Y64.T @ Y64 if YtY is None else np.asarray(YtY, dtype=np.float64)) + reg * np.eye(f)
+    indptr, indices, c, owner = _csr_parts64(Cui)
+    w, pos = np.abs(c) - 1.0, np.maximum(c, 0.0)
+    nonempty = np.diff(indptr) > 0
+    X = np.array(X0, dtype=np.float64)
+    X[~nonempty] = 0.0
+    # r = b - A x = sum_k (c_k^+ - (|c_k| - 1) y_k.x) y_k - (G + reg I) x          (:187-201)
+    r = _rows_times_Y(pos - w * _nnz_dots(Y64, X, indices, owner), indices, indptr, Y64) - X @ A
+    r[~nonempty] = 0.0
+    p = r.copy()
+    rsold = np.einsum("uf,uf->u", r, r)
+    rs0, rs_last = rsold.copy(), rsold.copy()
+    stop = np.zeros(n, dtype=np.int64)
+    active = nonempty & (rsold >= 1e-20)  # :206-207
+    for s in range(cg_steps):
+        rows = np.nonzero(active)[0]
+        if not len(rows):
+            break
+        # Ap = (G + reg I) p + sum_k (|c_k| - 1) (y_k.p) y_k                           (:212-222)
+        Ap = p @ A + _rows_times_Y(w * _nnz_dots(Y64, p, indices, owner), indices, indptr, Y64)
+        alpha = rsold[rows] / np.einsum("uf,uf->u", p[rows], Ap[rows])   # :225
+        X[rows] += alpha[:, None] * p[rows]                               # :228
+        r[rows] -= alpha[:, None] * Ap[rows]                              # :231-232
+        rsnew = np.einsum("uf,uf->u", r[rows], r[rows])                   # :234
+        stop[rows], rs_last[rows] = s + 1, rsnew
+        go = rsnew >= 1e-20                                               # :235-236
+        active[rows[~go]] = False
+        rows, rsnew = rows[go], rsnew[go]
+        p[rows] = r[rows] + (rsnew / rsold[rows])[:, None] * p[rows]     # :239-242
+        p[~active] = 0.0  # stopped rows take no further part
+        rsold[rows] = rsnew
+    return X, rs0, stop, rs_last
+
+
+def loss_truth(Cui, X, Y, reg, rows=None):
+    """The training loss in fp64 the way _calculate_loss computes it (_als.pyx:259-308, oracle_calculate_loss), row
+    by row: r = Y^T Y x_u + sum_k ((c_k > 0 ? -2 c_k : 0) + (|c_k| - 1) y_k.x_u) y_k, loss += r.x_u + sum_k |c_k| --
+    not through the expansion <Y^T Y, X^T X>_F + sum_k (...) that the device uses.
+    rows = (r0, r1) restricts the sums over users to those rows of Cui and X (a shard).
+    Returns (loss, terms, scale): terms are those of als_calculate_loss for the rows, [0] = sum_u (r.x_u + sum_k |c_k|)
+    + reg sum_u |x_u|^2, [1] = sum_k |c_k|, [2] = reg |Y|^2; loss = (terms[0] + terms[2]) / (terms[1] + U I - nnz)
+    with U and nnz of the rows (the loss of Cui for the whole range).  scale holds the same sums with every product
+    replaced by the product of absolute values: the size of the rounding an fp32 evaluation of each term can carry."""
+    r0, r1 = (0, Cui.shape[0]) if rows is None else rows
+    Y64 = np.asarray(Y, dtype=np.float64)
+    Xr = np.asarray(X, dtype=np.float64)[r0:r1]
+    indptr, indices, c, owner = _csr_parts64(Cui, r0, r1)
+    conf = np.abs(c)
+    terms, scale = np.zeros(3), np.zeros(3)
+    for k, (Yk, Xk) in enumerate(((Y64, Xr), (np.abs(Y64), np.abs(Xr)))):
+        d = _nnz_dots(Yk, Xk, indices, owner)
+        temp = (np.where(c > 0, -2.0 * c, 0.0) + (conf - 1.0) * d if k == 0
+                else np.where(c > 0, 2.0 * c, 0.0) + np.abs(conf - 1.0) * d)
+        r = Xk @ (Yk.T @ Yk) + _rows_times_Y(temp, indices, indptr, Yk)    # :282-298
+        out = terms if k == 0 else scale
+        out[0] = np.einsum("uf,uf->", r, Xk) + conf.sum() + reg * np.einsum("uf,uf->", Xk, Xk)  # :300-301, :307
+        out[1] = conf.sum()
+        out[2] = reg * np.einsum("if,if->", Yk, Yk)                         # :303-304
+    den = terms[1] + float(r1 - r0) * float(Cui.shape[1]) - float(len(c))
+    return (terms[0] + terms[2]) / den, terms, scale
+
+
 #: every knob of als_ctx_set_knob and its default (include/als_b200.h, csrc/common.h)
 KNOB_DEFAULTS = dict(short_max=48, short_serial=0, whiten_fma=0, gramian_fma=0, topk_legacy=0,
                      long_tc=0, cg_nv=2)

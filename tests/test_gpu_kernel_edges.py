@@ -10,7 +10,7 @@ import pytest
 import scipy.sparse as sp
 
 import oracle
-from helpers import (CG_MEDIAN, KNOB_DEFAULTS, cholesky_truth, factors_of, mixed_csr, row_err, topk_mismatches,
+from helpers import (KNOB_DEFAULTS, cholesky_truth, factors_of, mixed_csr, row_err, topk_mismatches,
                      topk_noise, worst_ratio)
 from helpers import ctx, default_knobs, lib, orc, sm  # noqa: F401  (fixtures)
 from implicit_b200 import synthetic
@@ -240,28 +240,6 @@ def test_least_squares_with_gramian_that_does_not_bound_Y(lib, ctx, orc, which):
     assert np.isfinite(got).all()
     assert e.max() <= max(2e-5, 3 * e_ref.max())
     assert np.median(e) <= max(2e-6, 1.5 * np.median(e_ref))
-
-
-# ---------------------------------------------------------------------------------------- CG, every cg_nv
-@pytest.mark.parametrize("f", [64, 128])
-@pytest.mark.parametrize("nv", [1, 2, 4])
-def test_cg_half_under_cg_nv(lib, ctx, orc, f, nv):
-    """The CG kernel with 1, 2 or 4 float4 words per lane against the oracle, with the bars of the CG parity tests."""
-    Cui = synthetic.power_law_csr(700, 450, 12000, 200 + f, 0.05)
-    X, Y = synthetic.initial_factors(700, 450, f)
-    oracle.fit(Cui, X, Y, iterations=2, use_cg=False, kind=orc.name)
-    exp = X.copy()
-    orc.least_squares_cg(Cui, exp, Y, 0.01, cg_steps=3)
-    ctx.set_knob("cg_nv", nv)
-    C = lib.DeviceCSR.upload(ctx, Cui)
-    dX, dY = lib.DeviceFactors.from_host(ctx, X), lib.DeviceFactors.from_host(ctx, Y)
-    lib.least_squares_cg(ctx, C, dX, dY, 0.01, 3)
-    got = dX.download()
-    for h in (C, dX, dY):
-        h.close()
-    e = row_err(got, exp)
-    print(f"cg_nv={nv} f={f}: max {e.max():.2e} median {np.median(e):.2e}")
-    assert e.max() < 1e-4 and np.median(e) < CG_MEDIAN
 
 
 # ---------------------------------------------------------------------------------------- top-k on wgmma

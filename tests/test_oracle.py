@@ -11,7 +11,8 @@ import pytest
 from scipy.sparse import csr_matrix
 
 import oracle
-from helpers import CHOL_MAX, GOLDEN, cholesky_truth, golden_cases, load_golden, row_err
+from helpers import (CG_MEDIAN, CG_P99, CHOL_MAX, GOLDEN, cg_truth, cholesky_truth, golden_cases, load_golden,
+                     loss_truth, row_err)
 
 sys.path.insert(0, GOLDEN)
 import make_golden_ref  # noqa: E402
@@ -94,6 +95,89 @@ def test_cholesky_truth_counts_zeros_duplicates_and_negatives():
     merged = Cui.copy()
     merged.sum_duplicates()
     assert row_err(cholesky_truth(merged, Y, 0.5), truth).max() > 1e-3  # merging duplicates is a different problem
+
+
+@pytest.mark.parametrize("name", [n for n in golden_cases() if n.startswith("cg")])
+def test_cg_truth_matches_golden_half(name):
+    """tests/helpers.cg_truth, the fp64 yardstick of the GPU CG tests, against the oracle port's fp32 half from the
+    stored warm state, within the CG parity bars (median and p99: truncated CG amplifies fp32 rounding)."""
+    _, Cui, _, _, z = load_golden(name)
+    truth, rs0, stop, _ = cg_truth(Cui, z["X"], z["Y"], 0.01, 3)
+    got = z["X"].copy()
+    PORT.least_squares_cg(Cui, got, z["Y"], 0.01, cg_steps=3)
+    e = row_err(got, truth)
+    print(f"{name}: fp32 port vs cg_truth max {e.max():.2e} median {np.median(e):.2e} p99 {np.quantile(e, 0.99):.2e}")
+    assert np.median(e) < CG_MEDIAN and np.quantile(e, 0.99) < CG_P99
+    assert row_err(z["Xh"], truth).max() < 1e-2 and np.median(row_err(z["Xh"], truth)) < CG_MEDIAN
+    lens = np.diff(Cui.indptr)
+    assert np.all(stop[lens > 0] == 3) and np.all(rs0[lens > 0] > 1e-18)
+
+
+def test_cg_truth_counts_zeros_duplicates_and_negatives():
+    """The CG yardstick on stored zeros, duplicates, negative confidences and an empty row, against the oracle's fp32
+    half; with cg_steps well past f on this small, well-conditioned problem it is the Cholesky solution."""
+    rng = np.random.default_rng(13)
+    indptr = np.array([0, 5, 9, 9, 12], dtype=np.int32)
+    indices = np.array([1, 1, 3, 7, 2, 0, 4, 4, 6, 5, 2, 5], dtype=np.int32)
+    data = np.array([2.0, 3.0, 0.0, -1.5, 1.0, 4.0, 0.0, 2.5, -0.5, 3.0, 0.5, 3.0], dtype=np.float32)
+    Cui = csr_matrix((data, indices, indptr), shape=(4, 8))
+    Y = (rng.standard_normal((8, 6)) * 0.4).astype(np.float32)
+    X0 = (rng.standard_normal((4, 6)) * 0.1).astype(np.float32)
+    for steps in (1, 3):
+        exp = X0.copy()
+        PORT.least_squares_cg(Cui, exp, Y, 0.5, cg_steps=steps)
+        truth, _, stop, _ = cg_truth(Cui, X0, Y, 0.5, steps)
+        assert np.all(truth[2] == 0) and np.all(stop == [steps, steps, 0, steps])
+        assert row_err(exp, truth).max() < 1e-5
+    X, _, stop, rs_last = cg_truth(Cui, X0, Y, 0.5, 24)
+    assert row_err(X, cholesky_truth(Cui, Y, 0.5)).max() < 1e-9
+    assert np.all(stop[[0, 1, 3]] < 24) and np.all(rs_last[[0, 1, 3]] < 1e-20)  # the rsnew break ended every row
+
+
+def test_cg_truth_skips_rows_below_the_threshold():
+    """rsold < 1e-20 leaves x as it is (_als.pyx:206-207); rsnew < 1e-20 stops after that step (:235-236): a row whose
+    items' factors span one direction converges in one step."""
+    Cui = csr_matrix((np.array([2.0, 3.0, 1.5], np.float32), np.array([0, 1, 2]), np.array([0, 2, 3])), shape=(2, 3))
+    Y = np.zeros((3, 4), dtype=np.float32)
+    Y[2, 1] = 1.0  # row 1 sees y = e1 only; row 0's items are zero
+    X0 = np.zeros((2, 4), dtype=np.float32)
+    X, rs0, stop, rs_last = cg_truth(Cui, X0, Y, 0.0, 3, YtY=np.diag([0.0, 1.0, 0.0, 0.0]))
+    assert rs0[0] == 0 and stop[0] == 0 and np.all(X[0] == 0)
+    assert stop[1] == 1 and rs_last[1] < 1e-20
+    np.testing.assert_allclose(X[1], [0, 1.5 / 1.5, 0, 0], atol=1e-12)  # (y y^T + 0.5 y y^T) x = 1.5 y
+
+
+@pytest.mark.parametrize("name", golden_cases())
+def test_loss_truth_matches_golden(name):
+    """tests/helpers.loss_truth against the reference's fp32 loss on the golden state, and term by term on two
+    shards against the whole."""
+    _, Cui, _, _, z = load_golden(name)
+    loss, terms, scale = loss_truth(Cui, z["X"], z["Y"], 0.01)
+    assert loss == pytest.approx(float(z["loss"]), rel=1e-5)
+    assert loss == pytest.approx(PORT.calculate_loss(Cui, z["X"], z["Y"], 0.01), rel=1e-5)
+    assert np.all(scale >= np.abs(terms))
+    m = Cui.shape[0] // 3
+    parts = [loss_truth(Cui, z["X"], z["Y"], 0.01, rows=r)[1] for r in ((0, m), (m, Cui.shape[0]))]
+    np.testing.assert_allclose(parts[0][:2] + parts[1][:2], terms[:2], rtol=1e-12)
+    assert parts[0][2] == parts[1][2] == terms[2]
+
+
+def test_loss_truth_known_answers_and_stored_entries():
+    """tests/als_test.py:304-324 (loss 1.0 at lambda 0, 2.0 at lambda 1), and the oracle's loss on stored zeros,
+    duplicates, negative confidences and an empty row."""
+    ratings = csr_matrix((np.array([1.0], np.float32), np.array([0]), np.array([0, 1])), shape=(1, 2))
+    item_factors = np.array([[0.0], [1.0]], dtype="float32")
+    user_factors = np.array([[1.0]], dtype="float32")
+    assert loss_truth(ratings, user_factors, item_factors, 0)[0] == pytest.approx(1.0, abs=1e-15)
+    assert loss_truth(ratings, user_factors, item_factors, 1.0)[0] == pytest.approx(2.0, abs=1e-15)
+    rng = np.random.default_rng(14)
+    indptr = np.array([0, 5, 9, 9, 12], dtype=np.int32)
+    indices = np.array([1, 1, 3, 7, 2, 0, 4, 4, 6, 5, 2, 5], dtype=np.int32)
+    data = np.array([2.0, 3.0, 0.0, -1.5, 1.0, 4.0, 0.0, 2.5, -0.5, 3.0, 0.5, 3.0], dtype=np.float32)
+    Cui = csr_matrix((data, indices, indptr), shape=(4, 8))
+    X = rng.standard_normal((4, 6)).astype(np.float32)
+    Y = rng.standard_normal((8, 6)).astype(np.float32)
+    assert loss_truth(Cui, X, Y, 0.3)[0] == pytest.approx(PORT.calculate_loss(Cui, X, Y, 0.3), rel=1e-6)
 
 
 @pytest.mark.parametrize("use_cg", [False, True])
