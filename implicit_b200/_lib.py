@@ -352,7 +352,7 @@ class DeviceCSR:
         self.ctx, self.h, self._parent = ctx, handle, parent
 
     @classmethod
-    def upload(cls, ctx, m, row_offset=0, rows=None, host=False):
+    def upload(cls, ctx, m, row_offset=0, host=False):
         """m: scipy.sparse.csr_matrix (any float dtype; values are cast to float32).  host: keep it host-resident
         (als_csr_upload_host64)."""
         data = np.ascontiguousarray(m.data, dtype=np.float32)
@@ -422,8 +422,7 @@ class DeviceCSR:
         indptr = self.indptr_host()
         indices = np.zeros(nnz, dtype=np.int32)
         data = np.zeros(nnz, dtype=np.float32)
-        download = self.ctx.lib.als_csr_download64 if indptr.dtype == np.int64 else self.ctx.lib.als_csr_download
-        check(download(self.ctx.h, self.h, None, ptr(indices), ptr(data)))
+        check(self.ctx.lib.als_csr_download64(self.ctx.h, self.h, None, ptr(indices), ptr(data)))
         return sp.csr_matrix((data, indices, indptr), shape=(rows, cols))
 
     def indptr_host(self):

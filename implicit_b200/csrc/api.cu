@@ -74,21 +74,6 @@ int ensure_device_buffer(als_ctx *ctx, void **buf, int64_t *cap, int64_t bytes) 
   return ALS_OK;
 }
 
-int ensure_pinned(als_ctx *ctx, int64_t bytes) {
-  if (bytes <= ctx->pinned_bytes) return ALS_OK;
-  if (ctx->pinned) {
-    ALS_CUDA(cudaStreamSynchronize(ctx->copy));
-    ALS_CUDA(cudaFreeHost(ctx->pinned));
-    ctx->pinned = nullptr;
-    ctx->pinned_bytes = 0;
-  }
-  int64_t cap = std::max<int64_t>(bytes, 1 << 20);
-  ALS_CUDA(cudaMallocHost(&ctx->pinned, cap));
-  ctx->pinned_bytes = cap;
-  return ALS_OK;
-}
-
-
 // ---- host -> device copies of ordinary (pageable) memory ---------------------------------------------------------
 // cudaMemcpyAsync from pageable memory is staged by the driver through one thread at ~12 GB/s; a user of the
 // reference hands fit() ordinary numpy / scipy arrays, so for large buffers four host threads copy 4 MB chunks into
@@ -221,25 +206,25 @@ static int h2d_indices(als_ctx *ctx, int32_t *dst, const void *src, int index_by
   return rc;
 }
 
-// n values -> a page-locked host array in the staging threads, folding the weight range of csr_wmax_kernel on the way
-static int fill_host_values(float *dst, const float *src, int64_t n, unsigned *wmax_bits, bool *neg) {
+// Writes the n values of a host-resident CSR at dst in the staging threads, chunk by chunk (fill(v, i0, m) writes values
+// i0 .. i0 + m - 1 to v), and folds the weight range of csr_wmax_kernel over what they wrote into c->wmax_dev.
+static int fill_host_values(als_ctx *ctx, als_csr *c, float *dst, int64_t n,
+                            const std::function<void(float *v, int64_t i0, int64_t m)> &fill) {
   std::atomic<unsigned> m{0};
   std::atomic<bool> ng{false};
-  const int rc = staged_fill_host(dst, (size_t)n * sizeof(float), [&](char *out, size_t off, size_t len) {
-    const float *in = src + off / 4;
-    memcpy(out, in, len);
+  staged_fill_host(dst, sizeof(float) * (size_t)n, [&](char *out, size_t off, size_t len) {
+    float *v = reinterpret_cast<float *>(out);
+    fill(v, (int64_t)(off / 4), (int64_t)(len / 4));
     unsigned cm;
     bool cn;
-    host_wmax(in, (int64_t)(len / 4), &cm, &cn);
+    host_wmax(v, (int64_t)(len / 4), &cm, &cn);
     unsigned cur = m.load();
     while (cm > cur && !m.compare_exchange_weak(cur, cm)) {
     }
     if (cn) ng = true;
     return true;
   });
-  *wmax_bits = m.load();
-  *neg = ng.load();
-  return rc;
+  return set_host_wmax(ctx, c, m.load(), ng.load());
 }
 
 // Longest-first schedule.  Rows with more than kSplitNnz nonzeros are cut into chunks of kChunkNnz
@@ -518,7 +503,6 @@ ALS_API int als_ctx_destroy(als_ctx *ctx) {
   cudaFree(ctx->status);
   cudaFree(ctx->dscalars);
   cudaFree(ctx->scratch);
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->stage_buf) {
     cudaFreeHost(ctx->stage_buf);
     for (int t = 0; t < 4; ++t) {
@@ -659,91 +643,30 @@ ALS_API int als_host_free(void *ptr) {
 }
 
 // ---- CSR ---------------------------------------------------------------------------------------
-ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int32_t *indptr,
-                           const int32_t *indices, const float *data, int64_t row_offset, als_csr **out) {
-  ALS_REQUIRE(ctx && out && indptr, "als_csr_upload: NULL argument");
-  ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "als_csr_upload: negative shape");
-  ALS_REQUIRE(nnz < (int64_t)INT32_MAX && rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX,
-              "als_csr_upload: int32 CSR only (rows, cols, nnz < 2^31), like implicit/gpu/matrix.h:93-100");
-  ALS_REQUIRE(indptr[0] >= 0 && (int64_t)indptr[rows] - indptr[0] == nnz,
-              "als_csr_upload: indptr[rows] - indptr[0] = %lld != nnz = %lld",
-              (long long)indptr[rows] - indptr[0], (long long)nnz);
-  ALS_REQUIRE(nnz == 0 || (indices && data), "als_csr_upload: indices/data NULL with nnz > 0");
-  *out = nullptr;
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
-  c->rows = rows;
-  c->cols = cols;
-  c->nnz = nnz;
-  c->row_offset = row_offset;
-  // a row shard arrives with indptr[0] != 0: rebase
-  std::vector<int32_t> rebased;
-  const int32_t base = indptr[0];
-  const int32_t *ip = indptr;
-  if (base != 0) {
-    rebased.resize(rows + 1);
-    for (int64_t r = 0; r <= rows; ++r) rebased[r] = indptr[r] - base;
-    ip = rebased.data();
-  }
-  for (int64_t r = 0; r < rows; ++r) {
-    if (ip[r + 1] < ip[r]) {
-      delete c;
-      set_error("als_csr_upload: indptr is not monotone at row %lld", (long long)r);
-      return ALS_E_INVALID;
-    }
-  }
-  int arc;
-  if (needs_segments(ctx, nnz)) {  // a cap set by the segment_nnz knob: the same layout as als_csr_upload64's
-    std::vector<int64_t> ip64(ip, ip + rows + 1);
-    if ((arc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (arc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * nnz)) != ALS_OK ||
-        (arc = h2d_copy(ctx, c->indices, indices + base, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (arc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz)) != ALS_OK ||
-        (arc = make_segments(ctx, c, ip64.data())) != ALS_OK) {
-      als_csr_destroy(c);
-      return arc;
-    }
-    *out = c;
-    return ALS_OK;
-  }
-  if ((arc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (rows + 1))) != ALS_OK ||
-      (arc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-      (arc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK) {
-    als_csr_destroy(c);
-    return arc;
-  }
-  ALS_CUDA(cudaMemcpyAsync(c->indptr, ip, sizeof(int32_t) * (rows + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if (nnz) {
-    int hrc;
-    if ((hrc = h2d_copy(ctx, c->indices, indices + base, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (hrc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz)) != ALS_OK) {
-      als_csr_destroy(c);
-      return hrc;
-    }
-  }
-  int rc = build_schedule(ctx, c, ip);
-  if (rc != ALS_OK) {
-    als_csr_destroy(c);
-    return rc;
-  }
-  *out = c;
-  return ALS_OK;
-}
-
-// als_csr_upload64 and als_csr_upload_host64: the same checks and refusals; host keeps indices / data in page-locked host
-// memory (always segmented) instead of uploading them
-static int csr_upload64(const char *who, bool host, als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
-                        const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+// The one builder behind the three uploads: the checks, the rebase of a row shard (indptr[0] != 0), the arrays of the
+// residency, the copies and the layout.  An int32 indptr is als_csr_upload's: int32 limits on nnz too, and its int32
+// indices are copied as they are; the 64-bit entries narrow the indices while they are staged and refuse any outside
+// [0, cols).
+template <typename IP>
+static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const IP *indptr,
+                     const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
+  constexpr bool int32_entry = sizeof(IP) == sizeof(int32_t);
   ALS_REQUIRE(ctx && out && indptr, "%s: NULL argument", who);
   ALS_REQUIRE(index_bytes == 4 || index_bytes == 8, "%s: index_bytes must be 4 or 8, got %d", who, index_bytes);
   ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "%s: negative shape", who);
-  ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "%s: rows and cols must be < 2^31 - 1", who);
-  ALS_REQUIRE(indptr[0] >= 0 && indptr[rows] - indptr[0] == nnz, "%s: indptr[rows] - indptr[0] = %lld != nnz = %lld", who,
-              (long long)(indptr[rows] - indptr[0]), (long long)nnz);
+  if (int32_entry)
+    ALS_REQUIRE(nnz < (int64_t)INT32_MAX && rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX,
+                "%s: int32 CSR only (rows, cols, nnz < 2^31), like implicit/gpu/matrix.h:93-100", who);
+  else
+    ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "%s: rows and cols must be < 2^31 - 1", who);
+  const int64_t base = indptr[0];
+  ALS_REQUIRE(base >= 0 && (int64_t)indptr[rows] - base == nnz, "%s: indptr[rows] - indptr[0] = %lld != nnz = %lld", who,
+              (long long)((int64_t)indptr[rows] - base), (long long)nnz);
   ALS_REQUIRE(nnz == 0 || (indices && data), "%s: indices/data NULL with nnz > 0", who);
+  std::vector<int64_t> ip((size_t)rows + 1);
+  for (int64_t r = 0; r <= rows; ++r) ip[r] = (int64_t)indptr[r] - base;
   for (int64_t r = 0; r < rows; ++r)
-    ALS_REQUIRE(indptr[r + 1] >= indptr[r], "%s: indptr is not monotone at row %lld", who, (long long)r);
+    ALS_REQUIRE(ip[r + 1] >= ip[r], "%s: indptr is not monotone at row %lld", who, (long long)r);
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
   als_csr *c = new als_csr();
@@ -753,26 +676,17 @@ static int csr_upload64(const char *who, bool host, als_ctx *ctx, int64_t rows, 
   c->nnz = nnz;
   c->row_offset = row_offset;
   c->host = host;
-  const int64_t base = indptr[0];  // a row shard arrives with indptr[0] != 0
-  int rc;
+  const char *ix = (const char *)indices + base * index_bytes;
   int64_t bad = -1;
-  unsigned wmax_bits = 0;
-  bool neg = false;
-  if (host) {
-    const size_t bytes = sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1);
-    cudaError_t e = cudaMallocHost((void **)&c->indices, bytes);
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&c->data, bytes);
-    if (e != cudaSuccess) {
-      als_csr_destroy(c);
-      return cuda_fail(e, "cudaMallocHost (host-resident CSR)", __FILE__, __LINE__);
-    }
-    rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad, true);
-    if (rc == ALS_OK) rc = fill_host_values(c->data, data + base, nnz, &wmax_bits, &neg);
-  } else if ((rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) == ALS_OK &&
-             (rc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) == ALS_OK &&
-             (rc = h2d_indices(ctx, c->indices, (const char *)indices + base * index_bytes, index_bytes, nnz, cols, &bad)) == ALS_OK) {
-    rc = h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz);
-  }
+  int rc = csr_alloc(ctx, c);
+  if (rc == ALS_OK)
+    rc = int32_entry ? h2d_copy(ctx, c->indices, ix, sizeof(int32_t) * nnz)
+                     : h2d_indices(ctx, c->indices, ix, index_bytes, nnz, cols, &bad, host);
+  if (rc == ALS_OK)
+    rc = host ? fill_host_values(ctx, c, c->data, nnz,
+                                 [&](float *v, int64_t i0, int64_t m) { memcpy(v, data + base + i0, sizeof(float) * m); })
+              : h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz);
+  if (rc == ALS_OK) rc = csr_layout(ctx, c, ip.data());
   if (rc != ALS_OK) {
     if (bad >= 0) {
       const int64_t v = index_bytes == 8 ? ((const int64_t *)indices)[base + bad] : ((const int32_t *)indices)[base + bad];
@@ -782,36 +696,24 @@ static int csr_upload64(const char *who, bool host, als_ctx *ctx, int64_t rows, 
     als_csr_destroy(c);
     return rc;
   }
-  std::vector<int64_t> ip((size_t)rows + 1);
-  for (int64_t r = 0; r <= rows; ++r) ip[r] = indptr[r] - base;
-  if (host) {
-    if ((rc = set_host_wmax(ctx, c, wmax_bits, neg)) == ALS_OK) rc = make_segments(ctx, c, ip.data());
-  } else if (needs_segments(ctx, nnz)) {
-    rc = make_segments(ctx, c, ip.data());
-  } else {
-    std::vector<int32_t> ip32(ip.begin(), ip.end());
-    if ((rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (rows + 1))) == ALS_OK) {
-      ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * (rows + 1), cudaMemcpyHostToDevice, ctx->stream));
-      rc = build_schedule(ctx, c, ip32.data());
-      ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-  }
-  if (rc != ALS_OK) {
-    als_csr_destroy(c);
-    return rc;
-  }
   *out = c;
   return ALS_OK;
 }
 
+ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int32_t *indptr,
+                           const int32_t *indices, const float *data, int64_t row_offset, als_csr **out) {
+  return csr_build("als_csr_upload", false, ctx, rows, cols, nnz, indptr, indices, 4, data, row_offset, out);
+}
+
+// als_csr_upload_host64 keeps indices / data in page-locked host memory (always segmented) instead of uploading them
 ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                              const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  return csr_upload64("als_csr_upload64", false, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+  return csr_build("als_csr_upload64", false, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
 }
 
 ALS_API int als_csr_upload_host64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                                   const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  return csr_upload64("als_csr_upload_host64", true, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+  return csr_build("als_csr_upload_host64", true, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
 }
 
 ALS_API int als_csr_is_host(const als_csr *csr, int *host) {
@@ -857,41 +759,25 @@ ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int6
     return ALS_E_UNSUPPORTED;
   }
   ALS_CUDA(cudaSetDevice(ctx->device));
-  if (!in->segs.empty()) {  // a shard of a segmented CSR can itself exceed 2^31 nonzeros: a segmented view
-    std::vector<int64_t> ip64;
-    int rc = csr_indptr64(ctx, in, ip64);
-    if (rc != ALS_OK) return rc;
-    als_csr *c = new als_csr();
-    c->ctx = ctx;
-    c->rows = r1 - r0;
-    c->cols = in->cols;
-    c->nnz = ip64[r1] - ip64[r0];
-    c->row_offset = r0;
-    c->owns = false;
-    c->indices = in->indices;
-    c->data = in->data;
-    if ((rc = make_segments(ctx, c, ip64.data() + r0)) != ALS_OK) {
-      als_csr_destroy(c);
-      return rc;
-    }
-    *out = c;
-    return ALS_OK;
-  }
-  const int64_t rows = r1 - r0;
-  std::vector<int32_t> ip((size_t)rows + 1);
-  ALS_CUDA(cudaMemcpyAsync(ip.data(), in->indptr + r0, sizeof(int32_t) * (rows + 1), cudaMemcpyDeviceToHost, ctx->stream));
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  std::vector<int64_t> ip64;
+  int rc = csr_indptr64(ctx, in, ip64);
+  if (rc != ALS_OK) return rc;
   als_csr *c = new als_csr();
   c->ctx = ctx;
-  c->rows = rows;
+  c->rows = r1 - r0;
   c->cols = in->cols;
-  c->nnz = (int64_t)ip[rows] - ip[0];
+  c->nnz = ip64[r1] - ip64[r0];
   c->row_offset = r0;
   c->owns = false;
-  c->indptr = in->indptr + r0;  // absolute positions into the parent's indices/data
   c->indices = in->indices;
   c->data = in->data;
-  int rc = build_schedule(ctx, c, ip.data());
+  if (!in->segs.empty()) {  // a shard of a segmented CSR can itself exceed 2^31 nonzeros: a segmented view
+    rc = make_segments(ctx, c, ip64.data() + r0);
+  } else {  // a view into the parent's indptr: absolute positions into its indices / data
+    c->indptr = in->indptr + r0;
+    const std::vector<int32_t> ip(ip64.begin() + r0, ip64.begin() + r1 + 1);
+    rc = build_schedule(ctx, c, ip.data());
+  }
   if (rc != ALS_OK) {
     als_csr_destroy(c);
     return rc;
@@ -911,22 +797,9 @@ ALS_API int als_csr_scale(als_ctx *ctx, als_csr *csr, float alpha) {
     // the weight range is folded on the way
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
     ALS_CUDA(cudaStreamSynchronize(ctx->copy));
-    std::atomic<unsigned> m{0};
-    std::atomic<bool> ng{false};
-    staged_fill_host(data, sizeof(float) * (size_t)csr->nnz, [&](char *out, size_t, size_t len) {
-      float *v = reinterpret_cast<float *>(out);
-      const int64_t n = (int64_t)(len / 4);
-      for (int64_t i = 0; i < n; ++i) v[i] *= alpha;
-      unsigned cm;
-      bool cn;
-      host_wmax(v, n, &cm, &cn);
-      unsigned cur = m.load();
-      while (cm > cur && !m.compare_exchange_weak(cur, cm)) {
-      }
-      if (cn) ng = true;
-      return true;
+    return fill_host_values(ctx, csr, data, csr->nnz, [alpha](float *v, int64_t, int64_t m) {
+      for (int64_t i = 0; i < m; ++i) v[i] *= alpha;
     });
-    return set_host_wmax(ctx, csr, m.load(), ng.load());
   }
   csr->wmax_valid = false;
   scale_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(data, csr->nnz, alpha);
@@ -947,29 +820,11 @@ ALS_API int als_csr_download(als_ctx *ctx, const als_csr *csr, int32_t *indptr, 
   ALS_REQUIRE(ctx && csr, "als_csr_download: NULL argument");
   ALS_REQUIRE(csr->nnz < (int64_t)INT32_MAX, "als_csr_download: %lld nonzeros need a 64-bit indptr: use als_csr_download64",
               (long long)csr->nnz);
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  if (!csr->segs.empty()) {
-    std::vector<int64_t> ip64((size_t)csr->rows + 1);
-    int rc = als_csr_download64(ctx, csr, indptr ? ip64.data() : nullptr, indices, data);
-    if (rc != ALS_OK) return rc;
-    if (indptr)
-      for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] = (int32_t)ip64[r];
-    return ALS_OK;
-  }
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  // a row-slice view keeps absolute positions into its parent's arrays: rebase on the way out
-  int32_t base = 0;
-  if (!csr->owns) ALS_CUDA(cudaMemcpy(&base, csr->indptr, sizeof(int32_t), cudaMemcpyDeviceToHost));
-  if (indptr) {
-    ALS_CUDA(cudaMemcpy(indptr, csr->indptr, sizeof(int32_t) * (csr->rows + 1), cudaMemcpyDeviceToHost));
-    if (base)
-      for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] -= base;
-  }
-  if (indices && csr->nnz)
-    ALS_CUDA(cudaMemcpy(indices, csr->indices + base, sizeof(int32_t) * csr->nnz, cudaMemcpyDeviceToHost));
-  if (data && csr->nnz)
-    ALS_CUDA(cudaMemcpy(data, csr->data + base, sizeof(float) * csr->nnz, cudaMemcpyDeviceToHost));
-  return ALS_OK;
+  std::vector<int64_t> ip64(indptr ? (size_t)csr->rows + 1 : 0);
+  int rc = als_csr_download64(ctx, csr, indptr ? ip64.data() : nullptr, indices, data);
+  if (rc == ALS_OK && indptr)
+    for (int64_t r = 0; r <= csr->rows; ++r) indptr[r] = (int32_t)ip64[r];
+  return rc;
 }
 
 ALS_API int als_csr_download64(als_ctx *ctx, const als_csr *csr, int64_t *indptr, int32_t *indices, float *data) {

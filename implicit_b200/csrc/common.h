@@ -109,9 +109,6 @@ struct als_ctx {
   // generic scratch (giant-row partial slots, L2 flush, top-k staging)
   void *scratch = nullptr;
   int64_t scratch_bytes = 0;
-  // pinned host staging
-  void *pinned = nullptr;
-  int64_t pinned_bytes = 0;
   // staged uploads of pageable host memory (api.cu h2d_copy): 4 threads x 2 page-locked 4 MB buffers, own streams
   void *stage_buf = nullptr;
   cudaStream_t stage_stream[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -216,7 +213,6 @@ int ensure_schedule(als_ctx *ctx, als_csr *csr);
 
 int ensure_scratch(als_ctx *ctx, int64_t bytes);
 int ensure_device_buffer(als_ctx *ctx, void **buf, int64_t *cap, int64_t bytes);
-int ensure_pinned(als_ctx *ctx, int64_t bytes);
 int build_schedule(als_ctx *ctx, als_csr *csr, const int32_t *indptr_host);
 // the segments a solve walks: the CSR itself, or its row-block segments in row order
 static inline std::vector<const als_csr *> segments_of(const als_csr *c) {
@@ -244,6 +240,11 @@ static inline bool needs_segments(const als_ctx *ctx, int64_t nnz) {
 // Cuts `p` (rows, cols, nnz, row_offset, indices and data set) into segments of at most segment_cap nonzeros.
 // ip[0 .. rows]: the host indptr as positions into p->indices / p->data.  Builds every segment's schedule.
 int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip);
+// The layout of a CSR whose indices / data are set, from its host indptr ip[0 .. rows] (positions into them): segments
+// when it is host-resident or above the segment cap, else one int32 indptr on the device and its schedule.
+int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip);
+// indices / data for c->nnz entries: page-locked host arrays for a host-resident CSR, else device arrays from the pool
+int csr_alloc(als_ctx *ctx, als_csr *c);
 // the indptr of any CSR as 64-bit positions relative to its first nonzero (synchronises)
 int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out);
 int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);

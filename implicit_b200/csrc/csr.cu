@@ -53,8 +53,8 @@ __global__ void indptr_from_sorted_kernel(const int32_t *__restrict__ sorted_col
   out_indptr[c] = (int32_t)lo;
 }
 
-// ---- the transpose of a CSR held as row-block segments -----------------------------------------------------------
-// Peak memory: input + output + O(piece).  Output positions are 64-bit: a column histogram over all segments, scanned
+// ---- the transpose of a CSR held as row-block segments, device- or host-resident --------------------------------
+// Peak memory of a device-resident transpose: input + output + O(piece).  Output positions are 64-bit: a column histogram over all segments, scanned
 // into the output indptr, gives every column its range; the input is then sorted in row pieces of bounded nnz, in row
 // order, each piece stably by column, and every entry goes to out_indptr[c] + (entries of column c in earlier pieces)
 // + (its rank within the piece's column c).  Pieces in row order and stable sorts keep scipy's order exactly.
@@ -77,7 +77,7 @@ __device__ __forceinline__ int64_t first_of_key(const int32_t *__restrict__ keys
 
 // sorted entry j of a piece (perm[j]: its position after the piece's first nonzero, keys[j]: its column) -> its place
 // in the output.  indptr: the piece's rows in the segment's indptr (indptr[0] is the piece's first nonzero).  Only the
-// columns [c0, c1) are written, to out + (output position - out_base): a window of the output (transpose_host).
+// columns [c0, c1) are written, to out + (output position - out_base): a window of a host-resident output.
 __global__ void scatter_piece_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ keys, int64_t n,
                                      const int32_t *__restrict__ indptr, int rows, int64_t row0,
                                      const float *__restrict__ data, const long long *__restrict__ next,
@@ -111,97 +111,16 @@ __global__ void advance_columns_kernel(const int32_t *__restrict__ keys, int64_t
   }
 }
 
-int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
-  const int64_t cols = in->cols;
-  int end_bit = 1;
-  while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
-  long long *count = nullptr, *out_ip = nullptr;
-  int rc;
-  if ((rc = dev_alloc(ctx, (void **)&count, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
-  if ((rc = dev_alloc(ctx, (void **)&out_ip, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
-  ALS_CUDA(cudaMemsetAsync(count, 0, sizeof(long long) * (cols + 1), ctx->stream));
-  const std::vector<const als_csr *> segs = segments_of(in);
-  for (const als_csr *S : segs) {
-    if (!S->nnz) continue;
-    column_histogram_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(S->indices, S->nnz, (unsigned long long *)count);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  {
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    ALS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count, out_ip, (int)(cols + 1), ctx->stream));
-    if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return rc;
-    ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, count, out_ip, (int)(cols + 1), ctx->stream));
-    dev_free(ctx, tmp);
-  }
-  std::vector<int64_t> ip((size_t)cols + 1);
-  ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
-  ALS_CUDA(cudaMemcpyAsync(count, out_ip, sizeof(long long) * (cols + 1), cudaMemcpyDeviceToDevice, ctx->stream));  // next[c]
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  dev_free(ctx, out_ip);
-  // pieces: whole rows of one segment, at most kPieceNnz nonzeros unless a single row is longer
-  struct Piece { const als_csr *S; int64_t r0, r1, b0, n; };
-  std::vector<Piece> pieces;
-  int64_t max_piece = 0;
-  for (const als_csr *S : segs) {
-    std::vector<int32_t> sip((size_t)S->rows + 1);
-    ALS_CUDA(cudaMemcpy(sip.data(), S->indptr, sizeof(int32_t) * (S->rows + 1), cudaMemcpyDeviceToHost));
-    for (int64_t a = 0; a < S->rows;) {
-      int64_t b = std::upper_bound(sip.begin() + a + 1, sip.end(), (int64_t)sip[a] + kPieceNnz) - sip.begin() - 1;
-      b = std::max(b, a + 1);
-      pieces.push_back(Piece{S, a, b, sip[a], (int64_t)sip[b] - sip[a]});
-      max_piece = std::max(max_piece, pieces.back().n);
-      a = b;
-    }
-  }
-  if (max_piece > 0) {
-    int32_t *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr;
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, segs[0]->indices, keys_out, vals_in, vals_out, (int)max_piece,
-                                             0, end_bit, ctx->stream));
-    if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * max_piece)) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
-        (rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK)
-      return rc;
-    iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, max_piece);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    for (const Piece &pc : pieces) {
-      const int64_t b0 = pc.b0, n = pc.n;
-      if (n == 0) continue;
-      ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pc.S->indices + b0, keys_out, vals_in, vals_out, (int)n, 0,
-                                               end_bit, ctx->stream));
-      scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
-          vals_out, keys_out, n, pc.S->indptr + pc.r0, (int)(pc.r1 - pc.r0), pc.S->row_offset - in->row_offset + pc.r0,
-          pc.S->data + b0, count, t->indices, t->data, 0, INT32_MAX, 0);
-      ALS_CUDA(cudaGetLastError());
-      advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, n, count);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches += 2;
-    }
-    dev_free(ctx, keys_out);  // stream ordered: after the kernels above
-    dev_free(ctx, vals_in);
-    dev_free(ctx, vals_out);
-    dev_free(ctx, tmp);
-  }
-  dev_free(ctx, count);
-  // the output's segments and their schedules are built right away (no lazy schedule for a segmented transpose)
-  return make_segments(ctx, t, ip.data());
-}
-
-// ---- the transpose of a host-resident CSR, into a host-resident CSR --------------------------------------------------
-// The same arithmetic as transpose_segmented with each segment as one piece, but the output is built on the device one
-// column window at a time: a window is a run of whole columns holding at most `budget` output nonzeros.  For each window
-// every input segment is streamed through the ring in row order, sorted stably by column, and only its entries of the
-// window's columns are scattered; the finished window goes to its contiguous place in the host output.  The device
-// working set is the ring, the sort buffers of one segment and one window, whatever nnz is.  When the whole output fits
-// the budget there is one window and the input crosses PCIe twice (the column histogram reads the indices only).
+// The output is built one column window at a time: a window is a run of whole columns, and for each window every
+// input segment is walked in row order (through the ring when it is host-resident) and only its entries of the
+// window's columns are scattered.  A device-resident output is one window, scattered straight into its arrays.  A
+// host-resident output takes windows of at most `budget` output nonzeros in a device buffer, each copied to its
+// contiguous place in the host output: the device working set is then the ring, the sort buffers of one piece and one
+// window, whatever nnz is.  When the whole output fits the budget there is one window and the input crosses PCIe twice
+// (the column histogram reads the indices only).
 constexpr int64_t kWindowSegments = 16;  // a window holds at most this many segment caps of output
 
-int transpose_host(als_ctx *ctx, const als_csr *in, als_csr *t) {
+int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
   const int64_t cols = in->cols;
   int end_bit = 1;
   while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
@@ -229,77 +148,102 @@ int transpose_host(als_ctx *ctx, const als_csr *in, als_csr *t) {
   std::vector<int64_t> ip((size_t)cols + 1);
   ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  int64_t max_seg = 1;
-  for (const als_csr *S : segments_of(in)) max_seg = std::max(max_seg, S->nnz);
+  dev_free(ctx, out_ip);
+  // pieces: whole rows of one segment, at most kPieceNnz nonzeros unless a single row is longer, cut from the segment
+  // indptrs (on the device for either residency)
+  const std::vector<const als_csr *> segs = segments_of(in);
+  struct Piece { int64_t r0, r1, b0, n; };
+  std::vector<std::vector<Piece>> pieces(segs.size());
+  int64_t max_piece = 1, max_seg = 1;
+  for (size_t s = 0; s < segs.size(); ++s) {
+    const als_csr *S = segs[s];
+    std::vector<int32_t> sip((size_t)S->rows + 1);
+    ALS_CUDA(cudaMemcpy(sip.data(), S->indptr, sizeof(int32_t) * (S->rows + 1), cudaMemcpyDeviceToHost));
+    for (int64_t a = 0; a < S->rows;) {
+      int64_t b = std::upper_bound(sip.begin() + a + 1, sip.end(), (int64_t)sip[a] + kPieceNnz) - sip.begin() - 1;
+      b = std::max(b, a + 1);
+      pieces[s].push_back(Piece{a, b, sip[a], (int64_t)sip[b] - sip[a]});
+      max_piece = std::max(max_piece, pieces[s].back().n);
+      a = b;
+    }
+    max_seg = std::max(max_seg, S->nnz);
+  }
   int32_t *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr, *win_indices = nullptr;
   float *win_data = nullptr;
   void *tmp = nullptr;
   size_t tmp_bytes = 0;
-  ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_out, keys_out, vals_in, vals_out, (int)max_seg, 0, end_bit,
-                                           ctx->stream));
-  if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * max_seg)) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * max_seg)) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * max_seg)) != ALS_OK ||
+  ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_out, keys_out, vals_in, vals_out, (int)max_piece, 0,
+                                           end_bit, ctx->stream));
+  if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
+      (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * max_piece)) != ALS_OK ||
+      (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
       (rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK)
     return rc;
-  // the window budget: what is left of free memory once the ring (two segments) is counted, less 1/8 for the pool's
-  // fragmentation, and at most kWindowSegments segment caps (so that a small segment_nnz forces several windows)
-  int64_t free_bytes = 0, total_bytes = 0;
-  if ((rc = mem_info(ctx, &free_bytes, &total_bytes)) != ALS_OK) return rc;
-  const int64_t avail = free_bytes - free_bytes / 8 - 2 * 8 * max_seg;
-  const int64_t budget = std::max<int64_t>(1, std::min(avail / 8, kWindowSegments * segment_cap(ctx, true)));
-  std::vector<std::pair<int64_t, int64_t>> windows;  // column ranges [c0, c1)
-  int64_t max_win = 1;
-  for (int64_t c0 = 0; c0 < cols;) {
-    int64_t c1 = std::upper_bound(ip.begin() + c0 + 1, ip.end(), ip[c0] + budget) - ip.begin() - 1;
-    c1 = std::max(c1, c0 + 1);  // a column longer than the budget is a window of its own
-    windows.emplace_back(c0, c1);
-    max_win = std::max(max_win, ip[c1] - ip[c0]);
-    c0 = c1;
+  std::vector<std::pair<int64_t, int64_t>> windows{{0, cols}};  // column ranges [c0, c1)
+  if (t->host) {
+    // the window budget: what is left of free memory once the ring (two segments) is counted, less 1/8 for the pool's
+    // fragmentation, and at most kWindowSegments segment caps (so that a small segment_nnz forces several windows)
+    int64_t free_bytes = 0, total_bytes = 0;
+    if ((rc = mem_info(ctx, &free_bytes, &total_bytes)) != ALS_OK) return rc;
+    const int64_t avail = free_bytes - free_bytes / 8 - 2 * 8 * max_seg;
+    const int64_t budget = std::max<int64_t>(1, std::min(avail / 8, kWindowSegments * segment_cap(ctx, true)));
+    windows.clear();
+    int64_t max_win = 1;
+    for (int64_t c0 = 0; c0 < cols;) {
+      int64_t c1 = std::upper_bound(ip.begin() + c0 + 1, ip.end(), ip[c0] + budget) - ip.begin() - 1;
+      c1 = std::max(c1, c0 + 1);  // a column longer than the budget is a window of its own
+      windows.emplace_back(c0, c1);
+      max_win = std::max(max_win, ip[c1] - ip[c0]);
+      c0 = c1;
+    }
+    if ((rc = dev_alloc(ctx, (void **)&win_indices, sizeof(int32_t) * max_win)) != ALS_OK ||
+        (rc = dev_alloc(ctx, (void **)&win_data, sizeof(float) * max_win)) != ALS_OK) {
+      set_error("als_csr_transpose: a column window of %lld nonzeros does not fit in device memory (%lld bytes free)",
+                (long long)max_win, (long long)free_bytes);
+      return rc;
+    }
   }
-  if ((rc = dev_alloc(ctx, (void **)&win_indices, sizeof(int32_t) * max_win)) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&win_data, sizeof(float) * max_win)) != ALS_OK) {
-    set_error("als_csr_transpose: a column window of %lld nonzeros does not fit in device memory (%lld bytes free)",
-              (long long)max_win, (long long)free_bytes);
-    return rc;
-  }
-  iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, max_seg);
+  int32_t *out_indices = t->host ? win_indices : t->indices;
+  float *out_data = t->host ? win_data : t->data;
+  iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, max_piece);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   for (const auto &w : windows) {
     const int64_t c0 = w.first, c1 = w.second, wn = ip[c1] - ip[c0];
     if (wn == 0) continue;
-    ALS_CUDA(cudaMemcpyAsync(next, out_ip, sizeof(long long) * (cols + 1), cudaMemcpyDeviceToDevice, ctx->stream));
-    rc = for_each_segment(ctx, in, [&](size_t, const als_csr *S) -> int {
-      const int64_t n = S->nnz;
-      if (n == 0) return ALS_OK;
-      size_t tb = tmp_bytes;
-      ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, S->indices, keys_out, vals_in, vals_out, (int)n, 0, end_bit, ctx->stream));
-      scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
-          vals_out, keys_out, n, S->indptr, (int)S->rows, S->row_offset - in->row_offset, S->data, next, win_indices, win_data,
-          (int32_t)c0, (int32_t)c1, ip[c0]);
-      ALS_CUDA(cudaGetLastError());
-      advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, n, next);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches += 2;
+    ALS_CUDA(cudaMemcpyAsync(next, ip.data(), sizeof(int64_t) * (cols + 1), cudaMemcpyHostToDevice, ctx->stream));
+    rc = for_each_segment(ctx, in, [&](size_t s, const als_csr *S) -> int {
+      for (const Piece &pc : pieces[s]) {
+        if (pc.n == 0) continue;
+        ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, S->indices + pc.b0, keys_out, vals_in, vals_out, (int)pc.n,
+                                                 0, end_bit, ctx->stream));
+        scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
+            vals_out, keys_out, pc.n, S->indptr + pc.r0, (int)(pc.r1 - pc.r0), S->row_offset - in->row_offset + pc.r0,
+            S->data + pc.b0, next, out_indices, out_data, (int32_t)c0, (int32_t)c1, ip[c0]);
+        ALS_CUDA(cudaGetLastError());
+        advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, pc.n, next);
+        ALS_CUDA(cudaGetLastError());
+        ctx->launches += 2;
+      }
       return ALS_OK;
     });
     if (rc != ALS_OK) return rc;
-    // stream ordered: the next window's scatter starts after these copies
-    ALS_CUDA(cudaMemcpyAsync(t->indices + ip[c0], win_indices, sizeof(int32_t) * wn, cudaMemcpyDeviceToHost, ctx->stream));
-    ALS_CUDA(cudaMemcpyAsync(t->data + ip[c0], win_data, sizeof(float) * wn, cudaMemcpyDeviceToHost, ctx->stream));
+    if (t->host) {  // stream ordered: the next window's scatter starts after these copies
+      ALS_CUDA(cudaMemcpyAsync(t->indices + ip[c0], win_indices, sizeof(int32_t) * wn, cudaMemcpyDeviceToHost, ctx->stream));
+      ALS_CUDA(cudaMemcpyAsync(t->data + ip[c0], win_data, sizeof(float) * wn, cudaMemcpyDeviceToHost, ctx->stream));
+    }
   }
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (void *p : {(void *)next, (void *)out_ip, (void *)keys_out, (void *)vals_in, (void *)vals_out, tmp, (void *)win_indices,
+  for (void *p : {(void *)next, (void *)keys_out, (void *)vals_in, (void *)vals_out, tmp, (void *)win_indices,
                   (void *)win_data})
-    dev_free(ctx, p);
-  // the values are the input's: so is their range
-  if ((rc = dev_alloc(ctx, (void **)&t->wmax_dev, 2 * sizeof(unsigned))) != ALS_OK) return rc;
-  ALS_CUDA(cudaMemcpyAsync(t->wmax_dev, in->wmax_dev, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, ctx->stream));
-  t->wmax_valid = in->wmax_valid;
-  t->neg_w_known = in->neg_w_known;
-  t->has_neg_w = in->has_neg_w;
-  return make_segments(ctx, t, ip.data());
+    dev_free(ctx, p);  // stream ordered: after the kernels and copies above
+  if (t->host) {  // the values are the input's: so is their range
+    if ((rc = dev_alloc(ctx, (void **)&t->wmax_dev, 2 * sizeof(unsigned))) != ALS_OK) return rc;
+    ALS_CUDA(cudaMemcpyAsync(t->wmax_dev, in->wmax_dev, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, ctx->stream));
+    t->wmax_valid = in->wmax_valid;
+    t->neg_w_known = in->neg_w_known;
+    t->has_neg_w = in->has_neg_w;
+  }
+  return csr_layout(ctx, t, ip.data());
 }
 
 }  // namespace
@@ -427,6 +371,28 @@ int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip) {
   return ALS_OK;
 }
 
+int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip) {
+  if (c->host || needs_segments(ctx, c->nnz)) return make_segments(ctx, c, ip);
+  std::vector<int32_t> ip32(ip, ip + c->rows + 1);
+  int rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (c->rows + 1));
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * ip32.size(), cudaMemcpyHostToDevice, ctx->stream));
+  rc = build_schedule(ctx, c, ip32.data());
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `ip32` dies here
+  return rc;
+}
+
+int csr_alloc(als_ctx *ctx, als_csr *c) {
+  const int64_t n = std::max<int64_t>(c->nnz, 1);
+  if (!c->host) {
+    int rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * n);
+    return rc != ALS_OK ? rc : dev_alloc(ctx, (void **)&c->data, sizeof(float) * n);
+  }
+  cudaError_t e = cudaMallocHost((void **)&c->indices, sizeof(int32_t) * n);
+  if (e == cudaSuccess) e = cudaMallocHost((void **)&c->data, sizeof(float) * n);
+  return e == cudaSuccess ? ALS_OK : cuda_fail(e, "cudaMallocHost (host-resident CSR)", __FILE__, __LINE__);
+}
+
 int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out) {
   out.assign((size_t)c->rows + 1, 0);
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -454,28 +420,11 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   t->rows = cols;
   t->cols = rows;
   t->nnz = nnz;
+  t->host = in->host;  // the transpose of a host-resident CSR is host-resident, built one column window at a time
   int rc;
-  if (in->host) {  // host-resident in, host-resident out, built one column window at a time
-    t->host = true;
-    const size_t bytes = sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1);
-    cudaError_t e = cudaMallocHost((void **)&t->indices, bytes);
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&t->data, bytes);
-    if (e != cudaSuccess) {
-      als_csr_destroy(t);
-      return cuda_fail(e, "cudaMallocHost (host-resident transpose)", __FILE__, __LINE__);
-    }
-    if ((rc = transpose_host(ctx, in, t)) != ALS_OK) {
+  if (in->host || !in->segs.empty() || needs_segments(ctx, nnz)) {
+    if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t)) != ALS_OK) {
       cudaStreamSynchronize(ctx->stream);  // D2H copies of a window may still be landing in t's arrays
-      als_csr_destroy(t);
-      return rc;
-    }
-    *out = t;
-    return ALS_OK;
-  }
-  if (!in->segs.empty() || needs_segments(ctx, nnz)) {
-    if ((rc = dev_alloc(ctx, (void **)&t->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&t->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-        (rc = transpose_segmented(ctx, in, t)) != ALS_OK) {
       als_csr_destroy(t);
       return rc;
     }
