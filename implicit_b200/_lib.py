@@ -130,6 +130,14 @@ def check(rc):
         raise AlsError(rc, msg or f"libals_b200 call failed with code {rc}")
 
 
+def check_half(rc, bad):
+    """check() for a Cholesky half: a row that is not positive definite (its index in `bad`) raises ValueError like
+    _als.pyx:136-138."""
+    if rc == ALS_E_NOT_POSDEF:
+        raise ValueError("cholesky failed on row %i. Try increasing the regularization parameter." % bad.value)
+    check(rc)
+
+
 def ptr(a):
     """Raw data pointer of a C-contiguous numpy array (None -> NULL)."""
     if a is None:
@@ -506,9 +514,7 @@ def least_squares(ctx, Cui, X, Y, regularization):
     """_als.least_squares(Cui, X, Y, regularization): raises ValueError like _als.pyx:136-138."""
     bad = c_i64(-1)
     rc = ctx.lib.als_least_squares(ctx.h, Cui.h, X.h, Y.h, float(regularization), ctypes.byref(bad))
-    if rc == ALS_E_NOT_POSDEF:
-        raise ValueError("cholesky failed on row %i. Try increasing the regularization parameter." % bad.value)
-    check(rc)
+    check_half(rc, bad)
 
 
 def whitened_factors(ctx, Y, regularization):
@@ -536,9 +542,7 @@ def solver_status(ctx):
     """Synchronises; raises ValueError for a bad row of this rank, AlsError when another rank failed."""
     bad, anyf = c_i64(-1), c_int(0)
     rc = ctx.lib.als_solver_status(ctx.h, ctypes.byref(bad), ctypes.byref(anyf))
-    if rc == ALS_E_NOT_POSDEF:
-        raise ValueError("cholesky failed on row %i. Try increasing the regularization parameter." % bad.value)
-    check(rc)
+    check_half(rc, bad)
     if anyf.value:
         raise AlsError(ALS_E_NOT_POSDEF, "another rank failed in this iteration (see its error message)")
 
@@ -550,9 +554,7 @@ def half_pregram(ctx, Cui, X, Y, regularization, use_cg, cg_steps=3):
         return
     bad = c_i64(-1)
     rc = ctx.lib.als_least_squares_pregram(ctx.h, Cui.h, X.h, Y.h, float(regularization), ctypes.byref(bad))
-    if rc == ALS_E_NOT_POSDEF:
-        raise ValueError("cholesky failed on row %i. Try increasing the regularization parameter." % bad.value)
-    check(rc)
+    check_half(rc, bad)
 
 
 def least_squares_with_gramian(ctx, YtY, Cui, X, Y, regularization):
@@ -561,9 +563,7 @@ def least_squares_with_gramian(ctx, YtY, Cui, X, Y, regularization):
     bad = c_i64(-1)
     rc = ctx.lib.als_least_squares_with_gramian(ctx.h, ptr(YtY), Cui.h, X.h, Y.h, float(regularization),
                                                 ctypes.byref(bad))
-    if rc == ALS_E_NOT_POSDEF:
-        raise ValueError("cholesky failed on row %i. Try increasing the regularization parameter." % bad.value)
-    check(rc)
+    check_half(rc, bad)
 
 
 def least_squares_cg(ctx, Cui, X, Y, regularization, cg_steps=3):

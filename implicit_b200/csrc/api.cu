@@ -1074,36 +1074,57 @@ ALS_API int als_gramian(als_ctx *ctx, const als_factors *Y, float *G_host) {
   return ALS_OK;
 }
 
-static int finish_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, double reg,
-                           int64_t *bad_row) {
-  int rc = launch_regularize(ctx, Y->f, Y->ld, (float)reg);
-  if (rc != ALS_OK) return rc;
-  rc = launch_cholesky(ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  long long bad = -1;
-  ALS_CUDA(cudaMemcpyAsync(&bad, ctx->bad_row, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+// Reads the first row whose normal equations were not positive definite from bad_row[0, n) (n = 1: the half just run;
+// 2: also the halves since the last als_solver_status) into *row, -1 for none (synchronises).  A row found is reported
+// here and now: both slots are cleared, so nothing is left for a later call to find.
+static int take_bad_row(als_ctx *ctx, int n, int64_t *row) {
+  long long bad[2] = {LLONG_MAX, LLONG_MAX};
+  ALS_CUDA(cudaMemcpyAsync(bad, ctx->bad_row, n * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (bad_row) *bad_row = (bad == LLONG_MAX) ? -1 : (int64_t)bad;
-  if (bad != LLONG_MAX) {
-    // reported here and now: nothing is left for a later als_solver_status to find
-    const long long init[2] = {LLONG_MAX, LLONG_MAX};
-    ALS_CUDA(cudaMemcpyAsync(ctx->bad_row, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  const long long first = std::min(bad[0], bad[1]);
+  if (row) *row = first == LLONG_MAX ? -1 : (int64_t)first;
+  if (first == LLONG_MAX) return ALS_OK;
+  const long long init[2] = {LLONG_MAX, LLONG_MAX};
+  ALS_CUDA(cudaMemcpyAsync(ctx->bad_row, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  set_error("cholesky failed on row %lld: normal equations not positive definite. Try increasing the "
+            "regularization parameter.", first);
+  return ALS_E_NOT_POSDEF;
+}
+
+enum class Gram { kCompute, kHost, kPresent };  // the Gramian of a half: Y^T Y from Y, the caller's YtY_host, or ctx->G
+enum class Solver { kCholesky, kCg };
+
+// One half-iteration: the checks, the Gramian, G + reg I and the solver.  With sync_bad_row a Cholesky half reads its
+// bad row back and fails with ALS_E_NOT_POSDEF; without, the row waits in bad_row for als_solver_status.
+static int solve_half(const char *who, als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y, Gram gram,
+                      const float *YtY_host, double reg, Solver solver, int cg_steps, bool sync_bad_row, int64_t *bad_row) {
+  int rc = check_half(who, ctx, C, X, Y);
+  if (rc != ALS_OK) return rc;
+  ALS_REQUIRE(solver != Solver::kCg || cg_steps >= 0, "%s: cg_steps < 0", who);
+  ALS_REQUIRE(gram != Gram::kHost || YtY_host, "%s: YtY is NULL", who);
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  if (gram == Gram::kCompute) {
+    rc = launch_gramian(ctx, Y);
+    if (rc != ALS_OK) return rc;
+  } else if (gram == Gram::kHost) {
+    std::vector<float> tmp((size_t)Y->ld * Y->ld, 0.f);
+    for (int i = 0; i < Y->f; ++i) memcpy(tmp.data() + (size_t)i * Y->ld, YtY_host + (size_t)i * Y->f, sizeof(float) * Y->f);
+    ALS_CUDA(cudaMemcpyAsync(ctx->G, tmp.data(), sizeof(float) * tmp.size(), cudaMemcpyHostToDevice, ctx->stream));
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    set_error("cholesky failed on row %lld: normal equations not positive definite. Try increasing the "
-              "regularization parameter.", bad);
-    return ALS_E_NOT_POSDEF;
   }
-  return ALS_OK;
+  rc = launch_regularize(ctx, Y->f, Y->ld, (float)reg);
+  if (rc != ALS_OK) return rc;
+  if (solver == Solver::kCg) return launch_cg(ctx, C, X, Y, cg_steps);
+  rc = launch_cholesky(ctx, C, X, Y);
+  if (rc != ALS_OK || !sync_bad_row) return rc;
+  return take_bad_row(ctx, 1, bad_row);
 }
 
 ALS_API int als_least_squares(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
                               double regularization, int64_t *bad_row) {
-  int rc = check_half("als_least_squares", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  rc = launch_gramian(ctx, Y);
-  if (rc != ALS_OK) return rc;
-  return finish_cholesky(ctx, C, X, Y, regularization, bad_row);
+  return solve_half("als_least_squares", ctx, C, X, Y, Gram::kCompute, nullptr, regularization, Solver::kCholesky, 0,
+                    true, bad_row);
 }
 
 // W = Y (2^14 P) / 2^14 and Z = Y G^-1 of the short-row path, downloaded (tests and tools: the wgmma apply of
@@ -1166,86 +1187,54 @@ ALS_API int als_gramian_shard(als_ctx *ctx, const als_factors *Y, int64_t row0, 
 
 ALS_API int als_least_squares_pregram(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
                                       double regularization, int64_t *bad_row) {
-  int rc = check_half("als_least_squares_pregram", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  return finish_cholesky(ctx, C, X, Y, regularization, bad_row);
+  return solve_half("als_least_squares_pregram", ctx, C, X, Y, Gram::kPresent, nullptr, regularization,
+                    Solver::kCholesky, 0, true, bad_row);
 }
 
 // The multi-GPU fit loop: the same half as als_least_squares_pregram without the host round trip for bad_row, so
 // the next half (and its collectives) are queued while this one runs; failures are collected by als_solver_status.
 ALS_API int als_least_squares_pregram_async(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
                                             double regularization) {
-  int rc = check_half("als_least_squares_pregram_async", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  rc = launch_regularize(ctx, Y->f, Y->ld, (float)regularization);
-  if (rc != ALS_OK) return rc;
-  return launch_cholesky(ctx, C, X, Y);
+  return solve_half("als_least_squares_pregram_async", ctx, C, X, Y, Gram::kPresent, nullptr, regularization,
+                    Solver::kCholesky, 0, false, nullptr);
 }
 
 ALS_API int als_solver_status(als_ctx *ctx, int64_t *bad_row, int *any_rank_failed) {
   ALS_REQUIRE(ctx, "als_solver_status: NULL context");
   ALS_CUDA(cudaSetDevice(ctx->device));
-  long long bad[2] = {LLONG_MAX, LLONG_MAX};
   int32_t st = 0;
   float flag = 0.f;
-  ALS_CUDA(cudaMemcpyAsync(bad, ctx->bad_row, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaMemcpyAsync(&st, ctx->status, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
   if (ctx->gram_ld)
     ALS_CUDA(cudaMemcpyAsync(&flag, ctx->G + ctx->gram_ld * ctx->gram_ld, sizeof(flag), cudaMemcpyDeviceToHost, ctx->stream));
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  const long long first = std::min(bad[0], bad[1]);
-  if (bad_row) *bad_row = first == LLONG_MAX ? -1 : (int64_t)first;
-  if (any_rank_failed) *any_rank_failed = (st != 0 || flag > 0.f || first != LLONG_MAX) ? 1 : 0;
-  const long long init[2] = {LLONG_MAX, LLONG_MAX};  // start a new collection period
-  ALS_CUDA(cudaMemcpyAsync(ctx->bad_row, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  int64_t first = -1;
+  const int rc = take_bad_row(ctx, 2, &first);  // synchronises: st and flag have landed too
+  if (rc != ALS_OK && rc != ALS_E_NOT_POSDEF) return rc;
+  if (bad_row) *bad_row = first;
+  if (any_rank_failed) *any_rank_failed = (st != 0 || flag > 0.f || first >= 0) ? 1 : 0;
+  // start a new collection period
   ALS_CUDA(cudaMemsetAsync(ctx->status, 0, sizeof(int32_t), ctx->stream));
   if (ctx->gram_ld) ALS_CUDA(cudaMemsetAsync(ctx->G + ctx->gram_ld * ctx->gram_ld, 0, sizeof(float), ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (first != LLONG_MAX) {
-    set_error("cholesky failed on row %lld: normal equations not positive definite. Try increasing the "
-              "regularization parameter.", first);
-    return ALS_E_NOT_POSDEF;
-  }
-  return ALS_OK;
+  return rc;
 }
 
 ALS_API int als_least_squares_cg_pregram(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
                                          float regularization, int cg_steps) {
-  int rc = check_half("als_least_squares_cg_pregram", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_REQUIRE(cg_steps >= 0, "als_least_squares_cg_pregram: cg_steps < 0");
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  rc = launch_regularize(ctx, Y->f, Y->ld, regularization);
-  if (rc != ALS_OK) return rc;
-  return launch_cg(ctx, C, X, Y, cg_steps);
+  return solve_half("als_least_squares_cg_pregram", ctx, C, X, Y, Gram::kPresent, nullptr, regularization, Solver::kCg,
+                    cg_steps, false, nullptr);
 }
 
 ALS_API int als_least_squares_with_gramian(als_ctx *ctx, const float *YtY_host, const als_csr *C, als_factors *X,
                                            const als_factors *Y, double regularization, int64_t *bad_row) {
-  int rc = check_half("als_least_squares_with_gramian", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_REQUIRE(YtY_host, "als_least_squares_with_gramian: YtY is NULL");
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  std::vector<float> tmp((size_t)Y->ld * Y->ld, 0.f);
-  for (int i = 0; i < Y->f; ++i) memcpy(tmp.data() + (size_t)i * Y->ld, YtY_host + (size_t)i * Y->f, sizeof(float) * Y->f);
-  ALS_CUDA(cudaMemcpyAsync(ctx->G, tmp.data(), sizeof(float) * tmp.size(), cudaMemcpyHostToDevice, ctx->stream));
-  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  return finish_cholesky(ctx, C, X, Y, regularization, bad_row);
+  return solve_half("als_least_squares_with_gramian", ctx, C, X, Y, Gram::kHost, YtY_host, regularization,
+                    Solver::kCholesky, 0, true, bad_row);
 }
 
 ALS_API int als_least_squares_cg(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y,
                                  float regularization, int cg_steps) {
-  int rc = check_half("als_least_squares_cg", ctx, C, X, Y);
-  if (rc != ALS_OK) return rc;
-  ALS_REQUIRE(cg_steps >= 0, "als_least_squares_cg: cg_steps < 0");
-  ALS_CUDA(cudaSetDevice(ctx->device));
-  rc = launch_gramian(ctx, Y);
-  if (rc != ALS_OK) return rc;
-  rc = launch_regularize(ctx, Y->f, Y->ld, regularization);
-  if (rc != ALS_OK) return rc;
-  return launch_cg(ctx, C, X, Y, cg_steps);
+  return solve_half("als_least_squares_cg", ctx, C, X, Y, Gram::kCompute, nullptr, regularization, Solver::kCg, cg_steps,
+                    false, nullptr);
 }
 
 ALS_API int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors *X, const als_factors *Y,

@@ -2,18 +2,20 @@
 //
 // One warp owns one row u of the CSR at a time (persistent warps pull rows, longest first, from an
 // atomic work counter):
-//   gather   the factor rows Y[i] of the row's nonzeros are staged 8 at a time into shared memory
-//            with 16-byte cp.async copies (3-deep ring per warp, prefetched across row boundaries;
-//            indices / confidences are prefetched 32 at a time into registers one block ahead);
+//   gather   the factor rows Y[i] of the row's nonzeros are staged 16 at a time (one k-step) into shared
+//            memory with 16-byte cp.async copies (Cfg16: 2 stages per warp, the next row's first two
+//            k-steps issued before this row is factored; indices / confidences are prefetched 32 at a
+//            time into registers one block ahead);
 //   A, b     A_u = (Y^T Y + lambda I) + sum_k (|c_k| - 1) y_k y_k^T is accumulated in REGISTERS as the
-//            upper-triangular set of 16x8 mma.sync.m16n8k8 TF32 tiles, with the 3xTF32 split
-//            (hi*hi + hi*lo + lo*hi) so the result is fp32-faithful (plain TF32 would miss the 1e-4
-//            parity bar); b_u = sum_{c_k > 0} c_k y_k rides along in fp32 FMAs;
+//            upper-triangular set of 16x8 mma.sync.m16n8k16 tiles on the fp16 split of sigma sqrt|w| y
+//            (hi*hi + hi*lo + lo*hi, both parts rounded to nearest), i.e. as sigma^2 A_u with sigma a
+//            power of two chosen per half (DESIGN 4.1); b_u = sum_{c_k > 0} c_k y_k rides along in fp32
+//            FMAs;
 //   solve    a right-looking blocked Cholesky with 8-row panels: each panel is spilled to shared
 //            memory, one lane owns one panel column (the rhs slice and 8 unit vectors ride along as
 //            extra columns), the 8 pivots are eliminated LDL^T-style with warp shuffles and the rows
-//            scaled by 1/sqrt(d) afterwards; the trailing matrix is updated IN REGISTERS by the same
-//            3xTF32 mma tiles; the back substitution resolves a panel at a time with the inverse of
+//            scaled by 1/sqrt(d) afterwards; the trailing matrix is updated IN REGISTERS by 3xTF32
+//            m16n8k8 tiles; the back substitution resolves a panel at a time with the inverse of
 //            its diagonal block (the forward-substituted unit vectors) on the packed U in shared memory.
 // Giant rows are split into chunks whose partial (A, b) go to global scratch and are summed in a
 // fixed order by a second "finish" launch, so results do not depend on scheduling.
@@ -229,6 +231,7 @@ __global__ void __launch_bounds__(256) factors_absmax_kernel(const float4 *__res
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
 
+// before every half of every width family: the counters are zeroed (only the narrow family reads them)
 __global__ void init_solver_scalars(int32_t *counters, long long *bad_row) {
   if (threadIdx.x < 16) counters[threadIdx.x] = 0;
   if (threadIdx.x == 0) {
@@ -261,12 +264,11 @@ __global__ void reset_segment_counters(int32_t *counters) {
   if (t < 16 && t != kCtrWhitenOk && t != kCtrHasNan && t != kCtrYAbsMax) counters[t] = 0;
 }
 
-// One half over C, which may be a list of row-block segments.  Everything that affects rounding is decided once for the
-// whole matrix (bad_row reset, max |y|, max ||c| - 1|, the long-row kernel, whether short rows take the whitened path,
-// the whitening itself); the deferred list, its counters and the giant-row slots are per segment.
+// The narrow family (ld <= 64) over C, which may be a list of row-block segments.  Everything that affects rounding is
+// decided once for the whole matrix (max |y|, max ||c| - 1|, the long-row kernel, whether short rows take the whitened
+// path, the whitening itself); the deferred list and its counters are per segment.
 template <int NB>
 int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_factors *Y) {
-  using C = Cfg<NB>;
   const int dbg = debug_flags();
   const int smem = Cfg16<NB>::WARP_FLOATS * kWarpsPerCta * (int)sizeof(float);
   auto kern = cholesky_half_kernel<NB>;
@@ -278,17 +280,6 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     return ALS_E_CUDA;
   }
   const std::vector<const als_csr *> segs = segments_of(Cm);
-  int64_t max_slots = 0;
-  for (const als_csr *S : segs) max_slots = std::max(max_slots, S->n_slots);
-  float *slots = nullptr;
-  if (max_slots) {
-    int rc = ensure_scratch(ctx, max_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
-    if (rc != ALS_OK) return rc;
-    slots = (float *)ctx->scratch;
-  }
-  init_solver_scalars<<<1, 32, 0, ctx->stream>>>(ctx->counters, ctx->bad_row);
-  ALS_CUDA(cudaGetLastError());
-  ctx->launches++;
   // the range of the fp16-split operands: max |y| of this half (one pass over Y) and max | |c| - 1 | of the CSR
   // (one pass over its values, cached in the handle until als_csr_scale changes them)
   unsigned *yabsmax = reinterpret_cast<unsigned *>(ctx->counters + kCtrYAbsMax);
@@ -335,10 +326,24 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     // of Y costs
     if (n_short * 16 < Y->rows) short_max = 0;
   }
-  const int max_grid = ctx->sm_count * ctas_per_sm;
+  CholFamily fam;
+  fam.slot_floats = Cfg<NB>::SLOT_FLOATS;
+  fam.items_per_cta = kWarpsPerCta;
+  fam.max_grid = (int64_t)ctx->sm_count * ctas_per_sm;
+  // items[0, n) of S on `stream`: n_dev, when set, replaces n on the device; counter: the work counter they pull from
+  auto kernel = [&](const als_csr *S, const WorkItem *items, int n, const int32_t *n_dev, int counter, int pass, int grid,
+                    float *slots, cudaStream_t stream) {
+    kern<<<grid, 32 * kWarpsPerCta, smem, stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg, items, n,
+                                                     n_dev, ctx->counters + counter, slots, ctx->bad_row, pass, dbg,
+                                                     X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+  };
+  fam.launch = [&](const als_csr *S, const WorkItem *items, int n, int pass, int grid, float *slots, float *) {
+    kernel(S, items, n, nullptr, pass ? kCtrFinish : kCtrMain, pass, grid, slots, ctx->stream);
+  };
+  auto grid_of = [&](int64_t n) { return (int)std::min<int64_t>(ceil_div(n, kWarpsPerCta), fam.max_grid); };
   // every launch below reads S on ctx->stream, or on aux / the class streams joined back into it by ev_join before the
   // segment ends, which is what for_each_segment needs to reuse a ring slot of a host-resident C
-  return for_each_segment(ctx, Cm, [&](size_t s, const als_csr *S) -> int {
+  fam.pass0 = [&](size_t s, const als_csr *S, float *slots) -> int {
     if (s > 0) {
       reset_segment_counters<<<1, 32, 0, ctx->stream>>>(ctx->counters);
       ALS_CUDA(cudaGetLastError());
@@ -346,68 +351,92 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     }
     const int64_t n_main = short_max > 0 ? S->le_begin[short_class] : S->n_work;
     const bool seg_short = short_max > 0 && S->n_work > n_main;
-    if (S->n_work) {
-      ProfScope prof(ctx, kProfCholesky);
-      // The short-row side (whitening, the short-row kernels, the second pass of the full-size kernel over what they
-      // hand back) runs on the aux stream.  The single-CTA factorisation of G is launched first and hides behind the
-      // full-size kernel; the rest moves in as that kernel's persistent CTAs run out of long rows.
-      const bool overlap = seg_short && n_main > 0 && !ctx->knobs.short_serial;
-      cudaStream_t side = overlap ? ctx->aux : ctx->stream;
-      if (short_max > 0) {
-        if (overlap) {
-          ALS_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
-          ALS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
-        }
-        if (s == 0) {  // once per half: the later segments find W and Z in place
-          int rc = short_rows_prepare(ctx, Y, side);
-          if (rc != ALS_OK) return rc;
-        }
+    if (!S->n_work) return ALS_OK;
+    ProfScope prof(ctx, kProfCholesky);
+    // The short-row side (whitening, the short-row kernels, the second pass of the full-size kernel over what they
+    // hand back) runs on the aux stream.  The single-CTA factorisation of G is launched first and hides behind the
+    // full-size kernel; the rest moves in as that kernel's persistent CTAs run out of long rows.
+    const bool overlap = seg_short && n_main > 0 && !ctx->knobs.short_serial;
+    cudaStream_t side = overlap ? ctx->aux : ctx->stream;
+    if (short_max > 0) {
+      if (overlap) {
+        ALS_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+        ALS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->ev_fork, 0));
       }
-      if (n_main && long_tc) {
-        // whole rows: normal equations on the wgmma tensor cores; chunks of giant rows: the mma.sync kernel
-        int rc = launch_cholesky_tc(ctx, S, X, Y, n_main, Cm->wmax_dev, ctx->stream);
+      if (s == 0) {  // once per half: the later segments find W and Z in place
+        int rc = short_rows_prepare(ctx, Y, side);
         if (rc != ALS_OK) return rc;
-        if (S->n_slots) {
-          const int grid = (int)std::min<int64_t>(ceil_div(S->n_slots, kWarpsPerCta), max_grid);
-          kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg, S->chunks,
-                                                         (int)S->n_slots, nullptr, ctx->counters + kCtrChunks, slots, ctx->bad_row,
-                                                         0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-          ALS_CUDA(cudaGetLastError());
-          ctx->launches++;
-        }
-      } else if (n_main) {
-        const int grid = (int)std::min<int64_t>(ceil_div(n_main, kWarpsPerCta), max_grid);
-        kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
-                                                              S->work, (int)n_main, nullptr, ctx->counters + kCtrMain,
-                                                              slots, ctx->bad_row, 0, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-        ALS_CUDA(cudaGetLastError());
-        ctx->launches++;
-      }
-      if (seg_short) {
-        int rc = short_rows_launch(ctx, S, X, Y, n_main, short_max, side);
-        if (rc != ALS_OK) return rc;
-        // whatever the short-row kernels handed back (negative weights, chunks of giant rows, G not PD)
-        const int grid = (int)std::min<int64_t>(ceil_div(S->n_work - n_main, kWarpsPerCta), max_grid);
-        kern<<<grid, 32 * kWarpsPerCta, smem, side>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
-                                                       ctx->deferred, 0, ctx->counters + kCtrDeferredCount,
-                                                       ctx->counters + kCtrDeferredWork, slots, ctx->bad_row, 0, dbg,
-                                                       X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
-        ALS_CUDA(cudaGetLastError());
-        ctx->launches++;
-        if (overlap) {
-          ALS_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
-          ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
-        }
       }
     }
+    if (n_main && long_tc) {
+      // whole rows: normal equations on the wgmma tensor cores; chunks of giant rows: the mma.sync kernel
+      int rc = launch_cholesky_tc(ctx, S, X, Y, n_main, Cm->wmax_dev, ctx->stream);
+      if (rc != ALS_OK) return rc;
+      if (S->n_slots) {
+        kernel(S, S->chunks, (int)S->n_slots, nullptr, kCtrChunks, 0, grid_of(S->n_slots), slots, side);
+        ALS_CUDA(cudaGetLastError());
+        ctx->launches++;
+      }
+    } else if (n_main) {
+      fam.launch(S, S->work, (int)n_main, 0, grid_of(n_main), slots, nullptr);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
+    if (seg_short) {
+      int rc = short_rows_launch(ctx, S, X, Y, n_main, short_max, side);
+      if (rc != ALS_OK) return rc;
+      // whatever the short-row kernels handed back (negative weights, chunks of giant rows, G not PD)
+      kernel(S, ctx->deferred, 0, ctx->counters + kCtrDeferredCount, kCtrDeferredWork, 0, grid_of(S->n_work - n_main),
+             slots, side);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+      if (overlap) {
+        ALS_CUDA(cudaEventRecord(ctx->ev_join, ctx->aux));
+        ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+      }
+    }
+    return ALS_OK;
+  };
+  return run_cholesky_half(ctx, Cm, Y, fam);
+}
+
+}  // namespace
+
+int run_cholesky_half(als_ctx *ctx, const als_csr *C, const als_factors *Y, const CholFamily &fam) {
+  // row-block segments run one after the other: one scratch block covers the largest, with the giant-row slots first
+  int64_t max_slots = 0, n_ws = 0;
+  for (const als_csr *S : segments_of(C)) {
+    max_slots = std::max(max_slots, S->n_slots);
+    if (fam.ws_floats) n_ws = std::max(n_ws, std::min(std::max(S->n_work, S->n_finish), fam.max_grid));
+  }
+  const int64_t floats = max_slots * fam.slot_floats + n_ws * fam.ws_floats;
+  float *slots = nullptr, *ws = nullptr;
+  if (floats) {
+    const int64_t bytes = floats * (int64_t)sizeof(float);
+    int rc = ensure_scratch(ctx, bytes);
+    if (rc != ALS_OK) {
+      set_error("cholesky: factors=%d needs %.2f GB of device scratch (%lld giant-row chunks and %lld workspaces of %.2f MB "
+                "each) and the allocation failed; split the rows into smaller calls or use the CG solver",
+                Y->f, bytes / 1e9, (long long)max_slots, (long long)n_ws, fam.slot_floats * 4 / 1e6);
+      return rc;
+    }
+    slots = (float *)ctx->scratch;
+    ws = slots + max_slots * fam.slot_floats;
+  }
+  auto grid_of = [&](int64_t n) { return (int)std::min<int64_t>(ceil_div(n, fam.items_per_cta), fam.max_grid); };
+  return for_each_segment(ctx, C, [&](size_t s, const als_csr *S) -> int {
+    if (fam.pass0) {
+      int rc = fam.pass0(s, S, slots);
+      if (rc != ALS_OK) return rc;
+    } else if (S->n_work) {
+      ProfScope prof(ctx, kProfCholesky);
+      fam.launch(S, S->work, (int)S->n_work, 0, grid_of(S->n_work), slots, ws);
+      ALS_CUDA(cudaGetLastError());
+      ctx->launches++;
+    }
     if (S->n_finish) {
-      const int64_t want = ceil_div(S->n_finish, kWarpsPerCta);
-      const int grid = (int)std::min<int64_t>(want, (int64_t)max_grid);
       ProfScope prof(ctx, kProfCholFinish);
-      kern<<<grid, 32 * kWarpsPerCta, smem, ctx->stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg,
-                                                            S->finish, (int)S->n_finish, nullptr,
-                                                            ctx->counters + kCtrFinish, slots,
-                                                            ctx->bad_row, 1, dbg, X->peers_dev, X->n_peers, Cm->wmax_dev, yabsmax);
+      fam.launch(S, S->finish, (int)S->n_finish, 1, grid_of(S->n_finish), slots, ws);
       ALS_CUDA(cudaGetLastError());
       ctx->launches++;
     }
@@ -415,21 +444,28 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
   });
 }
 
-}  // namespace
-
 int launch_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y) {
   if (X->ld != Y->ld) {
     set_error("cholesky: X and Y strides differ (%d vs %d)", X->ld, Y->ld);
     return ALS_E_INVALID;
   }
+  if (Y->ld > 1024 || (Y->ld > 128 && Y->ld % 64)) {
+    set_error("cholesky: padded factors %d out of range", Y->ld);
+    return ALS_E_INVALID;
+  }
+  init_solver_scalars<<<1, 32, 0, ctx->stream>>>(ctx->counters, ctx->bad_row);
+  ALS_CUDA(cudaGetLastError());
+  ctx->launches++;
   switch (Y->ld / 16) {
     case 1: return run_cholesky<1>(ctx, C, X, Y);
     case 2: return run_cholesky<2>(ctx, C, X, Y);
     case 3: return run_cholesky<3>(ctx, C, X, Y);
     case 4: return run_cholesky<4>(ctx, C, X, Y);
-    default:
-      if (Y->ld <= 128) return launch_cholesky_wide(ctx, C, X, Y);  // 64 < padded factors <= 128: cholesky_wide.cu
-      return launch_cholesky_xwide(ctx, C, X, Y);                    // 256 ... 1024: cholesky_xwide.cu
+    case 5: return launch_cholesky_wide<5>(ctx, C, X, Y);
+    case 6: return launch_cholesky_wide<6>(ctx, C, X, Y);
+    case 7: return launch_cholesky_wide<7>(ctx, C, X, Y);
+    case 8: return launch_cholesky_wide<8>(ctx, C, X, Y);
+    default: return launch_cholesky_xwide(ctx, C, X, Y);  // 256 ... 1024
   }
 }
 

@@ -5,8 +5,6 @@
 // This is the correctness path for wide models (recalculate_user / partial_fit on a factors=128 CG
 // model, `use_cg=False` at factors=100); the register-resident tensor-core kernel in cholesky.cu
 // covers factors <= 64, where BASELINE.json quotes the Cholesky metric.
-#include <limits.h>
-
 #include "common.h"
 
 namespace als {
@@ -172,57 +170,25 @@ cholesky_wide_kernel(const int32_t *__restrict__ indices, const float *__restric
   }
 }
 
-__global__ void init_bad_row(long long *bad_row) { bad_row[0] = LLONG_MAX; }
-
-template <int T>
-int run_wide(als_ctx *ctx, const als_csr *Cw, als_factors *X, const als_factors *Y) {
-  using C = WideCfg<T>;
-  const int smem = C::SMEM_FLOATS * (int)sizeof(float);
-  auto kern = cholesky_wide_kernel<T>;
-  ALS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const std::vector<const als_csr *> segs = segments_of(Cw);  // row-block segments: bad_row is reset once per half
-  int64_t max_slots = 0;
-  for (const als_csr *S : segs) max_slots = std::max(max_slots, S->n_slots);
-  float *slots = nullptr;
-  if (max_slots) {
-    int rc = ensure_scratch(ctx, max_slots * C::SLOT_FLOATS * (int64_t)sizeof(float));
-    if (rc != ALS_OK) return rc;
-    slots = (float *)ctx->scratch;
-  }
-  init_bad_row<<<1, 1, 0, ctx->stream>>>(ctx->bad_row);
-  ALS_CUDA(cudaGetLastError());
-  ctx->launches++;
-  const int per_sm = std::max(1, (227 * 1024) / (smem + 1024));
-  return for_each_segment(ctx, Cw, [&](size_t, const als_csr *Cm) -> int {
-    if (Cm->n_work) {
-      const int grid = (int)std::min<int64_t>(Cm->n_work, (int64_t)ctx->sm_count * per_sm);
-      ProfScope prof(ctx, kProfCholesky);
-      kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg, Cm->work,
-                                                      (int)Cm->n_work, slots, ctx->bad_row, 0, X->peers_dev, X->n_peers);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches++;
-    }
-    if (Cm->n_finish) {
-      const int grid = (int)std::min<int64_t>(Cm->n_finish, (int64_t)ctx->sm_count * per_sm);
-      ProfScope prof(ctx, kProfCholFinish);
-      kern<<<grid, kWideThreads, smem, ctx->stream>>>(Cm->indices, Cm->data, Y->d, X->d, Cm->row_offset, ctx->Greg,
-                                                      Cm->finish, (int)Cm->n_finish, slots, ctx->bad_row, 1, X->peers_dev, X->n_peers);
-      ALS_CUDA(cudaGetLastError());
-      ctx->launches++;
-    }
-    return ALS_OK;
-  });
-}
-
 }  // namespace
 
+template <int T>
 int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y) {
-  switch (Y->ld / 16) {
-    case 5: return run_wide<5>(ctx, C, X, Y);
-    case 6: return run_wide<6>(ctx, C, X, Y);
-    case 7: return run_wide<7>(ctx, C, X, Y);
-    default: return run_wide<8>(ctx, C, X, Y);  // launch_cholesky sends only padded factors 80 ... 128 here
-  }
+  const int smem = WideCfg<T>::SMEM_FLOATS * (int)sizeof(float);
+  auto kern = cholesky_wide_kernel<T>;
+  ALS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  CholFamily fam;
+  fam.slot_floats = WideCfg<T>::SLOT_FLOATS;
+  fam.max_grid = (int64_t)ctx->sm_count * std::max(1, (227 * 1024) / (smem + 1024));
+  fam.launch = [&](const als_csr *S, const WorkItem *items, int n, int pass, int grid, float *slots, float *) {
+    kern<<<grid, kWideThreads, smem, ctx->stream>>>(S->indices, S->data, Y->d, X->d, S->row_offset, ctx->Greg, items, n,
+                                                    slots, ctx->bad_row, pass, X->peers_dev, X->n_peers);
+  };
+  return run_cholesky_half(ctx, C, Y, fam);
 }
+template int launch_cholesky_wide<5>(als_ctx *, const als_csr *, als_factors *, const als_factors *);
+template int launch_cholesky_wide<6>(als_ctx *, const als_csr *, als_factors *, const als_factors *);
+template int launch_cholesky_wide<7>(als_ctx *, const als_csr *, als_factors *, const als_factors *);
+template int launch_cholesky_wide<8>(als_ctx *, const als_csr *, als_factors *, const als_factors *);
 
 }  // namespace als

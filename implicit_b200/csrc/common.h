@@ -261,8 +261,25 @@ int factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scal
 int launch_gramian(als_ctx *ctx, const als_factors *Y);                  // -> ctx->G
 int comm_allreduce_gramian(als_ctx *ctx, int n_floats);                   // sum ctx->G over ranks (comm.cu)
 int launch_regularize(als_ctx *ctx, int f, int ld, float lambda);         // ctx->G -> ctx->Greg
+// The Cholesky half: resets bad_row (folding the previous half's into bad_row[1]) and the counters, then hands the
+// half to the family of Y->ld: cholesky.cu (ld <= 64), cholesky_wide.cu (<= 128), cholesky_xwide.cu (<= 1024).
 int launch_cholesky(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);
-int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);   // 64 < ld <= 128
+// A width family of the Cholesky half, as the per-half driver run_cholesky_half sees it.
+struct CholFamily {
+  int64_t slot_floats = 0;  // one giant-row slot: a chunk's partial normal equations
+  int64_t ws_floats = 0;    // after the slots: one workspace of this many floats per resident CTA (0: none)
+  int items_per_cta = 1;    // work items one CTA takes at a time
+  int64_t max_grid = 0;     // the grid bound: CTAs resident on the device
+  // the family's kernel over items[0, n) on ctx->stream; pass 0: whole rows and chunks, pass 1: finish items
+  std::function<void(const als_csr *S, const WorkItem *items, int n, int pass, int grid, float *slots, float *ws)> launch;
+  // pass 0 of segment s in place of launch() over S->work (the narrow family: long rows, short rows, deferred items)
+  std::function<int(size_t s, const als_csr *S, float *slots)> pass0;
+};
+// Sizes the giant-row slots (and workspaces) once over the segments of C, then walks them: pass 0, then the finish
+// pass.  Y->f names the width in an allocation failure.
+int run_cholesky_half(als_ctx *ctx, const als_csr *C, const als_factors *Y, const CholFamily &fam);
+template <int T>
+int launch_cholesky_wide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);   // ld = 16 T, T = 5 ... 8
 int launch_cholesky_xwide(als_ctx *ctx, const als_csr *C, als_factors *X, const als_factors *Y);  // 128 < ld <= 1024
 // long rows on the wgmma tensor cores (cholesky_tc.cu): 64 padded factors, no weights |c| - 1 < 0
 bool cholesky_tc_eligible(const als_ctx *ctx, const als_csr *C, int ld);

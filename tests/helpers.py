@@ -266,6 +266,36 @@ def mixed_csr(users, items, seed, giants=(3073, 3500, 4100), duplicates=False):
     return Cui
 
 
+def bad_row_csr(f, bad_rows, users=40):
+    """With lambda = 0 and Y = I (f items), row u's normal equations are I + the e_i e_i^T of its four items (confidence
+    2); a row in bad_rows also holds three stored zeros on item 0, which subtract 3 e_0 e_0^T: not positive definite."""
+    rng = np.random.default_rng(1)
+    cols = [list(rng.choice(f, 4, replace=False)) + [0] * 3 * (u in bad_rows) for u in range(users)]
+    vals = np.concatenate([[2.0] * 4 + [0.0] * 3 * (u in bad_rows) for u in range(users)]).astype(np.float32)
+    indptr = np.cumsum([0] + [len(c) for c in cols]).astype(np.int32)
+    return sp.csr_matrix((vals, np.concatenate(cols).astype(np.int32), indptr), shape=(users, f))
+
+
+def check_bad_row_in_second_segment(lib, ctx, host):
+    """A bad row beyond the first segment of a segmented device- or host-resident CSR: the synchronous half and, after
+    the asynchronous one, solver_status name it.  Leaves the segment_nnz knob set."""
+    f, bad = 16, 30
+    C = bad_row_csr(f, [bad])
+    ctx.set_knob("segment_nnz", C.nnz // 3 + 1)
+    d = lib.DeviceCSR.upload(ctx, C, host=host)
+    assert d.host_resident == host and d.segment_count > 1
+    assert C.indptr[bad] > C.nnz // 3 + 1  # the bad row lies beyond the first segment
+    Yd, X = lib.DeviceFactors.from_host(ctx, np.eye(f, dtype=np.float32)), lib.DeviceFactors(ctx, C.shape[0], f)
+    with pytest.raises(ValueError, match=f"row {bad}\\b"):
+        lib.least_squares(ctx, d, X, Yd, 0.0)
+    lib.gramian(ctx, Yd)
+    lib.half_pregram_async(ctx, d, X, Yd, 0.0, use_cg=False)
+    with pytest.raises(ValueError, match=f"row {bad}\\b"):
+        lib.solver_status(ctx)
+    for h in (d, Yd, X):
+        h.close()
+
+
 def topk_noise(queries, items):
     """Per-row fp32 summation noise of a score q . i: 4 eps |q| max_i |i|, as an (n, 1) column.  The query side is
     per row (a kernel must hold its accuracy however small a query is next to the others); the item side is the

@@ -13,7 +13,8 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
-from helpers import CHOL_MAX, KNOB_DEFAULTS, cholesky_truth, factors_of, mixed_csr, row_err
+from helpers import (CHOL_MAX, KNOB_DEFAULTS, check_bad_row_in_second_segment, cholesky_truth, factors_of, mixed_csr,
+                     row_err)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -181,35 +182,7 @@ def test_alpha_scaling(lib, ctx, C):
 
 
 def test_bad_row_in_second_segment(lib, ctx):
-    """lambda = 0 and Y = I: a row whose three stored zeros subtract 3 e_0 e_0^T is not positive definite."""
-    f, users = 16, 40
-    rng = np.random.default_rng(1)
-    rows, cols, vals = [], [], []
-    for u in range(users):
-        for i in rng.choice(f, 4, replace=False):
-            rows.append(u)
-            cols.append(int(i))
-            vals.append(2.0)
-    bad = 30
-    rows += [bad] * 3
-    cols += [0] * 3
-    vals += [0.0] * 3
-    order = np.lexsort((np.arange(len(rows)), rows))
-    rows, cols, vals = np.array(rows)[order], np.array(cols)[order], np.array(vals, dtype=np.float32)[order]
-    indptr = np.concatenate([[0], np.cumsum(np.bincount(rows, minlength=users))]).astype(np.int32)
-    C = sp.csr_matrix((vals, cols.astype(np.int32), indptr), shape=(users, f))
-    Y = np.eye(f, dtype=np.float32)
-    d = upload(lib, ctx, C, C.nnz // 3 + 1)
-    assert C.indptr[bad] > C.nnz // 3 + 1  # the bad row lies beyond the first segment
-    Yd, X = lib.DeviceFactors.from_host(ctx, Y), lib.DeviceFactors(ctx, users, f)
-    with pytest.raises(ValueError, match=f"row {bad}\\b"):
-        lib.least_squares(ctx, d, X, Yd, 0.0)
-    lib.gramian(ctx, Yd)
-    lib.half_pregram_async(ctx, d, X, Yd, 0.0, use_cg=False)
-    with pytest.raises(ValueError, match=f"row {bad}\\b"):
-        lib.solver_status(ctx)
-    for h in (d, Yd, X):
-        h.close()
+    check_bad_row_in_second_segment(lib, ctx, host=False)
 
 
 @pytest.mark.parametrize("f", [16, 64])
