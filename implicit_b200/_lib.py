@@ -89,6 +89,12 @@ SIGNATURES = {
     "als_comm_allgather_bytes": (c_int, [c_void_p, c_void_p, c_void_p, c_int]),
     "als_comm_allreduce_f64": (c_int, [c_void_p, P(c_f64), c_int, c_int]),
     "als_comm_barrier": (c_int, [c_void_p]),
+    "als_mem_peak": (c_int, [c_void_p, P(c_i64), P(c_i64)]),
+    "als_csr_column_counts": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "als_csr_transpose_pieces": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "als_csr_merge_rows": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_i64, P(c_void_p)]),
+    "als_comm_allreduce_i64": (c_int, [c_void_p, c_void_p, c_i64]),
+    "als_comm_exchange_csr": (c_int, [c_void_p, c_void_p, c_void_p]),
 }
 
 
@@ -195,6 +201,13 @@ class Context:
         check(self.lib.als_mem_info(self.h, ctypes.byref(free), ctypes.byref(total)))
         return free.value, total.value
 
+    def mem_peak(self):
+        """(in use, peak since the previous call) bytes of the device memory pool the library allocates from; the peak
+        mark then restarts at the current use."""
+        used, peak = c_i64(), c_i64()
+        check(self.lib.als_mem_peak(self.h, ctypes.byref(used), ctypes.byref(peak)))
+        return used.value, peak.value
+
     def info(self):
         name = ctypes.create_string_buffer(256)
         sm, l2, mem = c_int(), c_i64(), c_i64()
@@ -260,6 +273,19 @@ class Context:
         v = np.ascontiguousarray(values, dtype=np.float64).copy()
         check(self.lib.als_comm_allreduce_f64(self.h, v.ctypes.data_as(P(c_f64)), len(v), 1 if op == "max" else 0))
         return v
+
+    def allreduce_i64(self, values):
+        """Exact sum of an int64 array of any length over ranks."""
+        v = np.ascontiguousarray(values, dtype=np.int64).copy()
+        check(self.lib.als_comm_allreduce_i64(self.h, ptr(v), len(v)))
+        return v
+
+    def exchange_csr(self, pieces):
+        """pieces[q] (one DeviceCSR per rank) goes to rank q; returns the pieces every rank sent here, in rank order."""
+        send = (c_void_p * self.world)(*[p.h for p in pieces])
+        recv = (c_void_p * self.world)()
+        check(self.lib.als_comm_exchange_csr(self.h, send, recv))
+        return [DeviceCSR(self, c_void_p(h)) for h in recv]
 
     def barrier(self):
         check(self.lib.als_comm_barrier(self.h))
@@ -381,6 +407,52 @@ class DeviceCSR:
         indptr = np.ascontiguousarray(indptr)
         check(ctx.lib.als_csr_upload(ctx.h, m.shape[0], m.shape[1], m.nnz, ptr(indptr), ptr(indices), ptr(data),
                                      int(row_offset), ctypes.byref(h)))
+        return cls(ctx, h)
+
+    @classmethod
+    def upload_rows(cls, ctx, m, r0, r1):
+        """Rows [r0, r1) of the scipy CSR m as a device-resident shard (row_offset = r0), copied straight out of m's
+        arrays: no host copy of the rows.  Refuses with ValueError what als_csr_upload64 refuses for these rows (an
+        index outside [0, cols), a non-monotone indptr) and an indptr that points past the arrays."""
+        r0, r1 = int(r0), int(r1)
+        if not 0 <= r0 <= r1 <= m.shape[0]:
+            raise ValueError(f"rows [{r0}, {r1}) are not rows of a {m.shape[0]}-row matrix")
+        indptr = np.ascontiguousarray(m.indptr[r0:r1 + 1], dtype=np.int64)
+        indices = m.indices
+        if indices.dtype not in (np.int32, np.int64) or not indices.flags.c_contiguous:
+            indices = np.ascontiguousarray(indices, dtype=np.int64)
+        data = np.ascontiguousarray(m.data, dtype=np.float32)
+        if indptr[0] < 0 or indptr[-1] > min(len(indices), len(data)):
+            raise ValueError(f"indptr[{r0}:{r1 + 1}] points outside the {min(len(indices), len(data))} stored entries")
+        h = c_void_p()
+        rc = ctx.lib.als_csr_upload64(ctx.h, r1 - r0, m.shape[1], int(indptr[-1] - indptr[0]), ptr(indptr), ptr(indices),
+                                      indices.dtype.itemsize, ptr(data), r0, ctypes.byref(h))
+        if rc == ALS_E_INVALID:
+            raise ValueError(ctx.lib.als_last_error().decode("utf-8", "replace"))
+        check(rc)
+        return cls(ctx, h)
+
+    def column_counts(self):
+        """int64 entries per column."""
+        counts = np.zeros(self.shape3[1], dtype=np.int64)
+        check(self.ctx.lib.als_csr_column_counts(self.ctx.h, self.h, ptr(counts)))
+        return counts
+
+    def transpose_pieces(self, col_bounds):
+        """The transpose of this (device-resident) shard cut at col_bounds[0 = b_0 <= ... <= b_n = cols]: n CSRs, the
+        q-th of rows [b_q, b_q+1) of the transpose, with global row ids as column indices."""
+        bounds = np.ascontiguousarray(col_bounds, dtype=np.int64)
+        n = len(bounds) - 1
+        out = (c_void_p * n)()
+        check(self.ctx.lib.als_csr_transpose_pieces(self.ctx.h, self.h, n, ptr(bounds), out))
+        return [DeviceCSR(self.ctx, c_void_p(h)) for h in out]
+
+    @classmethod
+    def merge_rows(cls, ctx, pieces, cols, row_offset):
+        """The pieces (equal row counts) concatenated row by row, in list order, as a shard of `cols` columns."""
+        arr = (c_void_p * len(pieces))(*[p.h for p in pieces])
+        h = c_void_p()
+        check(ctx.lib.als_csr_merge_rows(ctx.h, len(pieces), arr, int(cols), int(row_offset), ctypes.byref(h)))
         return cls(ctx, h)
 
     @property

@@ -15,7 +15,7 @@ import numpy as np
 from scipy.sparse import csr_matrix
 
 from . import _lib
-from .utils import ModelFitError, check_csr, check_random_state, nnz_balanced_splits
+from .utils import ModelFitError, check_csr, check_random_state, column_splits, nnz_balanced_splits
 
 log = logging.getLogger("implicit")
 
@@ -173,16 +173,25 @@ class AlternatingLeastSquares:
         ctx = self.ctx
 
         s = time.time()
-        # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a single-GPU
-        # fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise the same
-        host = False
-        if self.process_group is None:
-            host = bool(ctx.get_knob("host_csr")) or \
-                _lib.csr_residency(users, items, Cui_host.nnz, self.factors, ctx.mem_info()[0]) == "host"
-        Cui = _lib.DeviceCSR.upload(ctx, Cui_host, host=host)
-        if self.alpha != 1.0:
-            Cui.scale(self.alpha)  # cpu/als.py:133-134, on device
-        Ciu = Cui.transpose()      # cpu/als.py:137, on device
+        pg = self.process_group
+        # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
+        # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
+        row_cost = 20 if self.use_cg else 60
+        if pg is not None and pg.world > 1:
+            Cui_s, Ciu_s, usplit, isplit = self._ingest_shards(Cui_host, row_cost)
+        else:
+            # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a
+            # single-GPU fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise
+            # the same
+            host = False
+            if self.process_group is None:
+                host = bool(ctx.get_knob("host_csr")) or \
+                    _lib.csr_residency(users, items, Cui_host.nnz, self.factors, ctx.mem_info()[0]) == "host"
+            Cui_s = _lib.DeviceCSR.upload(ctx, Cui_host, host=host)
+            if self.alpha != 1.0:
+                Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
+            Ciu_s = Cui_s.transpose()    # cpu/als.py:137, on device
+            usplit = isplit = None
         log.debug("Uploaded and transposed in %.3fs", time.time() - s)
 
         # cpu/als.py:144-147: pre-set factors are kept, otherwise rng.random(...) * 0.01
@@ -202,25 +211,14 @@ class AlternatingLeastSquares:
         Y = self._device_factors("item")
         self._user_norms = self._item_norms = self._YtY = self._XtX = None  # cpu/als.py:152-154
 
-        # row shards for the multi-GPU fit (whole matrix on one GPU)
-        pg = self.process_group
-        Cui_s, Ciu_s, usplit, isplit = Cui, Ciu, None, None
         self._p2p = False
-        if pg is not None and pg.world > 1:
-            # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
-            # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
-            row_cost = 20 if self.use_cg else 60
-            usplit = nnz_balanced_splits(Cui_host.indptr, pg.world, row_cost)
-            isplit = nnz_balanced_splits(Ciu.indptr_host(), pg.world, row_cost)
-            if os.environ.get("ALS_B200_NO_P2P") != "1":
-                # fused exchange: solved rows are stored straight into the peers' replicas over NVLink
-                ctx.attach_peers(X)
-                ctx.attach_peers(Y)
-                self._p2p = True
-                # Gramian of the item factors for the first user half (each rank sums its own rows)
-                _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
-            Cui_s = Cui.slice_rows(usplit[pg.rank], usplit[pg.rank + 1])
-            Ciu_s = Ciu.slice_rows(isplit[pg.rank], isplit[pg.rank + 1])
+        if usplit is not None and os.environ.get("ALS_B200_NO_P2P") != "1":
+            # fused exchange: solved rows are stored straight into the peers' replicas over NVLink
+            ctx.attach_peers(X)
+            ctx.attach_peers(Y)
+            self._p2p = True
+            # Gramian of the item factors for the first user half (each rank sums its own rows)
+            _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
 
         loss = None
         progress = None
@@ -271,12 +269,70 @@ class AlternatingLeastSquares:
             ctx.detach_peers(Y)
         self._mark_device_updated("user")
         self._mark_device_updated("item")
-        for c in (Cui_s, Ciu_s):
-            if c is not Cui and c is not Ciu:
-                c.close()
-        Ciu.close()
-        Cui.close()
+        Ciu_s.close()
+        Cui_s.close()
         self._check_fit_errors()  # cpu/als.py:202
+
+    def _ingest_shards(self, Cui_host, row_cost):
+        """Multi-GPU: (Cui_s, Ciu_s, usplit, isplit), this rank's rows of user_items and of its transpose and the user and
+        item splits, built without either whole matrix on any device.  The rank uploads its own user rows; the ranks sum
+        their column counts, which plan the item split; each cuts the transpose of its rows into one piece per rank; the
+        pieces are exchanged and every rank concatenates the ones it received in rank order (scipy's Cui.T.tocsr() order,
+        since rank p's users precede rank p + 1's).  Every rank raises if any rank's part fails, before the next
+        collective: the failing rank its own error, the others an AlsError."""
+        pg, ctx = self.process_group, self.ctx
+        users, items = Cui_host.shape
+        usplit = nnz_balanced_splits(Cui_host.indptr, pg.world, row_cost)
+        held = []  # every device CSR this rank has built so far: closed when any rank fails
+
+        def run(fn):
+            try:
+                return fn(), None
+            except Exception as e:  # noqa: BLE001 -- whatever it is, the other ranks must learn of it
+                return None, e
+
+        def fail_together(err, failed):
+            if not failed:
+                return
+            for c in held:
+                c.close()
+            if err is not None:
+                raise err
+            raise _lib.AlsError(_lib.ALS_E_INVALID, "another rank's ingest of user_items failed (see its error message)")
+
+        def agreed(fn):
+            """fn() on every rank, then one all-reduce of a failure flag before anyone goes on"""
+            out, err = run(fn)
+            fail_together(err, ctx.allreduce([1.0 if err is not None else 0.0], "max")[0] > 0)
+            return out
+
+        def keep(csrs):
+            held.extend(csrs)
+            return csrs
+
+        def upload():
+            s = keep([_lib.DeviceCSR.upload_rows(ctx, Cui_host, usplit[pg.rank], usplit[pg.rank + 1])])[0]
+            if self.alpha != 1.0:
+                s.scale(self.alpha)  # cpu/als.py:133-134, on device
+            return s.column_counts()
+
+        counts, err = run(upload)
+        if err is not None:
+            counts = np.zeros(items, dtype=np.int64)
+        # the first collective of the fit: the failure flag rides along with the column counts
+        total = ctx.allreduce_i64(np.append(counts, 1 if err is not None else 0))
+        fail_together(err, total[-1] > 0)
+        Cui_s = held[0]
+        isplit = column_splits(total[:-1], pg.world, row_cost)
+        pieces = agreed(lambda: keep(Cui_s.transpose_pieces(isplit)))
+        # the exchange agrees inside on its own preparation and allocations; this flag covers what follows its last round
+        received = agreed(lambda: keep(ctx.exchange_csr(pieces)))
+        for c in pieces:
+            c.close()
+        Ciu_s = agreed(lambda: keep([_lib.DeviceCSR.merge_rows(ctx, received, users, isplit[pg.rank])])[0])
+        for c in received:
+            c.close()
+        return Cui_s, Ciu_s, usplit, isplit
 
     def _half(self, C, X, Y, splits, ysplits=None):
         """One half-iteration: solve the rows of (this rank's shard of) C, then exchange them.

@@ -38,8 +38,23 @@ void dev_free(als_ctx *ctx, void *ptr) {
   if (ptr) cudaFreeAsync(ptr, ctx->stream);
 }
 
-// Builds the schedule of a device-transposed CSR from the indptr copy that csr_transpose left in flight.
+// Builds the schedule of a device-transposed CSR from the indptr copy that csr_transpose left in flight, or the
+// schedules of a CSR laid out without them from its device indptrs.
 int ensure_schedule(als_ctx *ctx, als_csr *csr) {
+  if (csr->sched_lazy) {
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    std::vector<int32_t> ip;
+    csr->max_row_nnz = 0;
+    for (const als_csr *S : segments_of(csr)) {
+      ip.resize((size_t)S->rows + 1);
+      ALS_CUDA(cudaMemcpy(ip.data(), S->indptr, sizeof(int32_t) * ip.size(), cudaMemcpyDeviceToHost));
+      int rc = build_schedule(ctx, const_cast<als_csr *>(S), ip.data());
+      if (rc != ALS_OK) return rc;
+      csr->max_row_nnz = std::max(csr->max_row_nnz, S->max_row_nnz);
+    }
+    csr->sched_lazy = false;
+    return ALS_OK;
+  }
   if (!csr->sched_pending) return ALS_OK;
   ALS_CUDA(cudaEventSynchronize(ctx->sched_ev));
   csr->sched_pending = false;
@@ -745,6 +760,56 @@ ALS_API int als_factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed
 ALS_API int als_csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   ALS_REQUIRE(ctx && in && out, "als_csr_transpose: NULL argument");
   return als::csr_transpose(ctx, in, out);
+}
+
+ALS_API int als_csr_column_counts(als_ctx *ctx, const als_csr *csr, int64_t *counts) {
+  ALS_REQUIRE(ctx && csr && (counts || csr->cols == 0), "als_csr_column_counts: NULL argument");
+  return als::csr_column_counts(ctx, csr, counts);
+}
+
+ALS_API int als_csr_transpose_pieces(als_ctx *ctx, const als_csr *shard, int n, const int64_t *col_bounds,
+                                     als_csr **pieces) {
+  ALS_REQUIRE(ctx && shard && col_bounds && pieces && n >= 1, "als_csr_transpose_pieces: NULL argument or n < 1");
+  ALS_REQUIRE(col_bounds[0] == 0 && col_bounds[n] == shard->cols,
+              "als_csr_transpose_pieces: col_bounds must run from 0 to %lld", (long long)shard->cols);
+  for (int q = 0; q < n; ++q)
+    ALS_REQUIRE(col_bounds[q] <= col_bounds[q + 1], "als_csr_transpose_pieces: col_bounds decrease at %d", q);
+  if (shard->host) {
+    set_error("als_csr_transpose_pieces: a host-resident CSR cannot be cut into pieces");
+    return ALS_E_UNSUPPORTED;
+  }
+  return als::csr_transpose_pieces(ctx, shard, n, col_bounds, pieces);
+}
+
+ALS_API int als_csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset,
+                               als_csr **out) {
+  ALS_REQUIRE(ctx && pieces && out && n >= 1, "als_csr_merge_rows: NULL argument or n < 1");
+  for (int p = 0; p < n; ++p) {
+    ALS_REQUIRE(pieces[p], "als_csr_merge_rows: piece %d is NULL", p);
+    ALS_REQUIRE(pieces[p]->rows == pieces[0]->rows, "als_csr_merge_rows: piece %d has %lld rows, piece 0 has %lld", p,
+                (long long)pieces[p]->rows, (long long)pieces[0]->rows);
+    if (pieces[p]->host) {
+      set_error("als_csr_merge_rows: piece %d is host-resident", p);
+      return ALS_E_UNSUPPORTED;
+    }
+  }
+  ALS_REQUIRE(cols >= 0 && cols < (int64_t)INT32_MAX && row_offset >= 0, "als_csr_merge_rows: bad cols or row_offset");
+  return als::csr_merge_rows(ctx, n, pieces, cols, row_offset, out);
+}
+
+ALS_API int als_mem_peak(als_ctx *ctx, int64_t *used_bytes, int64_t *peak_bytes) {
+  ALS_REQUIRE(ctx && used_bytes && peak_bytes, "als_mem_peak: NULL argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  cudaMemPool_t pool;
+  ALS_CUDA(cudaDeviceGetDefaultMemPool(&pool, ctx->device));
+  uint64_t used = 0, high = 0, zero = 0;
+  ALS_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used));
+  ALS_CUDA(cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &high));
+  ALS_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));  // restarts the mark at `used`
+  *used_bytes = (int64_t)used;
+  *peak_bytes = (int64_t)high;
+  return ALS_OK;
 }
 
 ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int64_t r1, als_csr **out) {

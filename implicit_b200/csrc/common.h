@@ -161,6 +161,9 @@ struct als_csr {
   bool wmax_valid = false;
   bool neg_w_known = false, has_neg_w = false;  // host copy of wmax_dev[1]: weights |c| - 1 < 0 exist (then no wgmma long-row path)
   bool sched_pending = false;  // transposed on the device: the schedule is built at first use (ensure_schedule)
+  // laid out without schedules (the pieces of a sharded transpose, which are only copied): ensure_schedule builds them
+  // from the device indptrs at the first solve
+  bool sched_lazy = false;
   // as the liked lists of als_topk, whose fused kernels walk each row's columns in ascending order: checked once on
   // the device at first use; a CSR with an unsorted row gets a sorted copy (indptr rebased to 0) kept for later calls
   bool order_known = false;
@@ -238,16 +241,22 @@ static inline bool needs_segments(const als_ctx *ctx, int64_t nnz) {
   return ctx->knobs.segment_nnz > 0 ? nnz > ctx->knobs.segment_nnz : nnz >= (int64_t)INT32_MAX;
 }
 // Cuts `p` (rows, cols, nnz, row_offset, indices and data set) into segments of at most segment_cap nonzeros.
-// ip[0 .. rows]: the host indptr as positions into p->indices / p->data.  Builds every segment's schedule.
-int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip);
+// ip[0 .. rows]: the host indptr as positions into p->indices / p->data.  Builds every segment's schedule, or leaves
+// them to the first solve (schedule = false: p->sched_lazy).
+int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip, bool schedule = true);
 // The layout of a CSR whose indices / data are set, from its host indptr ip[0 .. rows] (positions into them): segments
 // when it is host-resident or above the segment cap, else one int32 indptr on the device and its schedule.
-int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip);
+int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip, bool schedule = true);
 // indices / data for c->nnz entries: page-locked host arrays for a host-resident CSR, else device arrays from the pool
 int csr_alloc(als_ctx *ctx, als_csr *c);
 // the indptr of any CSR as 64-bit positions relative to its first nonzero (synchronises)
 int csr_indptr64(als_ctx *ctx, const als_csr *c, std::vector<int64_t> &out);
 int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
+// The ingest of a row-sharded fit (als_b200.h): entries per column (host counts[cols]); the transpose of a device-resident
+// shard cut into n pieces of whole columns, in global row ids; pieces of equal row count concatenated row by row.
+int csr_column_counts(als_ctx *ctx, const als_csr *in, int64_t *counts);
+int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *col_bounds, als_csr **pieces);
+int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out);
 // the weight range of a host-resident CSR, computed on the host (bits of max | |c| - 1 | without NaN / inf, and whether
 // some |c| < 1: exactly what csr_wmax_kernel finds) -> c->wmax_dev, marked valid
 int set_host_wmax(als_ctx *ctx, als_csr *c, unsigned wmax_bits, bool neg);

@@ -120,7 +120,21 @@ __global__ void advance_columns_kernel(const int32_t *__restrict__ keys, int64_t
 // (the column histogram reads the indices only).
 constexpr int64_t kWindowSegments = 16;  // a window holds at most this many segment caps of output
 
-int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
+// count[c] += entries of column c in `in` (either residency; reads the indices only)
+int column_histogram(als_ctx *ctx, const als_csr *in, unsigned long long *count) {
+  return for_each_segment(ctx, in, [&](size_t, const als_csr *S) -> int {
+    if (!S->nnz) return ALS_OK;
+    column_histogram_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(S->indices, S->nnz, count);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+    return ALS_OK;
+  }, /*with_data=*/false);
+}
+
+// Writes the transpose of `in` into t->indices / t->data (t->rows, t->nnz and the arrays set) and its indptr, as
+// positions into them, into ip[0 .. cols]; the caller lays t out.  index_base is added to every output index: 0 numbers
+// the rows of `in` from its first row, in->row_offset gives the global rows of a shard.
+int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t index_base, std::vector<int64_t> &ip) {
   const int64_t cols = in->cols;
   int end_bit = 1;
   while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
@@ -129,14 +143,7 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
   if ((rc = dev_alloc(ctx, (void **)&next, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
   if ((rc = dev_alloc(ctx, (void **)&out_ip, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
   ALS_CUDA(cudaMemsetAsync(next, 0, sizeof(long long) * (cols + 1), ctx->stream));
-  rc = for_each_segment(ctx, in, [&](size_t, const als_csr *S) -> int {
-    if (!S->nnz) return ALS_OK;
-    column_histogram_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(S->indices, S->nnz, (unsigned long long *)next);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches++;
-    return ALS_OK;
-  }, /*with_data=*/false);
-  if (rc != ALS_OK) return rc;
+  if ((rc = column_histogram(ctx, in, (unsigned long long *)next)) != ALS_OK) return rc;
   {
     void *tmp = nullptr;
     size_t tmp_bytes = 0;
@@ -145,7 +152,7 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
     ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, next, out_ip, (int)(cols + 1), ctx->stream));
     dev_free(ctx, tmp);
   }
-  std::vector<int64_t> ip((size_t)cols + 1);
+  ip.assign((size_t)cols + 1, 0);
   ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   dev_free(ctx, out_ip);
@@ -218,7 +225,8 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
         ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, S->indices + pc.b0, keys_out, vals_in, vals_out, (int)pc.n,
                                                  0, end_bit, ctx->stream));
         scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
-            vals_out, keys_out, pc.n, S->indptr + pc.r0, (int)(pc.r1 - pc.r0), S->row_offset - in->row_offset + pc.r0,
+            vals_out, keys_out, pc.n, S->indptr + pc.r0, (int)(pc.r1 - pc.r0),
+            index_base + S->row_offset - in->row_offset + pc.r0,
             S->data + pc.b0, next, out_indices, out_data, (int32_t)c0, (int32_t)c1, ip[c0]);
         ALS_CUDA(cudaGetLastError());
         advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, pc.n, next);
@@ -243,7 +251,42 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t) {
     t->neg_w_known = in->neg_w_known;
     t->has_neg_w = in->has_neg_w;
   }
-  return csr_layout(ctx, t, ip.data());
+  return ALS_OK;
+}
+
+// out[dst[r] + j - ip[r]] = in[j] for every entry j of a piece: its row r is the largest with ip[r] <= j
+__global__ void merge_piece_kernel(const int32_t *__restrict__ in_indices, const float *__restrict__ in_data, int64_t n,
+                                   const long long *__restrict__ ip, const long long *__restrict__ dst, int rows,
+                                   int32_t *__restrict__ out_indices, float *__restrict__ out_data) {
+  int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; j < n; j += stride) {
+    int lo = 0, hi = rows;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (ip[mid] <= j) lo = mid; else hi = mid;
+    }
+    const int64_t o = dst[lo] + (j - ip[lo]);
+    out_indices[o] = in_indices[j];
+    out_data[o] = in_data[j];
+  }
+}
+
+// tables: per piece its rebased indptr (rows + 1) then its rows' output starts (rows), uploaded to tables_dev
+int merge_pieces(als_ctx *ctx, int n, const als_csr *const *pieces, const std::vector<int64_t> &base,
+                 const std::vector<int64_t> &tables, long long *tables_dev, als_csr *c) {
+  const int64_t rows = c->rows, stride = 2 * rows + 1;
+  ALS_CUDA(cudaMemcpyAsync(tables_dev, tables.data(), sizeof(int64_t) * tables.size(), cudaMemcpyHostToDevice, ctx->stream));
+  for (int p = 0; p < n; ++p) {
+    const int64_t m = tables[p * stride + rows];
+    if (!m) continue;
+    const long long *tb = tables_dev + p * stride;
+    merge_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(pieces[p]->indices + base[p], pieces[p]->data + base[p],
+                                                                  m, tb, tb + rows + 1, (int)rows, c->indices, c->data);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  return ALS_OK;
 }
 
 }  // namespace
@@ -327,7 +370,7 @@ int set_host_wmax(als_ctx *ctx, als_csr *c, unsigned wmax_bits, bool neg) {
   return ALS_OK;
 }
 
-int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip) {
+int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip, bool schedule) {
   const int64_t cap = segment_cap(ctx, p->host), rows = p->rows;
   std::vector<int64_t> starts;
   for (int64_t a = 0; a < rows || starts.empty();) {
@@ -364,20 +407,32 @@ int make_segments(als_ctx *ctx, als_csr *p, const int64_t *ip) {
     c->indices = p->indices + ip[a];
     c->data = p->data + ip[a];
     p->segs.push_back(c);
+    if (!schedule) continue;
     if ((rc = build_schedule(ctx, c, cat.data() + a + s)) != ALS_OK) return rc;
     p->max_row_nnz = std::max(p->max_row_nnz, c->max_row_nnz);
   }
+  p->sched_lazy = !schedule;
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `cat` dies here
   return ALS_OK;
 }
 
-int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip) {
-  if (c->host || needs_segments(ctx, c->nnz)) return make_segments(ctx, c, ip);
+int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip, bool schedule) {
+  if (!schedule) {  // what the schedule would have found, for the callers that read it without solving (als_topk)
+    c->max_row_nnz = 0;
+    for (int64_t r = 0; r < c->rows; ++r) c->max_row_nnz = std::max(c->max_row_nnz, ip[r + 1] - ip[r]);
+  }
+  if (c->host || needs_segments(ctx, c->nnz)) {
+    const int64_t longest = c->max_row_nnz;
+    const int rc = make_segments(ctx, c, ip, schedule);
+    if (!schedule) c->max_row_nnz = longest;
+    return rc;
+  }
   std::vector<int32_t> ip32(ip, ip + c->rows + 1);
   int rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (c->rows + 1));
   if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * ip32.size(), cudaMemcpyHostToDevice, ctx->stream));
-  rc = build_schedule(ctx, c, ip32.data());
+  c->sched_lazy = !schedule;
+  if (schedule) rc = build_schedule(ctx, c, ip32.data());
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `ip32` dies here
   return rc;
 }
@@ -423,7 +478,9 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   t->host = in->host;  // the transpose of a host-resident CSR is host-resident, built one column window at a time
   int rc;
   if (in->host || !in->segs.empty() || needs_segments(ctx, nnz)) {
-    if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t)) != ALS_OK) {
+    std::vector<int64_t> ip;
+    if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t, 0, ip)) != ALS_OK ||
+        (rc = csr_layout(ctx, t, ip.data())) != ALS_OK) {
       cudaStreamSynchronize(ctx->stream);  // D2H copies of a window may still be landing in t's arrays
       als_csr_destroy(t);
       return rc;
@@ -490,6 +547,111 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   t->sched_pending = true;
   ctx->sched_owner = t;
   *out = t;
+  return ALS_OK;
+}
+
+int csr_column_counts(als_ctx *ctx, const als_csr *in, int64_t *counts) {
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  unsigned long long *count = nullptr;
+  int rc = dev_alloc(ctx, (void **)&count, sizeof(long long) * std::max<int64_t>(in->cols, 1));
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemsetAsync(count, 0, sizeof(long long) * in->cols, ctx->stream));
+  rc = column_histogram(ctx, in, count);
+  if (rc == ALS_OK && in->cols) {
+    ALS_CUDA(cudaMemcpyAsync(counts, count, sizeof(long long) * in->cols, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  dev_free(ctx, count);
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return rc;
+}
+
+// One device transpose of the shard into a scratch CSR, in global row ids; piece q is then copied out of its rows
+// [col_bounds[q], col_bounds[q + 1]) and laid out.  The scratch costs one more copy of the shard's transpose, freed
+// before this returns; a transpose per window would instead sort the whole shard once per piece.
+int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *col_bounds, als_csr **pieces) {
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  for (int q = 0; q < n; ++q) pieces[q] = nullptr;
+  als_csr *t = new als_csr();
+  t->ctx = ctx;
+  t->rows = in->cols;
+  t->cols = in->row_offset + in->rows;
+  t->nnz = in->nnz;
+  std::vector<int64_t> ip;
+  int rc = csr_alloc(ctx, t);
+  if (rc == ALS_OK) rc = transpose_segmented(ctx, in, t, in->row_offset, ip);
+  for (int q = 0; q < n && rc == ALS_OK; ++q) {
+    const int64_t r0 = col_bounds[q], r1 = col_bounds[q + 1];
+    als_csr *p = new als_csr();
+    pieces[q] = p;
+    p->ctx = ctx;
+    p->rows = r1 - r0;
+    p->cols = t->cols;
+    p->nnz = ip[r1] - ip[r0];
+    if ((rc = csr_alloc(ctx, p)) != ALS_OK) break;
+    if (p->nnz) {
+      ALS_CUDA(cudaMemcpyAsync(p->indices, t->indices + ip[r0], sizeof(int32_t) * p->nnz, cudaMemcpyDeviceToDevice,
+                               ctx->stream));
+      ALS_CUDA(cudaMemcpyAsync(p->data, t->data + ip[r0], sizeof(float) * p->nnz, cudaMemcpyDeviceToDevice, ctx->stream));
+    }
+    std::vector<int64_t> pip(ip.begin() + r0, ip.begin() + r1 + 1);
+    for (int64_t &v : pip) v -= ip[r0];
+    rc = csr_layout(ctx, p, pip.data(), /*schedule=*/false);  // copied by the merge, rarely solved
+  }
+  als_csr_destroy(t);  // stream ordered: after the copies above
+  if (rc != ALS_OK) {
+    cudaStreamSynchronize(ctx->stream);
+    for (int q = 0; q < n; ++q) {
+      als_csr_destroy(pieces[q]);
+      pieces[q] = nullptr;
+    }
+  }
+  return rc;
+}
+
+int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out) {
+  *out = nullptr;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const int64_t rows = pieces[0]->rows;
+  // ips[p]: piece p's indptr, rebased to its first nonzero; dst[p][r]: where its row r starts in the output
+  // (csr_indptr64 positions count from the piece's indices pointer: base[p] is its first nonzero)
+  std::vector<std::vector<int64_t>> ips(n);
+  std::vector<int64_t> base(n), oip((size_t)rows + 1, 0);
+  for (int p = 0; p < n; ++p) {
+    int rc = csr_indptr64(ctx, pieces[p], ips[p]);
+    if (rc != ALS_OK) return rc;
+    base[p] = ips[p][0];
+    for (int64_t &v : ips[p]) v -= base[p];
+    for (int64_t r = 0; r < rows; ++r) oip[r + 1] += ips[p][r + 1] - ips[p][r];
+  }
+  for (int64_t r = 0; r < rows; ++r) oip[r + 1] += oip[r];
+  std::vector<int64_t> tables((size_t)n * (2 * rows + 1));  // per piece: ip[0 .. rows], then dst[0 .. rows - 1]
+  std::vector<int64_t> at(oip.begin(), oip.end() - 1);
+  for (int p = 0; p < n; ++p) {
+    int64_t *tb = tables.data() + (size_t)p * (2 * rows + 1);
+    std::copy(ips[p].begin(), ips[p].end(), tb);
+    for (int64_t r = 0; r < rows; ++r) {
+      tb[rows + 1 + r] = at[r];
+      at[r] += ips[p][r + 1] - ips[p][r];
+    }
+  }
+  als_csr *c = new als_csr();
+  c->ctx = ctx;
+  c->rows = rows;
+  c->cols = cols;
+  c->nnz = oip[rows];
+  c->row_offset = row_offset;
+  long long *tables_dev = nullptr;
+  int rc = csr_alloc(ctx, c);
+  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&tables_dev, sizeof(int64_t) * tables.size());
+  if (rc == ALS_OK) rc = merge_pieces(ctx, n, pieces, base, tables, tables_dev, c);
+  dev_free(ctx, tables_dev);
+  if (rc == ALS_OK) rc = csr_layout(ctx, c, oip.data());
+  if (rc != ALS_OK) {
+    cudaStreamSynchronize(ctx->stream);
+    als_csr_destroy(c);
+    return rc;
+  }
+  *out = c;
   return ALS_OK;
 }
 

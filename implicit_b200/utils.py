@@ -49,3 +49,10 @@ def nnz_balanced_splits(indptr, parts, row_cost=0):
     cuts = np.searchsorted(indptr, targets, side="left")
     splits = np.concatenate([[0], np.clip(cuts, 0, rows), [rows]]).astype(np.int64)
     return np.maximum.accumulate(splits)
+
+
+def column_splits(col_counts, parts, row_cost=0):
+    """nnz_balanced_splits of the transpose, planned from the entries per column of the matrix: the transpose's indptr
+    is their running sum."""
+    counts = np.asarray(col_counts, dtype=np.int64)
+    return nnz_balanced_splits(np.concatenate([[0], np.cumsum(counts)]), parts, row_cost)

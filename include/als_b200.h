@@ -71,6 +71,10 @@ int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value);
 /* Free and total device memory in bytes.  Blocks the context's stream-ordered pool keeps for reuse count as free
  * (cudaMemGetInfo alone under-reports after a fit has freed its arrays).  Synchronises the compute stream. */
 int als_mem_info(als_ctx *ctx, int64_t *free_bytes, int64_t *total_bytes);
+/* Bytes of the device's stream-ordered pool (every CSR, scratch array and temporary the library allocates per call) in
+ * use now, and the most in use at any moment since the previous call; the mark then restarts at the current use.
+ * Synchronises the compute stream.  (Measurement entry; no reference equivalent.) */
+int als_mem_peak(als_ctx *ctx, int64_t *used_bytes, int64_t *peak_bytes);
 
 /* Join the ctx streams (replaces the cudaDeviceSynchronize after every call, implicit/gpu/als.cu:147,151,196). */
 int als_sync(als_ctx *ctx);
@@ -134,6 +138,22 @@ int als_csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
  * parent's device arrays, so the parent must outlive it.  The view of a segmented CSR is segmented itself; its shape
  * is the shard's.  (No reference equivalent: multi-GPU sharding.) */
 int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int64_t r1, als_csr **out);
+/* The transpose of a row-sharded matrix without the whole matrix on one device (multi-GPU fit; no reference
+ * equivalent).  Rank p uploads its user rows as a shard (row_offset = its first row), then:
+ *   als_csr_column_counts: counts[c] = entries of column c in the CSR (host int64[cols]); summed over ranks
+ *     (als_comm_allreduce_i64) they are the row lengths of the whole transpose, from which the item split is planned.
+ *   als_csr_transpose_pieces: the transpose of a device-resident CSR cut by col_bounds[0 = b_0 <= ... <= b_n = cols]
+ *     into n CSRs: pieces[q] holds rows [b_q, b_q+1) of the transpose, numbered from 0, with the shard's global row
+ *     ids as column indices (cols = row_offset + rows of the shard) and row_offset 0.  Segmented inputs are taken and
+ *     a piece above the segment cap is segmented.  A host-resident CSR is refused (ALS_E_UNSUPPORTED).
+ *   als_comm_exchange_csr sends piece q to rank q and receives the piece of every rank, then
+ *   als_csr_merge_rows: n device-resident pieces of equal row count concatenated row by row, piece 0's row first,
+ *     into one CSR of `cols` columns with the given row_offset.  Rank order is user order, so the result is exactly
+ *     rows [b_p, b_p+1) of scipy's Cui.T.tocsr(), stored zeros and duplicates included, laid out like any CSR. */
+int als_csr_column_counts(als_ctx *ctx, const als_csr *csr, int64_t *counts);
+int als_csr_transpose_pieces(als_ctx *ctx, const als_csr *shard, int n, const int64_t *col_bounds, als_csr **pieces);
+int als_csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset,
+                       als_csr **out);
 /* data *= alpha on device (replaces `Cui = alpha * Cui`, implicit/cpu/als.py:133-134). */
 int als_csr_scale(als_ctx *ctx, als_csr *csr, float alpha);
 int als_csr_shape(const als_csr *csr, int64_t *rows, int64_t *cols, int64_t *nnz);
@@ -252,6 +272,11 @@ int als_factors_ipc_detach(als_ctx *ctx, als_factors *f);
 int als_comm_allgather_bytes(als_ctx *ctx, const void *send, void *recv, int nbytes);
 /* In-place sum / max of n doubles across ranks (host values; used for loss terms and timing). */
 int als_comm_allreduce_f64(als_ctx *ctx, double *values, int n, int op_max);
+/* In-place exact sum of n int64 host values across ranks (any n; the column counts of a sharded transpose). */
+int als_comm_allreduce_i64(als_ctx *ctx, int64_t *values, int64_t n);
+/* send[world]: device-resident CSRs, send[q] goes to rank q; recv[world] receives a new device CSR from every rank p
+ * (shape, indptr, indices and values, over grouped ncclSend / ncclRecv on the ctx stream).  Every rank must call it. */
+int als_comm_exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv);
 int als_comm_barrier(als_ctx *ctx);
 
 #ifdef __cplusplus
