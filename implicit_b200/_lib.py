@@ -93,6 +93,7 @@ SIGNATURES = {
     "als_csr_column_counts": (c_int, [c_void_p, c_void_p, c_void_p]),
     "als_csr_transpose_pieces": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "als_csr_merge_rows": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_i64, P(c_void_p)]),
+    "als_csr_concat_rows": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_i64, P(c_void_p)]),
     "als_comm_allreduce_i64": (c_int, [c_void_p, c_void_p, c_i64]),
     "als_comm_exchange_csr": (c_int, [c_void_p, c_void_p, c_void_p]),
 }
@@ -453,6 +454,14 @@ class DeviceCSR:
         arr = (c_void_p * len(pieces))(*[p.h for p in pieces])
         h = c_void_p()
         check(ctx.lib.als_csr_merge_rows(ctx.h, len(pieces), arr, int(cols), int(row_offset), ctypes.byref(h)))
+        return cls(ctx, h)
+
+    @classmethod
+    def concat_rows(cls, ctx, pieces, cols, row_offset):
+        """The pieces (any row counts) stacked in list order, piece 0's rows first, as a shard of `cols` columns."""
+        arr = (c_void_p * len(pieces))(*[p.h for p in pieces])
+        h = c_void_p()
+        check(ctx.lib.als_csr_concat_rows(ctx.h, len(pieces), arr, int(cols), int(row_offset), ctypes.byref(h)))
         return cls(ctx, h)
 
     @property

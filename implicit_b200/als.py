@@ -15,7 +15,9 @@ import numpy as np
 from scipy.sparse import csr_matrix
 
 from . import _lib
-from .utils import ModelFitError, check_csr, check_random_state, column_splits, nnz_balanced_splits
+from .distributed import RowBlock
+from .utils import (BLOCK_FIELDS, ModelFitError, block_cuts, check_block_table, check_csr, check_random_state,
+                    column_splits, nnz_balanced_splits, splits_from_cuts)
 
 log = logging.getLogger("implicit")
 
@@ -38,6 +40,75 @@ def liked_batches(indptr, limit):
         out.append((start, end))
         start = end
     return out
+
+
+class _Ingest:
+    """The failure protocol of a multi-GPU ingest: every rank raises if any rank's step fails, before the next
+    collective; the failing rank its own error, the others an AlsError.  held: every device CSR this rank has built so
+    far, closed when any rank fails."""
+
+    def __init__(self, ctx):
+        self.ctx, self.held = ctx, []
+
+    @staticmethod
+    def run(fn):
+        try:
+            return fn(), None
+        except Exception as e:  # noqa: BLE001 -- whatever it is, the other ranks must learn of it
+            return None, e
+
+    def fail(self, err, failed):
+        if not failed:
+            return
+        for c in self.held:
+            c.close()
+        if err is not None:
+            raise err
+        raise _lib.AlsError(_lib.ALS_E_INVALID, "another rank's ingest of user_items failed (see its error message)")
+
+    def agreed(self, fn):
+        """fn() on every rank, then one all-reduce of a failure flag before anyone goes on"""
+        out, err = self.run(fn)
+        self.fail(err, self.ctx.allreduce([1.0 if err is not None else 0.0], "max")[0] > 0)
+        return out
+
+    def keep(self, csrs):
+        self.held.extend(csrs)
+        return csrs
+
+
+def block_pieces(ctx, block, first_row, usplit):
+    """The rows of a row block (scipy CSR, rows [first_row, first_row + block.shape[0]) of user_items) cut along the
+    user split: one device CSR per rank q, its rows in [usplit[q], usplit[q + 1]) (mostly none), each uploaded straight
+    out of the block's arrays.  A bad index or indptr raises ValueError naming its row of user_items."""
+    cut = np.clip(np.asarray(usplit, dtype=np.int64) - int(first_row), 0, block.shape[0])
+    pieces = []
+    try:
+        for q in range(len(cut) - 1):
+            pieces.append(_lib.DeviceCSR.upload_rows(ctx, block, cut[q], cut[q + 1]))
+    except BaseException as e:
+        for c in pieces:
+            c.close()
+        where = _first_bad_row(block, first_row) if isinstance(e, ValueError) else None
+        if where is not None:
+            raise ValueError(where) from e
+        raise
+    return pieces
+
+
+def _first_bad_row(block, first_row):
+    """What als_csr_upload64 refuses in a row block, named by its row of user_items (None if nothing is found)."""
+    ip = np.asarray(block.indptr, dtype=np.int64)
+    down = np.flatnonzero(np.diff(ip) < 0)
+    if down.size:
+        return f"user_items: indptr is not monotone at row {first_row + int(down[0])}"
+    idx = block.indices[ip[0]:ip[-1]]
+    bad = np.flatnonzero((idx < 0) | (idx >= block.shape[1]))
+    if not bad.size:
+        return None
+    row = int(np.searchsorted(ip, ip[0] + bad[0], side="right")) - 1
+    return (f"user_items: row {first_row + row} holds column index {int(idx[bad[0]])}, which is outside "
+            f"[0, {block.shape[1]})")
 
 
 class AlternatingLeastSquares:
@@ -164,22 +235,32 @@ class AlternatingLeastSquares:
 
     # ------------------------------------------------------------------ fit (implicit/cpu/als.py:98-202)
     def fit(self, user_items, show_progress=True, callback=None):
-        """Factorizes the user_items matrix (CSR, users x items, values = confidence)."""
+        """Factorizes the user_items matrix (CSR, users x items, values = confidence).  On a process group of several
+        ranks, each rank may instead pass only its own rows, as a distributed.RowBlock."""
         random_state = check_random_state(self.random_state)
-        Cui_host = check_csr(user_items)  # ParameterWarning on non-CSR input (utils.py:159-169)
-        if Cui_host.dtype != np.float32:
-            Cui_host = Cui_host.astype(np.float32)  # cpu/als.py:129-130
-        users, items = Cui_host.shape
+        pg = self.process_group
+        from_blocks = isinstance(user_items, RowBlock) and pg is not None and pg.world > 1
+        if from_blocks:
+            Cui_host = None
+        elif isinstance(user_items, RowBlock):
+            Cui_host = user_items.whole()  # one rank: the block must be the whole matrix
+        else:
+            Cui_host = check_csr(user_items)  # ParameterWarning on non-CSR input (utils.py:159-169)
+            if Cui_host.dtype != np.float32:
+                Cui_host = Cui_host.astype(np.float32)  # cpu/als.py:129-130
         ctx = self.ctx
 
         s = time.time()
-        pg = self.process_group
         # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
         # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
         row_cost = 20 if self.use_cg else 60
-        if pg is not None and pg.world > 1:
+        if from_blocks:
+            Cui_s, Ciu_s, usplit, isplit, (users, items, nnz) = self._ingest_row_blocks(user_items, row_cost)
+        elif pg is not None and pg.world > 1:
+            users, items, nnz = *Cui_host.shape, Cui_host.nnz
             Cui_s, Ciu_s, usplit, isplit = self._ingest_shards(Cui_host, row_cost)
         else:
+            users, items, nnz = *Cui_host.shape, Cui_host.nnz
             # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a
             # single-GPU fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise
             # the same
@@ -239,7 +320,7 @@ class AlternatingLeastSquares:
                 if progress is not None:
                     progress.update(1)
                 if self.calculate_training_loss:
-                    loss = self._loss(Cui_s, X, Y, users, items, Cui_host.nnz)
+                    loss = self._loss(Cui_s, X, Y, users, items, nnz)
                     if self._p2p:  # the loss pass reuses the Gramian buffers: restore Y^T Y for the next half
                         _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
                     if progress is not None:
@@ -283,56 +364,86 @@ class AlternatingLeastSquares:
         pg, ctx = self.process_group, self.ctx
         users, items = Cui_host.shape
         usplit = nnz_balanced_splits(Cui_host.indptr, pg.world, row_cost)
-        held = []  # every device CSR this rank has built so far: closed when any rank fails
+        ing = _Ingest(ctx)
+        # the first collective of the fit is the column-count all-reduce, which carries the upload's failure flag
+        Cui_s, Ciu_s, isplit = self._transpose_shards(
+            ing, lambda: _lib.DeviceCSR.upload_rows(ctx, Cui_host, usplit[pg.rank], usplit[pg.rank + 1]),
+            users, items, row_cost)
+        return Cui_s, Ciu_s, usplit, isplit
 
-        def run(fn):
-            try:
-                return fn(), None
-            except Exception as e:  # noqa: BLE001 -- whatever it is, the other ranks must learn of it
-                return None, e
+    def _ingest_row_blocks(self, block, row_cost):
+        """Multi-GPU from row blocks: (Cui_s, Ciu_s, usplit, isplit, (users, items, nnz)) like _ingest_shards, when this
+        rank holds only its own distributed.RowBlock of user_items.  The ranks all-gather their blocks' extents, plan
+        the user split _ingest_shards would plan from the whole indptr (each searches only its own indptr), upload
+        their rows in one piece per rank of that split and exchange the pieces; every rank stacks the pieces it
+        received into its user shard, and the transpose follows as in _ingest_shards.  Failures are agreed on the same
+        way; a bad index or indptr names its row of the whole matrix."""
+        pg, ctx = self.process_group, self.ctx
+        rank, W = pg.rank, pg.world
+        ing = _Ingest(ctx)
 
-        def fail_together(err, failed):
-            if not failed:
-                return
-            for c in held:
-                c.close()
-            if err is not None:
-                raise err
-            raise _lib.AlsError(_lib.ALS_E_INVALID, "another rank's ingest of user_items failed (see its error message)")
+        def read():
+            m = block.csr()
+            return m, (block.first_row, m.shape[0], block.users, m.shape[1], int(m.indptr[-1]) - int(m.indptr[0]), 0)
 
-        def agreed(fn):
-            """fn() on every rank, then one all-reduce of a failure flag before anyone goes on"""
-            out, err = run(fn)
-            fail_together(err, ctx.allreduce([1.0 if err is not None else 0.0], "max")[0] > 0)
-            return out
-
-        def keep(csrs):
-            held.extend(csrs)
-            return csrs
-
-        def upload():
-            s = keep([_lib.DeviceCSR.upload_rows(ctx, Cui_host, usplit[pg.rank], usplit[pg.rank + 1])])[0]
-            if self.alpha != 1.0:
-                s.scale(self.alpha)  # cpu/als.py:133-134, on device
-            return s.column_counts()
-
-        counts, err = run(upload)
+        out, err = ing.run(read)
+        mine = out[1] if err is None else (0, 0, 0, 0, 0, 1)
+        # the first collective of the fit: every rank's block extent and whether it could read its block (48 bytes)
+        table = np.frombuffer(ctx.allgather_bytes(np.array(mine, dtype=np.int64).tobytes()), dtype=np.int64)
+        table = table.reshape(W, len(BLOCK_FIELDS))
+        ing.fail(err, table[:, -1].any())
+        m = out[0]
+        users, items, nnz = check_block_table(table)  # the same table on every rank: the same error on every rank
+        cuts, err = ing.run(lambda: block_cuts(table, m.indptr, rank, row_cost))
         if err is not None:
-            counts = np.zeros(items, dtype=np.int64)
-        # the first collective of the fit: the failure flag rides along with the column counts
-        total = ctx.allreduce_i64(np.append(counts, 1 if err is not None else 0))
-        fail_together(err, total[-1] > 0)
-        Cui_s = held[0]
-        isplit = column_splits(total[:-1], pg.world, row_cost)
-        pieces = agreed(lambda: keep(Cui_s.transpose_pieces(isplit)))
-        # the exchange agrees inside on its own preparation and allocations; this flag covers what follows its last round
-        received = agreed(lambda: keep(ctx.exchange_csr(pieces)))
+            cuts = np.zeros(W - 1, dtype=np.int64)
+        total = ctx.allreduce_i64(np.append(cuts, 1 if err is not None else 0))
+        ing.fail(err, total[-1] > 0)
+        usplit = splits_from_cuts(total[:-1], users)
+        pieces = ing.agreed(lambda: ing.keep(block_pieces(ctx, m, block.first_row, usplit)))
+        received = ing.agreed(lambda: ing.keep(ctx.exchange_csr(pieces)))
         for c in pieces:
             c.close()
-        Ciu_s = agreed(lambda: keep([_lib.DeviceCSR.merge_rows(ctx, received, users, isplit[pg.rank])])[0])
+
+        def stack():
+            s = _lib.DeviceCSR.concat_rows(ctx, received, items, usplit[rank])
+            for c in received:
+                c.close()
+            return s
+
+        # the stack's failure flag rides along with the column counts
+        Cui_s, Ciu_s, isplit = self._transpose_shards(ing, stack, users, items, row_cost)
+        return Cui_s, Ciu_s, usplit, isplit, (users, items, nnz)
+
+    def _transpose_shards(self, ing, build, users, items, row_cost):
+        """(Cui_s, Ciu_s, isplit): this rank's user shard from build(), scaled by alpha; the ranks sum their column
+        counts, which plan the item split; each cuts the transpose of its rows into one piece per rank; the pieces are
+        exchanged and every rank concatenates the ones it received in rank order (scipy's Cui.T.tocsr() order, since
+        rank p's users precede rank p + 1's)."""
+        pg, ctx = self.process_group, self.ctx
+
+        def shard():
+            s = ing.keep([build()])[0]
+            if self.alpha != 1.0:
+                s.scale(self.alpha)  # cpu/als.py:133-134, on device
+            return s, s.column_counts()
+
+        out, err = ing.run(shard)
+        counts = out[1] if err is None else np.zeros(items, dtype=np.int64)
+        # the failure flag rides along with the column counts
+        total = ctx.allreduce_i64(np.append(counts, 1 if err is not None else 0))
+        ing.fail(err, total[-1] > 0)
+        Cui_s = out[0]
+        isplit = column_splits(total[:-1], pg.world, row_cost)
+        pieces = ing.agreed(lambda: ing.keep(Cui_s.transpose_pieces(isplit)))
+        # the exchange agrees inside on its own preparation and allocations; this flag covers what follows its last round
+        received = ing.agreed(lambda: ing.keep(ctx.exchange_csr(pieces)))
+        for c in pieces:
+            c.close()
+        Ciu_s = ing.agreed(lambda: ing.keep([_lib.DeviceCSR.merge_rows(ctx, received, users, isplit[pg.rank])])[0])
         for c in received:
             c.close()
-        return Cui_s, Ciu_s, usplit, isplit
+        return Cui_s, Ciu_s, isplit
 
     def _half(self, C, X, Y, splits, ysplits=None):
         """One half-iteration: solve the rows of (this rank's shard of) C, then exchange them.

@@ -797,6 +797,26 @@ ALS_API int als_csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces
   return als::csr_merge_rows(ctx, n, pieces, cols, row_offset, out);
 }
 
+ALS_API int als_csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset,
+                                als_csr **out) {
+  ALS_REQUIRE(ctx && pieces && out && n >= 1, "als_csr_concat_rows: NULL argument or n < 1");
+  ALS_REQUIRE(cols >= 0 && cols < (int64_t)INT32_MAX && row_offset >= 0, "als_csr_concat_rows: bad cols or row_offset");
+  *out = nullptr;
+  int64_t rows = 0;
+  for (int p = 0; p < n; ++p) {
+    ALS_REQUIRE(pieces[p], "als_csr_concat_rows: piece %d is NULL", p);
+    ALS_REQUIRE(pieces[p]->cols <= cols, "als_csr_concat_rows: piece %d has %lld columns, more than %lld", p,
+                (long long)pieces[p]->cols, (long long)cols);
+    if (pieces[p]->host) {
+      set_error("als_csr_concat_rows: piece %d is host-resident", p);
+      return ALS_E_UNSUPPORTED;
+    }
+    rows += pieces[p]->rows;
+  }
+  ALS_REQUIRE(rows < (int64_t)INT32_MAX, "als_csr_concat_rows: %lld rows in all, more than 2^31 - 2", (long long)rows);
+  return als::csr_concat_rows(ctx, n, pieces, cols, row_offset, out);
+}
+
 ALS_API int als_mem_peak(als_ctx *ctx, int64_t *used_bytes, int64_t *peak_bytes) {
   ALS_REQUIRE(ctx && used_bytes && peak_bytes, "als_mem_peak: NULL argument");
   ALS_CUDA(cudaSetDevice(ctx->device));

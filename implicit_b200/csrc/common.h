@@ -257,6 +257,8 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
 int csr_column_counts(als_ctx *ctx, const als_csr *in, int64_t *counts);
 int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *col_bounds, als_csr **pieces);
 int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out);
+// The ingest from row blocks: device-resident pieces (any row counts) stacked in list order, piece 0's rows first.
+int csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out);
 // the weight range of a host-resident CSR, computed on the host (bits of max | |c| - 1 | without NaN / inf, and whether
 // some |c| < 1: exactly what csr_wmax_kernel finds) -> c->wmax_dev, marked valid
 int set_host_wmax(als_ctx *ctx, als_csr *c, unsigned wmax_bits, bool neg);

@@ -289,6 +289,17 @@ int merge_pieces(als_ctx *ctx, int n, const als_csr *const *pieces, const std::v
   return ALS_OK;
 }
 
+// One segment of a piece of a row stack: its rows + 1 entries of the output indptr, as 64-bit positions from the
+// output's first nonzero (out_base is where the segment's first nonzero lands), and the segment's first position in
+// its own indptr (a row-slice view's indptr does not start at 0), which tells the host where to copy its entries from.
+__global__ void concat_indptr_kernel(const int32_t *__restrict__ ip, int64_t rows, long long out_base,
+                                     long long *__restrict__ out, long long *__restrict__ first) {
+  const long long f = ip[0];
+  int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) *first = f;
+  for (; r <= rows; r += (int64_t)gridDim.x * blockDim.x) out[r] = out_base + (ip[r] - f);
+}
+
 }  // namespace
 
 int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch, bool with_data) {
@@ -646,6 +657,69 @@ int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t co
   if (rc == ALS_OK) rc = merge_pieces(ctx, n, pieces, base, tables, tables_dev, c);
   dev_free(ctx, tables_dev);
   if (rc == ALS_OK) rc = csr_layout(ctx, c, oip.data());
+  if (rc != ALS_OK) {
+    cudaStreamSynchronize(ctx->stream);
+    als_csr_destroy(c);
+    return rc;
+  }
+  *out = c;
+  return ALS_OK;
+}
+
+// One kernel per segment writes its share of the output indptr; one copy of that indptr (and of every segment's first
+// position) to the host; then every segment's entries are one asynchronous device-to-device copy each, and the layout
+// cuts the result into segments above the cap and builds its schedule.
+int csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out) {
+  *out = nullptr;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  struct Seg {
+    const als_csr *S;
+    int64_t row, pos;  // its first row and first nonzero in the output
+  };
+  std::vector<Seg> segs;
+  int64_t rows = 0, nnz = 0;
+  for (int p = 0; p < n; ++p) {
+    int64_t pos = nnz;
+    for (const als_csr *S : segments_of(pieces[p])) {
+      segs.push_back({S, rows + (S->row_offset - pieces[p]->row_offset), pos});
+      pos += S->nnz;
+    }
+    rows += pieces[p]->rows;
+    nnz += pieces[p]->nnz;
+  }
+  const int64_t ns = (int64_t)segs.size();
+  als_csr *c = new als_csr();
+  c->ctx = ctx;
+  c->rows = rows;
+  c->cols = cols;
+  c->nnz = nnz;
+  c->row_offset = row_offset;
+  long long *ip_dev = nullptr;  // the output indptr (rows + 1), then the segments' first positions (ns)
+  std::vector<int64_t> ip((size_t)(rows + 1 + ns));
+  int rc = csr_alloc(ctx, c);
+  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&ip_dev, sizeof(int64_t) * ip.size());
+  for (int64_t k = 0; k < ns && rc == ALS_OK; ++k) {
+    const Seg &g = segs[k];
+    const int blocks = (int)std::min<int64_t>((g.S->rows + 256) / 256, (int64_t)ctx->sm_count * 8);
+    concat_indptr_kernel<<<blocks, 256, 0, ctx->stream>>>(g.S->indptr, g.S->rows, g.pos, ip_dev + g.row, ip_dev + rows + 1 + k);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  if (rc == ALS_OK) {
+    ALS_CUDA(cudaMemcpyAsync(ip.data(), ip_dev, sizeof(int64_t) * ip.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int64_t k = 0; k < ns; ++k) {
+      const Seg &g = segs[k];
+      if (!g.S->nnz) continue;
+      const int64_t first = ip[rows + 1 + k];
+      ALS_CUDA(cudaMemcpyAsync(c->indices + g.pos, g.S->indices + first, sizeof(int32_t) * g.S->nnz,
+                               cudaMemcpyDeviceToDevice, ctx->stream));
+      ALS_CUDA(cudaMemcpyAsync(c->data + g.pos, g.S->data + first, sizeof(float) * g.S->nnz, cudaMemcpyDeviceToDevice,
+                               ctx->stream));
+    }
+  }
+  dev_free(ctx, ip_dev);
+  if (rc == ALS_OK) rc = csr_layout(ctx, c, ip.data());
   if (rc != ALS_OK) {
     cudaStreamSynchronize(ctx->stream);
     als_csr_destroy(c);

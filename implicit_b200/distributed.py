@@ -9,12 +9,16 @@ Only the 128-byte NCCL unique id crosses between the processes on the host side:
 (als_comm_unique_id) and serves it over a loopback/TCP socket next to MASTER_PORT; every rank then
 calls als_comm_init.  No PyTorch is involved; all collectives are NCCL calls inside libals_b200.so.
 """
+import numbers
 import os
 import socket
 import struct
 import time
 
+import numpy as np
+
 from . import _lib
+from .utils import check_csr
 
 _MAGIC = b"ALSB200\x01"
 _PORT_OFFSETS = (1, 2, 3, 5, 8, 13, 21, 34)
@@ -99,6 +103,46 @@ def _recv_exact(conn, n):
             raise ConnectionError("peer closed")
         buf += chunk
     return buf
+
+
+def row_block(users, rank, world):
+    """(first_row, end_row): rank's even share of `users` rows, for a loader that reads only its own rows from disk and
+    passes them to fit as RowBlock(rows, first_row, users).  The blocks of ranks 0 .. world - 1 tile [0, users)."""
+    users, rank, world = int(users), int(rank), int(world)
+    if world < 1 or not 0 <= rank < world or users < 0:
+        raise ValueError(f"row_block: no rank {rank} of {world} for {users} rows")
+    return users * rank // world, users * (rank + 1) // world
+
+
+class RowBlock:
+    """This rank's rows [first_row, first_row + user_items.shape[0]) of a `users` x user_items.shape[1] interaction
+    matrix, for AlternatingLeastSquares.fit.  On a process group of several ranks each rank passes only its own block;
+    the blocks, of any sizes (none at all included), must tile [0, users) in rank order.  Without a process group, or on
+    one rank, the block must hold every row, and the fit is the fit of the plain matrix.
+
+    Conversion to CSR (with the usual ParameterWarning) and the cast of the values to float32 happen in fit, where a
+    failure on one rank is reported to every rank instead of leaving the others waiting for it."""
+
+    def __init__(self, user_items, first_row, users):
+        self.user_items, self.first_row, self.users = user_items, first_row, users
+
+    def csr(self):
+        """The block as a float32 scipy CSR, after checking its own shape."""
+        m = check_csr(self.user_items)
+        if m.dtype != np.float32:
+            m = m.astype(np.float32)  # cpu/als.py:129-130
+        first, users = self.first_row, self.users
+        if not (isinstance(first, numbers.Integral) and isinstance(users, numbers.Integral)) or first < 0 or users < 0:
+            raise ValueError(f"RowBlock: first_row ({first!r}) and users ({users!r}) must be integers >= 0")
+        return m
+
+    def whole(self):
+        """The block as the whole matrix, for a fit without a process group or on one rank: it must hold every row."""
+        m = self.csr()
+        if self.first_row != 0 or m.shape[0] != self.users:
+            raise ValueError(f"a RowBlock of rows [{self.first_row}, {self.first_row + m.shape[0]}) of a {self.users}-row "
+                             "matrix is fitted only on a process group of several ranks; on one it must hold every row")
+        return m
 
 
 class ProcessGroup:

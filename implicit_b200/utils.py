@@ -51,6 +51,72 @@ def nnz_balanced_splits(indptr, parts, row_cost=0):
     return np.maximum.accumulate(splits)
 
 
+#: the fields of one rank's row of the block table a multi-GPU fit from row blocks all-gathers first (int64 each)
+BLOCK_FIELDS = ("first_row", "rows", "users", "items", "nnz", "failed")
+
+
+def check_block_table(table):
+    """(users, items, nnz) of the matrix the ranks' blocks tile, from the block table (one row of BLOCK_FIELDS per rank,
+    in rank order), or the same ValueError, naming the offending rank, on every rank that checks the same table."""
+    t = np.asarray(table, dtype=np.int64).reshape(-1, len(BLOCK_FIELDS))
+    users, items = int(t[0, 2]), int(t[0, 3])
+    end = 0
+    for p, (first, rows, u, i, nnz, _) in enumerate(t.tolist()):
+        if u != users:
+            raise ValueError(f"rank {p}'s row block is of a {u}-row matrix, rank 0's of a {users}-row one")
+        if i != items:
+            raise ValueError(f"rank {p}'s row block has {i} columns, rank 0's {items}")
+        if first < 0 or rows < 0 or nnz < 0:
+            raise ValueError(f"rank {p}'s row block has first_row {first}, {rows} rows and {nnz} nonzeros")
+        if first + rows > users:
+            raise ValueError(f"rank {p}'s row block, rows [{first}, {first + rows}), runs past the {users} rows of the "
+                             "matrix")
+        if first != end:
+            raise ValueError(f"rank {p}'s row block starts at row {first}, but the blocks of the ranks before it end at "
+                             f"row {end}: the blocks must tile the rows in rank order, without gaps or overlaps")
+        end = first + rows
+    if end != users:
+        raise ValueError(f"rank {len(t) - 1}'s row block ends at row {end}: the blocks must tile all {users} rows")
+    return users, items, int(t[:, 4].sum())
+
+
+def block_cuts(table, local_indptr, rank, row_cost=0):
+    """This rank's part of the user split of a fit from row blocks: the W - 1 inner cuts of
+    nnz_balanced_splits(whole.indptr, W, row_cost) that fall in its block, zeros elsewhere.  Summed over the ranks and
+    passed to splits_from_cuts, they are that split exactly, although no rank holds the whole indptr.
+
+    Every rank knows from the (checked) table the value of g = indptr + row_cost * row at every block boundary, so which
+    block holds the first row whose g reaches each target; only that block's owner searches its own indptr."""
+    t = np.asarray(table, dtype=np.int64).reshape(-1, len(BLOCK_FIELDS))
+    W = len(t)
+    first, rows, users, nnz = t[:, 0], t[:, 1], int(t[0, 2]), t[:, 4]
+    before = np.concatenate([[0], np.cumsum(nnz)])  # nonzeros of the rows before each block
+    total = int(before[-1]) + row_cost * users
+    targets = (total * np.arange(1, W, dtype=np.int64)) // max(W, 1)
+    cuts = np.zeros(max(W - 1, 0), dtype=np.int64)
+    lo = before[rank] + row_cost * first[rank]                     # g at the block's first row
+    hi = before[rank + 1] + row_cost * (first[rank] + rows[rank])  # ... and one past its last
+    mine = np.flatnonzero((targets > lo) & (targets <= hi)) if rows[rank] > 0 else []
+    if len(mine):
+        ip = np.asarray(local_indptr, dtype=np.int64)
+        g = lo + (ip - ip[0]) + row_cost * np.arange(len(ip), dtype=np.int64)
+        cuts[mine] = first[rank] + np.searchsorted(g, targets[mine], side="left")
+    return cuts
+
+
+def splits_from_cuts(cuts, users):
+    """The user split from the summed block_cuts: the clip and running maximum of nnz_balanced_splits."""
+    splits = np.concatenate([[0], np.clip(np.asarray(cuts, dtype=np.int64), 0, users), [users]]).astype(np.int64)
+    return np.maximum.accumulate(splits)
+
+
+def simulate_block_splits(table, local_indptrs, row_cost=0):
+    """The user split the W ranks of a fit from row blocks agree on (their block_cuts summed), computed in one process."""
+    users, _, _ = check_block_table(table)
+    cuts = sum(block_cuts(table, ip, p, row_cost) for p, ip in enumerate(local_indptrs))
+    return splits_from_cuts(cuts, users)
+
+
 def column_splits(col_counts, parts, row_cost=0):
     """nnz_balanced_splits of the transpose, planned from the entries per column of the matrix: the transpose's indptr
     is their running sum."""

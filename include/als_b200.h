@@ -149,11 +149,20 @@ int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int64_t r1, 
  *   als_comm_exchange_csr sends piece q to rank q and receives the piece of every rank, then
  *   als_csr_merge_rows: n device-resident pieces of equal row count concatenated row by row, piece 0's row first,
  *     into one CSR of `cols` columns with the given row_offset.  Rank order is user order, so the result is exactly
- *     rows [b_p, b_p+1) of scipy's Cui.T.tocsr(), stored zeros and duplicates included, laid out like any CSR. */
+ *     rows [b_p, b_p+1) of scipy's Cui.T.tocsr(), stored zeros and duplicates included, laid out like any CSR.
+ *   als_csr_concat_rows: n device-resident CSRs of any row counts stacked in list order, piece 0's rows first (a vstack,
+ *     not the row-by-row interleave of merge_rows), into one CSR of `cols` columns with the given row_offset.  When
+ *     every rank holds only its own block of user rows, rank p uploads it in one piece per rank q (the rows of its block
+ *     that fall in q's share of the user split, mostly none), the pieces go through als_comm_exchange_csr, and rank q
+ *     stacks the W pieces it receives, which cover consecutive rows in rank order, into its user shard.  Flat,
+ *     segmented and row-slice pieces are taken; the result is laid out with its launch schedule and segmented above
+ *     the cap like any CSR.  A host-resident piece is refused (ALS_E_UNSUPPORTED). */
 int als_csr_column_counts(als_ctx *ctx, const als_csr *csr, int64_t *counts);
 int als_csr_transpose_pieces(als_ctx *ctx, const als_csr *shard, int n, const int64_t *col_bounds, als_csr **pieces);
 int als_csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset,
                        als_csr **out);
+int als_csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset,
+                        als_csr **out);
 /* data *= alpha on device (replaces `Cui = alpha * Cui`, implicit/cpu/als.py:133-134). */
 int als_csr_scale(als_ctx *ctx, als_csr *csr, float alpha);
 int als_csr_shape(const als_csr *csr, int64_t *rows, int64_t *cols, int64_t *nnz);
