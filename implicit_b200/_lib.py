@@ -79,6 +79,8 @@ SIGNATURES = {
     "als_calculate_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_f32, P(c_f64)]),
     "als_topk": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p, c_void_p, c_i64,
                          c_void_p, c_void_p]),
+    "als_ranking_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
     "als_comm_unique_id": (c_int, [c_void_p]),
     "als_comm_init": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "als_comm_destroy": (c_int, [c_void_p]),
@@ -681,3 +683,15 @@ def topk(ctx, items, queries, k, query_rows=None, n_query=None, item_norms=None,
                            liked.h if liked is not None else None, ptr(fl), 0 if fl is None else len(fl),
                            ptr(ids), ptr(scores)))
     return ids, scores
+
+
+def ranking_metrics(ctx, items, queries, k, query_rows, test, gain, gain_sum, liked=None):
+    """The six fp64 sums of ranking_metrics_at_k (hits, sum min(K, L), AP, nDCG, AUC, users) over the queries
+    `query_rows` of `queries`, scored against `test` (a DeviceCSR over those rows) on the device."""
+    query_rows = np.ascontiguousarray(query_rows, dtype=np.int32)
+    gain = np.ascontiguousarray(gain, dtype=np.float64)
+    gain_sum = np.ascontiguousarray(gain_sum, dtype=np.float64)
+    sums = np.zeros(6, dtype=np.float64)
+    check(ctx.lib.als_ranking_metrics(ctx.h, items.h, queries.h, ptr(query_rows), len(query_rows), int(k),
+                                      liked.h if liked is not None else None, test.h, ptr(gain), ptr(gain_sum), ptr(sums)))
+    return sums

@@ -47,8 +47,8 @@ class _Ingest:
     collective; the failing rank its own error, the others an AlsError.  held: every device CSR this rank has built so
     far, closed when any rank fails."""
 
-    def __init__(self, ctx):
-        self.ctx, self.held = ctx, []
+    def __init__(self, ctx, what="ingest of user_items"):
+        self.ctx, self.held, self.what = ctx, [], what
 
     @staticmethod
     def run(fn):
@@ -64,7 +64,7 @@ class _Ingest:
             c.close()
         if err is not None:
             raise err
-        raise _lib.AlsError(_lib.ALS_E_INVALID, "another rank's ingest of user_items failed (see its error message)")
+        raise _lib.AlsError(_lib.ALS_E_INVALID, f"another rank's {self.what} failed (see its error message)")
 
     def agreed(self, fn):
         """fn() on every rank, then one all-reduce of a failure flag before anyone goes on"""
@@ -641,6 +641,32 @@ class AlternatingLeastSquares:
         if items is not None:
             ids = items[ids]
         return ids, scores
+
+    def _ranking_sums(self, userids, user_items, test_items, K, gain, gain_sum):
+        """The six sums of evaluation.ranking_metrics_at_k (hits, sum min(K, L), AP, nDCG, AUC, users) for the users
+        `userids`: the ids of recommend(userids, user_items, N=K) scored against the same rows of test_items (scipy
+        CSRs, one row per user) without leaving the device.  Refuses what recommend refuses, the same way."""
+        queries = self._device_factors("user")
+        query_rows = np.asarray(userids, dtype=np.int64)
+        if query_rows.size and (query_rows.min() < 0 or query_rows.max() >= queries.rows):
+            raise IndexError("userid out of range")
+        items, ctx = self._device_factors("item"), self.ctx
+        batches = [(0, len(query_rows))]
+        if user_items.nnz > _LIKED_NNZ_MAX:
+            batches = liked_batches(user_items.indptr, _LIKED_NNZ_MAX)
+        sums = np.zeros(6)
+        for b0, b1 in batches:
+            held = []
+            try:
+                liked = _lib.DeviceCSR.upload_rows(ctx, user_items, b0, b1)
+                held.append(liked)
+                test = _lib.DeviceCSR.upload_rows(ctx, test_items, b0, b1)
+                held.append(test)
+                sums += _lib.ranking_metrics(ctx, items, queries, K, query_rows[b0:b1], test, gain, gain_sum, liked)
+            finally:
+                for c in held:
+                    c.close()
+        return sums
 
     def rank_items(self, userid, user_items, selected_items, recalculate_user=False):
         """implicit/recommender_base.py:204-216 (deprecated alias)"""

@@ -1344,23 +1344,52 @@ ALS_API int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors
   return ALS_OK;
 }
 
+// what als_topk and als_ranking_metrics refuse in their common arguments
+static int check_topk(const char *who, const als_factors *items, const als_factors *queries, int64_t n_query, int k,
+                      const als_csr *liked) {
+  ALS_REQUIRE(items->f == queries->f, "%s: items have %d factors, queries %d", who, items->f, queries->f);
+  ALS_REQUIRE(k >= 0 && n_query >= 0, "%s: negative k or n_query", who);
+  ALS_REQUIRE(!liked || liked->rows == n_query, "%s: liked has %lld rows for %lld queries", who,
+              liked ? (long long)liked->rows : 0LL, (long long)n_query);
+  ALS_REQUIRE(!liked || liked->host || liked->segs.empty(), "%s: the liked CSR (%lld nonzeros) is held as segments; split the queries "
+              "into calls whose liked rows hold fewer than 2^31 - 1 nonzeros", who, liked ? (long long)liked->nnz : 0LL);
+  if (liked && liked->host) {
+    set_error("%s: the liked CSR is host-resident; upload the filter with als_csr_upload or als_csr_upload64", who);
+    return ALS_E_UNSUPPORTED;
+  }
+  ALS_REQUIRE(!liked || liked->cols == items->rows, "%s: liked has %lld columns for %lld items", who,
+              liked ? (long long)liked->cols : 0LL, (long long)items->rows);
+  return ALS_OK;
+}
+
 ALS_API int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
                      int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
                      const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host) {
   ALS_REQUIRE(ctx && items && queries && ids_host && scores_host, "als_topk: NULL argument");
-  ALS_REQUIRE(items->f == queries->f, "als_topk: items have %d factors, queries %d", items->f, queries->f);
-  ALS_REQUIRE(k >= 0 && n_query >= 0, "als_topk: negative k or n_query");
-  ALS_REQUIRE(!liked || liked->rows == n_query, "als_topk: liked has %lld rows for %lld queries",
-              liked ? (long long)liked->rows : 0LL, (long long)n_query);
-  ALS_REQUIRE(!liked || liked->host || liked->segs.empty(), "als_topk: the liked CSR (%lld nonzeros) is held as segments; split the queries "
-              "into calls whose liked rows hold fewer than 2^31 - 1 nonzeros", liked ? (long long)liked->nnz : 0LL);
-  if (liked && liked->host) {
-    set_error("als_topk: the liked CSR is host-resident; upload the filter with als_csr_upload or als_csr_upload64");
-    return ALS_E_UNSUPPORTED;
-  }
-  ALS_REQUIRE(!liked || liked->cols == items->rows, "als_topk: liked has %lld columns for %lld items",
-              liked ? (long long)liked->cols : 0LL, (long long)items->rows);
+  int rc = check_topk("als_topk", items, queries, n_query, k, liked);
+  if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaSetDevice(ctx->device));
   return launch_topk(ctx, items, queries, query_rows, n_query, k, item_norms_host, liked, filter_items, n_filter,
                      ids_host, scores_host);
+}
+
+ALS_API int als_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+                                int64_t n_query, int k, const als_csr *liked, const als_csr *test, const double *gain_host,
+                                const double *gain_sum_host, double *sums) {
+  ALS_REQUIRE(ctx && items && queries && test && sums, "als_ranking_metrics: NULL argument");
+  int rc = check_topk("als_ranking_metrics", items, queries, n_query, k, liked);
+  if (rc != ALS_OK) return rc;
+  ALS_REQUIRE(k >= 1, "als_ranking_metrics: k = %d ranks nothing", k);
+  ALS_REQUIRE(gain_host && gain_sum_host, "als_ranking_metrics: NULL gain table");
+  ALS_REQUIRE(test->rows == n_query, "als_ranking_metrics: test has %lld rows for %lld queries", (long long)test->rows,
+              (long long)n_query);
+  ALS_REQUIRE(test->cols == items->rows, "als_ranking_metrics: test has %lld columns for %lld items", (long long)test->cols,
+              (long long)items->rows);
+  if (test->host || !test->segs.empty()) {
+    set_error("als_ranking_metrics: the test CSR is %s; upload it as one device-resident CSR of fewer than 2^31 - 1 "
+              "nonzeros (split the queries)", test->host ? "host-resident" : "held as segments");
+    return ALS_E_UNSUPPORTED;
+  }
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  return launch_ranking_metrics(ctx, items, queries, query_rows, n_query, k, liked, test, gain_host, gain_sum_host, sums);
 }

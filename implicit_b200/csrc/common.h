@@ -318,5 +318,22 @@ int launch_topk_tc(als_ctx *ctx, const float *items, int64_t n_items, const floa
 int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
                 int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
                 const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host);
+// The top-k of launch_topk left on the device: ids and scores [n_query, k_eff] in ctx->scratch, valid until the next call
+// that uses the scratch.  k_eff = min(k, items); 0 (and NULL arrays) when there is nothing to rank.
+struct TopkDevice {
+  int32_t *ids = nullptr;
+  float *scores = nullptr;
+  int k_eff = 0;
+};
+int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+                int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
+                const int32_t *filter_items, int64_t n_filter, TopkDevice *out);
+// (indptr, indices) of a device CSR with every row in ascending column order: checked once on the device, and a CSR with
+// an unsorted row gets a sorted copy (indptr rebased to 0) kept with the handle (topk.cu)
+int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, const int32_t **indices);
+// The ranking metrics of the top-k against the withheld items in `test` (metrics.cu; als_ranking_metrics)
+int launch_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+                           int64_t n_query, int k, const als_csr *liked, const als_csr *test, const double *gain_host,
+                           const double *gain_sum_host, double *sums);
 
 }  // namespace als

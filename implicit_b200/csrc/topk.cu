@@ -251,7 +251,7 @@ topk_kernel(const float *__restrict__ items, int n_items, const float *__restric
         const int row = warp * C::ROWS_PER_WARP + rr;
         if (q0 + row >= n_query) break;
         float *srow = Ss + row * SLD;
-        if (liked_indptr && Nxt[row] < i0 + IT) {  // topk.pyx:51-53 (rows in ascending column order: liked_in_order)
+        if (liked_indptr && Nxt[row] < i0 + IT) {  // topk.pyx:51-53 (rows in ascending column order: rows_in_order)
           const int end = liked_indptr[q0 + row + 1];
           int cur = Cur[row];
           for (;;) {
@@ -369,8 +369,8 @@ int run_topk(als_ctx *ctx, const TopkArgs &a) {
 // query row writes a 64-bit sort key per item -- the score in its order-preserving integer form above a tie-breaker
 // that reproduces the reference's heap on ties -- and cub sorts every row descending:
 //   * unfiltered items: tie-breaker ~id, so equal scores come out smaller column first and the boundary of the
-//     first k prefers the smaller column (select.h:23 admits only strictly better scores); the host then reverses
-//     each run of equal scores (select.h:33 emits larger columns first);
+//     first k prefers the smaller column (select.h:23 admits only strictly better scores); sorted_rows_to_topk_kernel
+//     then reverses each run of equal scores (select.h:33 emits larger columns first);
 //   * filtered items all tie at -FLT_MAX, and there the heap's history matters: the first k columns fill it, later
 //     (better) items evict the smallest column first and later filtered columns never enter, so the survivors are the
 //     LARGEST filtered columns below k: tie-breaker id + 1 for id < k, 0 beyond (never selected), already in
@@ -419,7 +419,62 @@ __global__ void segment_offsets_kernel(int32_t *off, int n_seg, int n_items) {
   if (i <= n_seg) off[i] = i * n_items;
 }
 
-int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld, int32_t *ids_host, float *scores_host, int k_out) {
+// The first k entries of each sorted row -> top-k output rows [nq, k]: the scores decoded from the keys, and the ids of
+// every run of equal scores reversed (select.h:33 emits larger columns first), except the filtered tail at -FLT_MAX,
+// which is already in output order.  One warp per row.  A backward pass over the row stores where each entry's run
+// ends (run_end, the sort's free input values); the forward pass finds where it starts and moves the id.
+__global__ void __launch_bounds__(256) sorted_rows_to_topk_kernel(const unsigned long long *__restrict__ keys,
+                                                                  const int32_t *__restrict__ vals, int64_t ld, int k, int nq,
+                                                                  int32_t *__restrict__ run_end, int32_t *__restrict__ ids,
+                                                                  float *__restrict__ scores) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= nq) return;
+  const unsigned long long *kr = keys + row * ld;
+  const int32_t *vr = vals + row * ld;
+  int32_t *er = run_end + row * ld;
+  int32_t *ir = ids + (int64_t)row * k;
+  float *sr = scores + (int64_t)row * k;
+  auto score = [&](int j) {
+    const unsigned ord = (unsigned)(kr[j] >> 32);
+    return __uint_as_float((ord & 0x80000000u) ? (ord & 0x7fffffffu) : ~ord);
+  };
+  const int n_chunks = (k + 31) / 32;
+  int carry_e = k;
+  float carry_s = 0.f;  // score of the entry after the chunk
+  for (int c = n_chunks - 1; c >= 0; --c) {
+    const int j = 32 * c + lane;
+    const bool in = j < k;
+    const float s = in ? score(j) : 0.f;
+    float next = __shfl_down_sync(0xffffffffu, s, 1);
+    if (lane == 31) next = carry_s;
+    const unsigned ends = __ballot_sync(0xffffffffu, in && (j == k - 1 || s != next));
+    const unsigned from_here = ends & (0xffffffffu << lane);
+    const int e = from_here ? 32 * c + __ffs(from_here) : carry_e;  // one past the run's last entry
+    if (in) er[j] = e;
+    carry_e = __shfl_sync(0xffffffffu, e, 0);
+    carry_s = __shfl_sync(0xffffffffu, s, 0);
+  }
+  int carry_b = 0;
+  float carry_p = 0.f;  // score of the entry before the chunk
+  for (int c = 0; c < n_chunks; ++c) {
+    const int j = 32 * c + lane;
+    const bool in = j < k;
+    const float s = in ? score(j) : 0.f;
+    float prev = __shfl_up_sync(0xffffffffu, s, 1);
+    if (lane == 0) prev = carry_p;
+    const unsigned starts = __ballot_sync(0xffffffffu, in && (j == 0 || s != prev));
+    const unsigned upto = starts & (0xffffffffu >> (31 - lane));
+    const int b = upto ? 32 * c + 31 - __clz(upto) : carry_b;  // the run's first entry
+    if (in) {
+      ir[s != -FLT_MAX ? b + er[j] - 1 - j : j] = vr[j];
+      sr[j] = s;
+    }
+    carry_b = __shfl_sync(0xffffffffu, b, 31);
+    carry_p = __shfl_sync(0xffffffffu, s, 31);
+  }
+}
+
+int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld) {
   const int64_t I = a.n_items;
   // rows per pass: keys + values, in and out, within ~1.5 GB and 2^31 elements
   const int64_t per_row = I * 24;
@@ -440,8 +495,6 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld, int32_t *ids_host, flo
   ALS_CUDA(cudaMalloc(&tmp, std::max<size_t>(tmp_bytes, 16)));
   segment_offsets_kernel<<<(rows_per_pass + 256) / 256, 256, 0, ctx->stream>>>(off, rows_per_pass, (int)I);
   int rc = ALS_OK;
-  std::vector<unsigned long long> hk((size_t)rows_per_pass * a.k);
-  std::vector<int32_t> hi((size_t)rows_per_pass * a.k);
   for (int q0 = 0; q0 < a.n_query && rc == ALS_OK; q0 += rows_per_pass) {
     const int nq = std::min(rows_per_pass, a.n_query - q0);
     ProfScope prof(ctx, kProfTopk);
@@ -454,32 +507,18 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld, int32_t *ids_host, flo
       rc = ALS_E_CUDA;
       break;
     }
-    ctx->launches += 2;
-    cudaMemcpy2DAsync(hk.data(), 8 * (size_t)a.k, K_out, 8 * (size_t)I, 8 * (size_t)a.k, nq, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaMemcpy2DAsync(hi.data(), sizeof(int32_t) * a.k, V_out, sizeof(int32_t) * I, sizeof(int32_t) * a.k, nq, cudaMemcpyDeviceToHost,
-                      ctx->stream);
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+    sorted_rows_to_topk_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, ctx->stream>>>(
+        K_out, V_out, I, a.k, nq, V_in, a.ids + (int64_t)q0 * a.k, a.scores + (int64_t)q0 * a.k);
+    if (cudaGetLastError() != cudaSuccess) {
       set_error("topk: fallback pass failed");
       rc = ALS_E_CUDA;
       break;
     }
-    for (int r = 0; r < nq; ++r) {
-      const unsigned long long *kr = hk.data() + (size_t)r * a.k;
-      int32_t *ir = hi.data() + (size_t)r * a.k;
-      float *sr = scores_host + (size_t)(q0 + r) * k_out;
-      for (int j = 0; j < a.k; ++j) {
-        const unsigned ord = (unsigned)(kr[j] >> 32);
-        const unsigned b = (ord & 0x80000000u) ? (ord & 0x7fffffffu) : ~ord;
-        memcpy(&sr[j], &b, sizeof(float));
-      }
-      for (int b = 0; b < a.k;) {  // runs of equal scores come out larger column first (select.h:33)
-        int e2 = b + 1;
-        while (e2 < a.k && sr[e2] == sr[b]) ++e2;
-        if (sr[b] != -FLT_MAX) std::reverse(ir + b, ir + e2);  // the filtered tail is already in output order
-        b = e2;
-      }
-      memcpy(ids_host + (size_t)(q0 + r) * k_out, ir, sizeof(int32_t) * a.k);
-    }
+    ctx->launches += 3;
+  }
+  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess && rc == ALS_OK) {
+    set_error("topk: fallback pass failed");
+    rc = ALS_E_CUDA;
   }
   cudaFree(K_in);
   cudaFree(K_out);
@@ -509,9 +548,11 @@ __global__ void rebase_indptr_kernel(const int32_t *__restrict__ in, int64_t n, 
   if (i < n) out[i] = in[i] - in[0];
 }
 
-// (indptr, indices) of `liked` with every row in ascending column order
-int liked_in_order(als_ctx *ctx, const als_csr *liked, const int32_t **indptr, const int32_t **indices) {
-  als_csr *c = const_cast<als_csr *>(liked);  // the check and the sorted copy are caches of the handle
+}  // namespace
+
+// (indptr, indices) of `csr` with every row in ascending column order
+int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, const int32_t **indices) {
+  als_csr *c = const_cast<als_csr *>(csr);  // the check and the sorted copy are caches of the handle
   if (!c->order_known && c->rows > 0 && c->nnz > 0) {
     int *flag = nullptr;
     int rc = dev_alloc(ctx, (void **)&flag, sizeof(int));
@@ -548,6 +589,8 @@ int liked_in_order(als_ctx *ctx, const als_csr *liked, const int32_t **indptr, c
   return ALS_OK;
 }
 
+namespace {
+
 template <int F>
 int run_topk_f(als_ctx *ctx, const TopkArgs &a) {
   if (a.k <= 64) return run_topk<F, 4>(ctx, a);
@@ -556,16 +599,15 @@ int run_topk_f(als_ctx *ctx, const TopkArgs &a) {
 
 }  // namespace
 
-int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
                 int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
-                const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host) {
+                const int32_t *filter_items, int64_t n_filter, TopkDevice *out) {
+  *out = TopkDevice();
   if (items->ld != queries->ld) {
     set_error("topk: items and queries strides differ");
     return ALS_E_INVALID;
   }
   if (n_query == 0 || k == 0) return ALS_OK;
-  memset(ids_host, 0, sizeof(int32_t) * n_query * k);      // topk.pyx:20-21
-  memset(scores_host, 0, sizeof(float) * n_query * k);
   const int64_t I = items->rows;
   if (I == 0) return ALS_OK;
   if (n_query >= INT32_MAX || I >= INT32_MAX) {
@@ -632,7 +674,7 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
   a.mask = n_filter ? (const uint8_t *)(base + o_mask) : nullptr;
   a.liked_indptr = nullptr;
   a.liked_indices = nullptr;
-  if (liked && (rc = liked_in_order(ctx, liked, &a.liked_indptr, &a.liked_indices)) != ALS_OK) return rc;
+  if (liked && (rc = rows_in_order(ctx, liked, &a.liked_indptr, &a.liked_indices)) != ALS_OK) return rc;
   a.ids = (int32_t *)(base + o_ids);
   a.scores = (float *)(base + o_sc);
 #define CALL(FF) run_topk_f<FF>(ctx, a)
@@ -640,9 +682,8 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
   // (also every model wider than 128 padded factors: its scores come from the generic one-CTA-per-query kernel)
   const bool by_sort = !use_tc && ((k_eff > 64 && (int64_t)k_eff * 16 * 2 * 4 + 96 * 1024 > 227 * 1024) || items->ld > 128);
   if (by_sort) {
-    return topk_by_sort(ctx, a, items->ld, ids_host, scores_host, k);
-  }
-  if (use_tc) {
+    rc = topk_by_sort(ctx, a, items->ld);
+  } else if (use_tc) {
     rc = launch_topk_tc(ctx, a.items, I, a.queries, a.query_rows, n_query, k_eff, a.mask, a.liked_indptr, a.liked_indices,
                         a.ids, a.scores, base + o_tc);
   } else
@@ -661,11 +702,27 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
   }
 #undef CALL
   if (rc != ALS_OK) return rc;
+  out->ids = a.ids;
+  out->scores = a.scores;
+  out->k_eff = k_eff;
+  return ALS_OK;
+}
+
+int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+                int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
+                const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host) {
+  if (n_query > 0 && k > 0 && items->ld == queries->ld) {
+    memset(ids_host, 0, sizeof(int32_t) * n_query * k);  // topk.pyx:20-21
+    memset(scores_host, 0, sizeof(float) * n_query * k);
+  }
+  TopkDevice t;
+  int rc = topk_device(ctx, items, queries, query_rows, n_query, k, item_norms_host, liked, filter_items, n_filter, &t);
+  if (rc != ALS_OK || t.k_eff == 0) return rc;
   // outputs: device [n_query, k_eff] -> host [n_query, k]
-  ALS_CUDA(cudaMemcpy2DAsync(ids_host, sizeof(int32_t) * k, base + o_ids, sizeof(int32_t) * k_eff,
-                             sizeof(int32_t) * k_eff, n_query, cudaMemcpyDeviceToHost, ctx->stream));
-  ALS_CUDA(cudaMemcpy2DAsync(scores_host, sizeof(float) * k, base + o_sc, sizeof(float) * k_eff,
-                             sizeof(float) * k_eff, n_query, cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaMemcpy2DAsync(ids_host, sizeof(int32_t) * k, t.ids, sizeof(int32_t) * t.k_eff, sizeof(int32_t) * t.k_eff,
+                             n_query, cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaMemcpy2DAsync(scores_host, sizeof(float) * k, t.scores, sizeof(float) * t.k_eff, sizeof(float) * t.k_eff,
+                             n_query, cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   return ALS_OK;
 }

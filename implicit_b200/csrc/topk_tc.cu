@@ -208,7 +208,7 @@ topk_tc_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   }
   auto consider = [&](float s, int id) {
     if (id >= n_items) return;
-    while (lnext < id) {  // both the candidates and the liked list come in increasing item order (liked_in_order)
+    while (lnext < id) {  // both the candidates and the liked list come in increasing item order (rows_in_order)
       ++lp;
       lnext = lp < lend ? liked_indices[lp] : INT_MAX;
     }

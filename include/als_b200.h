@@ -256,6 +256,24 @@ int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors *X, con
 int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
              int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
              const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host);
+/* Ranking metrics at k of the top-k above, without its ids leaving the device: the ids als_topk would return (no item
+ * norms, no filter_items; ranks past the items are id 0) are scored against `test`, a CSR over the query rows of the
+ * withheld items (any order within a row, repeats and stored zeros allowed; sorted on the device like `liked`).  Per
+ * query with L > 0 distinct withheld items and hit_j = "the id at rank j is withheld":
+ *   sums[0] += sum_j hit_j                          sums[1] += min(k, L)
+ *   sums[2] += sum_j hit_j * (hits at ranks <= j) / (j + 1) / min(k, L)
+ *   sums[3] += sum_j hit_j * gain[j] / gain_sum[min(k, L) - 1]
+ *   sums[4] += [sum_{miss j} (hits before j) + (hits + L) / 2 * (items - L - misses)] / (L * (items - L))
+ *   sums[5] += 1
+ * in fp64, with the caller's gain[k] (1 / log2(j + 2)) and gain_sum[k] (its running sum) tables.  Queries without
+ * withheld items add nothing.  The sums are deterministic: two identical calls return the same bits.  Refuses what
+ * als_topk refuses, k < 1, a `test` of other than n_query rows or other than items' row count of columns, and a
+ * host-resident or segmented `test`.  Synchronises.
+ * Replaces the per-user loop of ranking_metrics_at_k, implicit/evaluation.pyx:366-475 (precision = sums[0] / sums[1],
+ * map, ndcg and auc = sums[2 .. 4] / sums[5]). */
+int als_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
+                        int64_t n_query, int k, const als_csr *liked, const als_csr *test, const double *gain_host,
+                        const double *gain_sum_host, double *sums /* [6] */);
 
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink/NVSwitch) -------------------------------- */
 /* The reference has no multi-GPU path (`// TODO: multi-gpu support`, implicit/gpu/als.cu:169). */
