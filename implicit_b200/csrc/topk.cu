@@ -366,18 +366,13 @@ int run_topk(als_ctx *ctx, const TopkArgs &a) {
 
 // ---- very large k (the k-lists no longer fit in shared memory): scores to HBM, one segmented sort ---------------
 // rank_items / recommend with N in the thousands up to "all items" (the reference's select.h takes any k).  One CTA per
-// query row writes a 64-bit sort key per item -- the score in its order-preserving integer form above a tie-breaker
-// that reproduces the reference's heap on ties -- and cub sorts every row descending:
-//   * unfiltered items: tie-breaker ~id, so equal scores come out smaller column first and the boundary of the
-//     first k prefers the smaller column (select.h:23 admits only strictly better scores); sorted_rows_to_topk_kernel
-//     then reverses each run of equal scores (select.h:33 emits larger columns first);
-//   * filtered items all tie at -FLT_MAX, and there the heap's history matters: the first k columns fill it, later
-//     (better) items evict the smallest column first and later filtered columns never enter, so the survivors are the
-//     LARGEST filtered columns below k: tie-breaker id + 1 for id < k, 0 beyond (never selected), already in
-//     output order.
+// query row writes a 64-bit sort key per item -- the score in its order-preserving integer form above the column --
+// and cub sorts every row descending: by score, equal scores larger column first (select.h:33's output order).
+// Filtered items are scores of -FLT_MAX like any other.  Which of the items tied at the k-th score survive is
+// decided afterwards, from the sorted row (sorted_rows_to_topk_kernel).
 __global__ void __launch_bounds__(256) score_rows_kernel(const float *__restrict__ items, int n_items, int ld,
                                                          const float *__restrict__ queries, const int32_t *__restrict__ query_rows,
-                                                         int q0, int k, const float *__restrict__ norms,
+                                                         int q0, const float *__restrict__ norms,
                                                          const uint8_t *__restrict__ mask, const int32_t *__restrict__ liked_indptr,
                                                          const int32_t *__restrict__ liked_indices,
                                                          unsigned long long *__restrict__ keys, int32_t *__restrict__ ids) {
@@ -388,11 +383,10 @@ __global__ void __launch_bounds__(256) score_rows_kernel(const float *__restrict
   __syncthreads();
   unsigned long long *out = keys + (int64_t)blockIdx.x * n_items;
   int32_t *oid = ids + (int64_t)blockIdx.x * n_items;
-  auto key_of = [&](float sc, int i, bool filtered) -> unsigned long long {
+  auto key_of = [&](float sc, int i) -> unsigned long long {
     const unsigned b = __float_as_uint(sc);
     const unsigned ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);  // monotone map of floats onto unsigned integers
-    const unsigned tie = filtered ? (i < k ? (unsigned)i + 1u : 0u) : ~(unsigned)i;
-    return ((unsigned long long)ord << 32) | tie;
+    return ((unsigned long long)ord << 32) | (unsigned)i;
   };
   for (int i = threadIdx.x; i < n_items; i += blockDim.x) {
     const float4 *it = reinterpret_cast<const float4 *>(items + (int64_t)i * ld);
@@ -403,14 +397,14 @@ __global__ void __launch_bounds__(256) score_rows_kernel(const float *__restrict
     }
     if (norms) acc /= norms[i];                 // topk.pyx:48-49
     const bool filtered = mask && mask[i];      // topk.pyx:55-56
-    out[i] = key_of(filtered ? -FLT_MAX : acc, i, filtered);
+    out[i] = key_of(filtered ? -FLT_MAX : acc, i);
     oid[i] = i;
   }
   __syncthreads();
   if (liked_indptr)                              // topk.pyx:51-54
     for (int p = liked_indptr[q] + threadIdx.x; p < liked_indptr[q + 1]; p += blockDim.x) {
       const int i = liked_indices[p];
-      out[i] = key_of(-FLT_MAX, i, true);
+      out[i] = key_of(-FLT_MAX, i);
     }
 }
 
@@ -419,58 +413,58 @@ __global__ void segment_offsets_kernel(int32_t *off, int n_seg, int n_items) {
   if (i <= n_seg) off[i] = i * n_items;
 }
 
-// The first k entries of each sorted row -> top-k output rows [nq, k]: the scores decoded from the keys, and the ids of
-// every run of equal scores reversed (select.h:33 emits larger columns first), except the filtered tail at -FLT_MAX,
-// which is already in output order.  One warp per row.  A backward pass over the row stores where each entry's run
-// ends (run_end, the sort's free input values); the forward pass finds where it starts and moves the id.
+// Each sorted row -> its top-k output row [k], as select.h leaves it.  select.h (:23) admits an item only while its heap
+// has room or the item beats the heap's minimum strictly, and evicts the minimum by (score, column).  So with T the
+// k-th largest score and g the number of items above T (the sorted row's positions [0, g)): every item above T is
+// kept, and of the items scoring exactly T the heap holds the m = k - g with the largest columns <= c*, where c* is
+// the column of the k-th item scoring >= T in column order (the heap fills with items >= T up to c*; after c* no
+// T-item enters, and each later, better item evicts the smallest column scoring T).  The filtered tail at -FLT_MAX
+// is the case T = -FLT_MAX, where c* = k - 1.
+// In the sorted row the T-items are one run [g, e) in descending column order, so the kept ones are m consecutive
+// entries of it, already in output order.  Their place follows from r, the number of T-items with a column <= c*: the
+// c-th smallest T column (run position e - c) is c* or below exactly when c plus the number of better items with a
+// smaller column is at most k.  That holds for every c <= m, so r is found by a binary search over [m, min(k, e - g)],
+// each probe counting the better columns below it across the warp.  One warp per row.
 __global__ void __launch_bounds__(256) sorted_rows_to_topk_kernel(const unsigned long long *__restrict__ keys,
-                                                                  const int32_t *__restrict__ vals, int64_t ld, int k, int nq,
-                                                                  int32_t *__restrict__ run_end, int32_t *__restrict__ ids,
-                                                                  float *__restrict__ scores) {
+                                                                  const int32_t *__restrict__ vals, int n_items, int k, int nq,
+                                                                  int32_t *__restrict__ ids, float *__restrict__ scores) {
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= nq) return;
-  const unsigned long long *kr = keys + row * ld;
-  const int32_t *vr = vals + row * ld;
-  int32_t *er = run_end + row * ld;
-  int32_t *ir = ids + (int64_t)row * k;
-  float *sr = scores + (int64_t)row * k;
-  auto score = [&](int j) {
-    const unsigned ord = (unsigned)(kr[j] >> 32);
-    return __uint_as_float((ord & 0x80000000u) ? (ord & 0x7fffffffu) : ~ord);
-  };
-  const int n_chunks = (k + 31) / 32;
-  int carry_e = k;
-  float carry_s = 0.f;  // score of the entry after the chunk
-  for (int c = n_chunks - 1; c >= 0; --c) {
-    const int j = 32 * c + lane;
-    const bool in = j < k;
-    const float s = in ? score(j) : 0.f;
-    float next = __shfl_down_sync(0xffffffffu, s, 1);
-    if (lane == 31) next = carry_s;
-    const unsigned ends = __ballot_sync(0xffffffffu, in && (j == k - 1 || s != next));
-    const unsigned from_here = ends & (0xffffffffu << lane);
-    const int e = from_here ? 32 * c + __ffs(from_here) : carry_e;  // one past the run's last entry
-    if (in) er[j] = e;
-    carry_e = __shfl_sync(0xffffffffu, e, 0);
-    carry_s = __shfl_sync(0xffffffffu, s, 0);
+  const unsigned long long *kr = keys + (int64_t)row * n_items;
+  const int32_t *vr = vals + (int64_t)row * n_items;
+  auto ord = [&](int j) { return (unsigned)(kr[j] >> 32); };
+  const unsigned t = ord(k - 1);
+  int lo = 0, hi = k - 1;  // g: the first position scoring T
+  while (lo < hi) {
+    const int mid = (lo + hi) / 2;
+    if (ord(mid) == t) hi = mid;
+    else lo = mid + 1;
   }
-  int carry_b = 0;
-  float carry_p = 0.f;  // score of the entry before the chunk
-  for (int c = 0; c < n_chunks; ++c) {
-    const int j = 32 * c + lane;
-    const bool in = j < k;
-    const float s = in ? score(j) : 0.f;
-    float prev = __shfl_up_sync(0xffffffffu, s, 1);
-    if (lane == 0) prev = carry_p;
-    const unsigned starts = __ballot_sync(0xffffffffu, in && (j == 0 || s != prev));
-    const unsigned upto = starts & (0xffffffffu >> (31 - lane));
-    const int b = upto ? 32 * c + 31 - __clz(upto) : carry_b;  // the run's first entry
-    if (in) {
-      ir[s != -FLT_MAX ? b + er[j] - 1 - j : j] = vr[j];
-      sr[j] = s;
+  const int g = lo, m = k - g;
+  lo = k, hi = n_items;  // e: one past the last position scoring T
+  while (lo < hi) {
+    const int mid = (lo + hi) / 2;
+    if (ord(mid) != t) hi = mid;
+    else lo = mid + 1;
+  }
+  const int e = lo;
+  int r = m;
+  if (e > k) {  // some T-items are left out
+    lo = m, hi = min(k, e - g);
+    while (lo < hi) {
+      const int c = (lo + hi + 1) / 2, col = vr[e - c];
+      int below = 0;
+      for (int p = lane; p < g; p += 32) below += vr[p] < col;
+      if (c + __reduce_add_sync(0xffffffffu, below) <= k) lo = c;
+      else hi = c - 1;
     }
-    carry_b = __shfl_sync(0xffffffffu, b, 31);
-    carry_p = __shfl_sync(0xffffffffu, s, 31);
+    r = lo;
+  }
+  for (int j = lane; j < k; j += 32) {
+    const int p = j < g ? j : e - r + (j - g);
+    const unsigned o = ord(p);
+    ids[(int64_t)row * k + j] = vr[p];
+    scores[(int64_t)row * k + j] = __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
   }
 }
 
@@ -498,7 +492,7 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld) {
   for (int q0 = 0; q0 < a.n_query && rc == ALS_OK; q0 += rows_per_pass) {
     const int nq = std::min(rows_per_pass, a.n_query - q0);
     ProfScope prof(ctx, kProfTopk);
-    score_rows_kernel<<<nq, 256, ld * sizeof(float), ctx->stream>>>(a.items, a.n_items, ld, a.queries, a.query_rows, q0, a.k, a.norms,
+    score_rows_kernel<<<nq, 256, ld * sizeof(float), ctx->stream>>>(a.items, a.n_items, ld, a.queries, a.query_rows, q0, a.norms,
                                                                      a.mask, a.liked_indptr, a.liked_indices, K_in, V_in);
     cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairsDescending(tmp, tmp_bytes, K_in, K_out, V_in, V_out, (int)((int64_t)nq * I), nq,
                                                                        off, off + 1, 0, 64, ctx->stream);
@@ -508,7 +502,7 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld) {
       break;
     }
     sorted_rows_to_topk_kernel<<<(unsigned)ceil_div(nq, 8), 256, 0, ctx->stream>>>(
-        K_out, V_out, I, a.k, nq, V_in, a.ids + (int64_t)q0 * a.k, a.scores + (int64_t)q0 * a.k);
+        K_out, V_out, a.n_items, a.k, nq, a.ids + (int64_t)q0 * a.k, a.scores + (int64_t)q0 * a.k);
     if (cudaGetLastError() != cudaSuccess) {
       set_error("topk: fallback pass failed");
       rc = ALS_E_CUDA;

@@ -189,10 +189,21 @@ def _port_topk(items, query, k, item_norms=None, filter_query_items=None, filter
     return indices, distances
 
 
+def _port_select(scores, k):
+    """select<float>(batch, k, ids, distances) on precomputed scores (implicit/cpu/select.h:12-39): (ids, scores) of
+    shape [rows, k], zero past the row's item count like topk.pyx:20-21."""
+    scores = np.ascontiguousarray(np.atleast_2d(scores), dtype=np.float32)
+    rows, cols = scores.shape
+    ids = np.zeros((rows, k), dtype=np.int32)
+    distances = np.zeros((rows, k), dtype=np.float32)
+    _port_lib().oracle_select(_f32(scores), rows, cols, int(k), _i32(ids), _f32(distances))
+    return ids, distances
+
+
 port = types.SimpleNamespace(
     name="port", least_squares=_port_least_squares, _least_squares=_port__least_squares,
     least_squares_cg=_port_least_squares_cg, least_squares_cg_with_gramian=_port_least_squares_cg_with_gramian,
-    calculate_loss=_port_calculate_loss, topk=_port_topk, gramian=_port_gramian,
+    calculate_loss=_port_calculate_loss, topk=_port_topk, gramian=_port_gramian, select=_port_select,
 )
 
 

@@ -313,6 +313,31 @@ def topk_mismatches(ids, scores, ref_ids, ref_scores, noise):
     return same, bad
 
 
+def select_h(scores, k):
+    """The top-k that select.h's heap (implicit/cpu/select.h:12-39) leaves, restated without the heap, for rows of
+    scores of any float type.  With kk = min(k, I), T the kk-th largest score of a row and g the number of items
+    above T: every item above T is kept, and the m = kk - g items with the largest columns <= c* among those scoring
+    exactly T, where c* is the column of the kk-th item scoring >= T in column order.  Output descending by score,
+    equal scores larger column first; ids and scores are zero past kk (topk.pyx:20-21)."""
+    S = np.atleast_2d(np.asarray(scores))
+    n, I = S.shape
+    kk = min(k, I)
+    ids = np.zeros((n, k), dtype=np.int32)
+    out = np.zeros((n, k), dtype=S.dtype)
+    if kk == 0:
+        return ids, out
+    for r in range(n):
+        s = S[r]
+        T = np.partition(s, I - kk)[I - kk]
+        above = np.flatnonzero(s > T)
+        c_star = np.flatnonzero(s >= T)[kk - 1]
+        tied = np.flatnonzero(s[:c_star + 1] == T)
+        sel = np.concatenate([above, tied[len(tied) - (kk - len(above)):]])
+        sel = sel[np.lexsort((-sel, -s[sel]))]
+        ids[r, :kk], out[r, :kk] = sel, s[sel]
+    return ids, out
+
+
 def golden_cases():
     """The fit fixtures (chol_*, cg_*); eval_metrics.npz belongs to tests/test_evaluation.py."""
     return sorted(f[:-4] for f in os.listdir(GOLDEN) if f.endswith(".npz") and f.startswith(("chol_", "cg_")))
