@@ -70,6 +70,7 @@ SIGNATURES = {
     "als_least_squares": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_f64, P(c_i64)]),
     "als_least_squares_with_gramian": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_f64, P(c_i64)]),
     "als_gramian_shard": (c_int, [c_void_p, c_void_p, c_i64, c_i64]),
+    "als_gramian_read": (c_int, [c_void_p, c_void_p, c_void_p]),
     "als_least_squares_pregram_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_f64]),
     "als_solver_status": (c_int, [c_void_p, P(c_i64), P(c_int)]),
     "als_whitened_factors": (c_int, [c_void_p, c_void_p, c_f64, c_void_p, c_void_p]),
@@ -611,6 +612,13 @@ def whitened_factors(ctx, Y, regularization):
 def gramian_shard(ctx, Y, row0, nrows):
     """Gramian over this rank's rows of Y, summed across ranks, left on the device for the *_pregram solves."""
     check(ctx.lib.als_gramian_shard(ctx.h, Y.h, int(row0), int(nrows)))
+
+
+def gramian_read(ctx, Y):
+    """The Gramian the context holds from the last gramian / gramian_shard on Y, downloaded."""
+    G = np.empty((Y.factors, Y.factors), dtype=np.float32)
+    check(ctx.lib.als_gramian_read(ctx.h, Y.h, ptr(G)))
+    return G
 
 
 def half_pregram_async(ctx, Cui, X, Y, regularization, use_cg, cg_steps=3):

@@ -1145,18 +1145,22 @@ static int check_half(const char *who, als_ctx *ctx, const als_csr *C, const als
   return ensure_schedule(ctx, const_cast<als_csr *>(C));  // a device-transposed matrix sorts its rows at first use
 }
 
+ALS_API int als_gramian_read(als_ctx *ctx, const als_factors *Y, float *G_host) {
+  ALS_REQUIRE(ctx && Y && G_host, "als_gramian_read: NULL argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  std::vector<float> tmp((size_t)Y->ld * Y->ld);
+  ALS_CUDA(cudaMemcpyAsync(tmp.data(), ctx->G, sizeof(float) * tmp.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < Y->f; ++i) memcpy(G_host + (size_t)i * Y->f, tmp.data() + (size_t)i * Y->ld, sizeof(float) * Y->f);
+  return ALS_OK;
+}
+
 ALS_API int als_gramian(als_ctx *ctx, const als_factors *Y, float *G_host) {
   ALS_REQUIRE(ctx && Y, "als_gramian: NULL argument");
   ALS_CUDA(cudaSetDevice(ctx->device));
   int rc = launch_gramian(ctx, Y);
   if (rc != ALS_OK) return rc;
-  if (G_host) {
-    std::vector<float> tmp((size_t)Y->ld * Y->ld);
-    ALS_CUDA(cudaMemcpyAsync(tmp.data(), ctx->G, sizeof(float) * tmp.size(), cudaMemcpyDeviceToHost, ctx->stream));
-    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    for (int i = 0; i < Y->f; ++i) memcpy(G_host + (size_t)i * Y->f, tmp.data() + (size_t)i * Y->ld, sizeof(float) * Y->f);
-  }
-  return ALS_OK;
+  return G_host ? als_gramian_read(ctx, Y, G_host) : ALS_OK;
 }
 
 // Reads the first row whose normal equations were not positive definite from bad_row[0, n) (n = 1: the half just run;

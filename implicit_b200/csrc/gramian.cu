@@ -5,9 +5,13 @@
 // memory and writes one F x F partial; a second tiny kernel sums the partials in a fixed order in fp64 so the
 // result is deterministic and independent of the grid size rounding.
 //   64 padded factors: gramian_tc_kernel on wgmma (dense.cu), unless the gramian_fma knob is set;
-//   f <= 128: gramian_partial_kernel -- fp32 FMA register tiles (the CG configurations).
-// An mma.sync 3xTF32 variant (long fp32 accumulator chains on the tensor core) was removed: on one H100 it was
-// 8-11x outside |G - G64| <= 1e-6 |Y|^T|Y| at a million rows (tests/test_gpu_kernel_edges.py).
+//   f <= 128: gramian_partial_kernel -- fp32 FMA register tiles (the CG configurations);
+//   128 < padded factors <= 1024: gramian_wide_kernel -- fp32 FMA 4 x 4 register tiles per 64 x 64 tile of G.
+// No fp32 register accumulator adds more than kFoldRows = 256 rows: each FMA kernel then folds its register tile into
+// a second accumulator (fp32 in shared memory at <= 128 factors, fp64 above), and the wgmma kernel adds chains of 64
+// rows into fp32 registers.  One fp32 chain over all of a thread's rows (350k rows in the wide kernel at 2^20 rows and
+// 1024 factors, 38k in the partial kernel at 10M rows) walks far outside |G - G64| <= 1e-6 |Y|^T|Y| elementwise
+// (tests/test_gpu_gramian_widths.py); so did an mma.sync 3xTF32 variant, 8-11x at a million rows on one H100.
 #include <limits.h>
 
 #include "cholesky_device.cuh"
@@ -16,24 +20,35 @@ namespace als {
 
 namespace {
 
-constexpr int kGramRows = 32;  // rows of Y staged per step (FMA version)
+constexpr int kGramRows = 32;   // rows of Y staged per step (FMA version)
+constexpr int kFoldRows = 256;  // rows an fp32 register accumulator adds at most before it is folded
 
 // fp32 FMA version (round-to-nearest accumulation).  Thread (ty, tx) of the 16 x 16 block owns the T x T
 // sub-block of G at rows T ty .. T ty + T - 1, columns T tx .. T tx + T - 1 (T = F / 16), so both of its operands
 // are contiguous in a staged row and arrive as 16-byte shared-memory loads: T^2 FMAs per 2 T / 4 loads.
+// Every kFoldRows / kGramRows steps of the CTA, and after its last step, the register tile is added into the thread's
+// fp32 second level in dynamic shared memory, T^2 x 256 floats at word (i T + j) 256 + thread (conflict-free), and the
+// partial is written from there: registers have no room for a second level at T = 8 with two CTAs per SM, and adding
+// the register tile at the store instead spills at T = 8.  Two fp32 levels suffice, as 2 x SMs CTAs share the rows:
+// an fp32 emulation of 10M rows at 128 factors stays within 0.02 of the bar.
 template <int T>  // F = 16 * T
 __global__ void __launch_bounds__(256) gramian_partial_kernel(const float *__restrict__ Y, int64_t rows, int ld,
                                                               float *__restrict__ partials) {
   constexpr int F = 16 * T;
   __shared__ __align__(16) float tile[kGramRows][F];
+  extern __shared__ float folded[];  // [T * T][256]
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[T][T];
 #pragma unroll
   for (int a = 0; a < T; ++a)
 #pragma unroll
-    for (int b = 0; b < T; ++b) acc[a][b] = 0.f;
+    for (int b = 0; b < T; ++b) {
+      acc[a][b] = 0.f;
+      folded[(a * T + b) * 256 + threadIdx.x] = 0.f;
+    }
 
   const int64_t steps = (rows + kGramRows - 1) / kGramRows;
+  int pending = 0;
   for (int64_t s = blockIdx.x; s < steps; s += gridDim.x) {
     const int64_t r0 = s * kGramRows;
     // coalesced float4 staging (ld == F by construction)
@@ -68,19 +83,31 @@ __global__ void __launch_bounds__(256) gramian_partial_kernel(const float *__res
         for (int j = 0; j < T; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
     }
     __syncthreads();
+    if (++pending == kFoldRows / kGramRows || s + gridDim.x >= steps) {
+      pending = 0;
+#pragma unroll
+      for (int i = 0; i < T; ++i)
+#pragma unroll
+        for (int j = 0; j < T; ++j) {
+          folded[(i * T + j) * 256 + threadIdx.x] += acc[i][j];
+          acc[i][j] = 0.f;
+        }
+    }
   }
   float *out = partials + (size_t)blockIdx.x * F * F;
 #pragma unroll
   for (int i = 0; i < T; ++i)
 #pragma unroll
-    for (int j = 0; j < T; ++j) out[(T * ty + i) * F + T * tx + j] = acc[i][j];
+    for (int j = 0; j < T; ++j) out[(T * ty + i) * F + T * tx + j] = folded[(i * T + j) * 256 + threadIdx.x];
 }
 
 // 128 < padded factors <= 1024: one 64 x 64 tile of G per CTA and row chunk (blockIdx = (tile column, tile row, chunk)),
-// fp32 FMA register tiles of 4 x 4 per thread; the chunk partials are summed in fp64 in a fixed order like the others.
+// fp32 FMA register tiles of 4 x 4 per thread, added every kFoldRows rows into an fp64 tile in shared memory (registers
+// would cost a CTA per SM); the chunk partials are summed in fp64 in a fixed order like the others.
 __global__ void __launch_bounds__(256) gramian_wide_kernel(const float *__restrict__ Y, int64_t rows, int ld, float *__restrict__ partials,
                                                            int64_t rows_per_part) {
   __shared__ __align__(16) float A[16][64], B[16][64];
+  __shared__ double folded[16][256];  // [4 i + j][thread]
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int bj = blockIdx.x, bi = blockIdx.y;
   const int64_t r0 = (int64_t)blockIdx.z * rows_per_part, r1 = min(rows, r0 + rows_per_part);
@@ -88,7 +115,11 @@ __global__ void __launch_bounds__(256) gramian_wide_kernel(const float *__restri
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int j = 0; j < 4; ++j) {
+      acc[i][j] = 0.f;
+      folded[4 * i + j][threadIdx.x] = 0.0;
+    }
+  int pending = 0;
   for (int64_t r = r0; r < r1; r += 16) {
     const int64_t row = r + ty;  // 16 rows x 16 float4 words: one word of each tile per thread
     float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
@@ -110,12 +141,27 @@ __global__ void __launch_bounds__(256) gramian_wide_kernel(const float *__restri
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
     }
     __syncthreads();
+    if (++pending == kFoldRows / 16) {
+      pending = 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          folded[4 * i + j][threadIdx.x] += acc[i][j];
+          acc[i][j] = 0.f;
+        }
+    }
   }
+  float v[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[i][j] = (float)(folded[4 * i + j][threadIdx.x] + acc[i][j]);
   float *out = partials + (size_t)blockIdx.z * ld * ld;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
     *reinterpret_cast<float4 *>(out + (size_t)(64 * bi + 4 * ty + i) * ld + 64 * bj + 4 * tx) =
-        make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+        make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
 }
 
 // 32 consecutive elements x 8 groups of partials per block: group pg sums partials pg, pg + 8, ... in fp64, the 8
@@ -157,7 +203,9 @@ __global__ void regularize_kernel(const float *__restrict__ G, float *__restrict
 
 template <int T>
 static int run_gramian(als_ctx *ctx, const als_factors *Y, int grid) {
-  gramian_partial_kernel<T><<<grid, 256, 0, ctx->stream>>>(Y->d, Y->rows, Y->ld, ctx->gram_partials);
+  const int smem = T * T * 256 * (int)sizeof(float);  // the fp32 second level; up to 64 KB at T = 8
+  ALS_CUDA(cudaFuncSetAttribute(gramian_partial_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  gramian_partial_kernel<T><<<grid, 256, smem, ctx->stream>>>(Y->d, Y->rows, Y->ld, ctx->gram_partials);
   return ALS_OK;
 }
 
@@ -218,10 +266,10 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
     case 2: rc = run_gramian<2>(ctx, Y, grid); break;
     case 3: rc = run_gramian<3>(ctx, Y, grid); break;
     case 4: rc = run_gramian<4>(ctx, Y, grid); break;
-    case 5: run_gramian<5>(ctx, Y, grid); break;
-    case 6: run_gramian<6>(ctx, Y, grid); break;
-    case 7: run_gramian<7>(ctx, Y, grid); break;
-    case 8: run_gramian<8>(ctx, Y, grid); break;
+    case 5: rc = run_gramian<5>(ctx, Y, grid); break;
+    case 6: rc = run_gramian<6>(ctx, Y, grid); break;
+    case 7: rc = run_gramian<7>(ctx, Y, grid); break;
+    case 8: rc = run_gramian<8>(ctx, Y, grid); break;
     default: set_error("gramian: bad padded factors %d", F); return ALS_E_UNSUPPORTED;
   }
   if (rc != ALS_OK) return rc;

@@ -191,6 +191,10 @@ int als_factors_destroy(als_factors *f);
  * may be NULL) receives a copy.  Replaces np.dot(Y.T, Y) (implicit/cpu/_als.pyx:70,164,268) and
  * LeastSquaresSolver::calculate_yty (implicit/gpu/als.cu:122-152). */
 int als_gramian(als_ctx *ctx, const als_factors *Y, float *G_host);
+/* Copies the Gramian that the context holds (from the last als_gramian or als_gramian_shard on Y, which
+ * must not have been followed by another Gramian) into G_host (factors*factors floats).  Test / tooling entry:
+ * als_gramian_shard leaves its result on the device. */
+int als_gramian_read(als_ctx *ctx, const als_factors *Y, float *G_host);
 
 /* One Cholesky half-iteration: for every row u of C:  X[row_offset + u] = (Y^T Y + reg I + Y^T (|C_u| - I) Y)^-1 Y^T C_u+ p_u.
  * Computes the Gramian of Y itself.  *bad_row = -1, or the first (global) row whose normal

@@ -43,7 +43,7 @@ REG = 0.01
 #: further).  The factors below keep a margin of 1.2x over those measurements.
 MAX_FACTOR, WIDE_MAX_FACTOR = 4.0, 12.5
 #: floor of the item half's max bar, 4x the fp32 floor.  A cold user half leaves X with some rows far off (see above);
-#: the device forms X^T X with fp32 FMA chains (1e-6 |X|^T |X| elementwise, test_gpu_kernel_edges.py), the reference
+#: the device forms X^T X with fp32 FMA chains (1e-6 |X|^T |X| elementwise, test_gpu_gramian_widths.py), the reference
 #: with a blocked BLAS product.  Measured on one H100 80GB HBM3 at 400 W: up to 4.2e-5 (f = 64 cold) where the
 #: reference's worst item row is 6.5e-6; medians stay at 0.13 ... 0.16 of their bar.
 ITEM_MAX_FLOOR = 8e-5

@@ -27,47 +27,7 @@ KINDS = ["mixed", "cold", "decades", "zero_rows"]
 
 
 # ---------------------------------------------------------------------------------------- Gramian
-def gramian_paths(f):
-    if (f + 15) // 16 * 16 == 64:  # the path follows the padded width: 49..63 factors run the wgmma kernel too
-        return {"wgmma": {}, "gramian_fma": {"gramian_fma": 1}}
-    return {"fma": {}}
-
-
-@pytest.mark.parametrize("kind", KINDS)
-@pytest.mark.parametrize("f", [16, 40, 49, 63, 64, 100, 128])
-def test_gramian_elementwise_against_fp64(lib, ctx, sm, f, kind):
-    """Error model: an fp32-faithful Gramian is the fp64 one up to a few ulps of the sum of |terms| per entry, so
-    |G - G64| <= 1e-6 (|Y|^T |Y|) elementwise -- the normwise 1e-6 of C2 applied entry by entry, which a wrong
-    off-diagonal entry that is small next to the diagonal cannot hide under.
-    The FMA kernels (every width but 64, and gramian_fma) sum about 4000 rows per thread in fp32 at a million rows,
-    whose round-to-nearest walk reaches ~sqrt(4000) ulps: there the bar is 3e-6 (measured on one H100: 2.2e-6 with row
-    norms over six decades, under 1e-6 for the other data).  The wgmma kernel adds chains of 64 rows into its fp32
-    accumulators and stays under 1e-6 at every size.  (An mma.sync variant measured 8-11e-6 at a million rows and was
-    removed.)"""
-    worst = {}
-    for rows in row_counts(sm):
-        Y = factors_of(kind, rows, f, seed=rows + f)
-        Y64 = Y.astype(np.float64)
-        G64 = Y64.T @ Y64
-        A = np.abs(Y64)
-        bar = 1e-6 * (A.T @ A)
-        d = lib.DeviceFactors.from_host(ctx, Y)
-        for name, knobs in gramian_paths(f).items():
-            for k, v in knobs.items():
-                ctx.set_knob(k, v)
-            G = lib.gramian(ctx, d)
-            for k in knobs:
-                ctx.set_knob(k, KNOB_DEFAULTS[k])
-            scale = 3.0 if name != "wgmma" and rows > 1e6 else 1.0
-            r = worst_ratio(np.abs(G - G64), scale * bar)
-            worst[(name, rows)] = r
-        d.close()
-    for (name, rows), r in sorted(worst.items()):
-        print(f"Gramian f={f} {kind} {name} rows={rows}: worst |G - G64| / bar = {r:.3f}")
-    bad = {key: r for key, r in worst.items() if not r <= 1.0}
-    assert not bad, f"Gramian outside 1e-6 |Y|^T|Y|: {bad}"
-
-
+# The Gramian itself, at every width, path and partition edge: test_gpu_gramian_widths.py.
 def test_gramian_shard_window_feeds_the_half(lib, ctx, orc, sm):
     """als_gramian_shard on a window [37, 37 + 128 sm + 5) of Y (the TMA map starts at an offset pointer), then a
     Cholesky half with that device-resident Gramian, against cholesky_truth with the window's fp64 Gramian.

@@ -83,7 +83,7 @@ def test_loss_terms_on_shards(lib, ctx, orc, f):
     0, in the middle and on a giant row: each of the three terms against loss_truth over that row range (terms[0] within K
     times its absolute sum, terms[1], a sum of fp32 |c| in fp64, within 1e-12), and the shards'
     terms summed into the loss of the whole.  terms[2] = reg tr(Y^T Y) comes from the device's fp32 Gramian, whose
-    bar is 1e-6 |Y|^T |Y| elementwise (test_gpu_kernel_edges.py); measured on one H100 80GB HBM3 at 400 W: 3.2e-7 of
+    bar is 1e-6 |Y|^T |Y| elementwise (test_gpu_gramian_widths.py); measured on one H100 80GB HBM3 at 400 W: 3.2e-7 of
     its absolute sum at 6000 items."""
     users, items, Cui = case(f)
     giant = 3 + 47 * 1  # mixed_csr's second giant length (3073) sits on row 50

@@ -1,5 +1,6 @@
 """Models wider than 128 factors (the reference's CUDA solver takes up to 1024, implicit/gpu/als.cu:177-178; its CPU
-path any width): CG half, Gramian, loss, top-k and the fit loop at 192 / 260 / 512 factors against the oracle."""
+path any width): CG half, loss, top-k and the fit loop at 192 / 260 / 512 factors against the oracle (the Gramian:
+test_gpu_gramian_widths.py)."""
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -36,18 +37,6 @@ def _case(users, items, nnz, f, seed):
     X = (rng.standard_normal((users, f)) * 0.1).astype(np.float32)
     Y = (rng.standard_normal((items, f)) * 0.1).astype(np.float32)
     return Cui, X, Y
-
-
-@pytest.mark.parametrize("f", [192, 260, 512])
-def test_wide_gramian(lib, ctx, f):
-    rng = np.random.default_rng(f)
-    Y = (rng.standard_normal((3001, f)) * 0.2).astype(np.float32)
-    dY = lib.DeviceFactors.from_host(ctx, Y)
-    G = lib.gramian(ctx, dY)
-    ref = Y.astype(np.float64).T @ Y.astype(np.float64)
-    assert G.shape == (f, f)
-    assert np.abs(G - ref).max() < 2e-6 * np.abs(ref).max()
-    dY.close()
 
 
 @pytest.mark.parametrize("f", [192, 260, 512])
