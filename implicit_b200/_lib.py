@@ -8,7 +8,7 @@ import os
 
 import numpy as np
 
-from . import _build
+from . import _build, utils
 
 ALS_OK = 0
 ALS_E_INVALID = -1
@@ -99,6 +99,12 @@ SIGNATURES = {
     "als_csr_concat_rows": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_i64, P(c_void_p)]),
     "als_comm_allreduce_i64": (c_int, [c_void_p, c_void_p, c_i64]),
     "als_comm_exchange_csr": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "als_csr_upload_device": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                                      c_i64, ctypes.c_uint64, P(c_void_p)]),
+    "als_factors_import_device": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, ctypes.c_uint64]),
+    "als_factors_export_device": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64]),
+    "als_device_alloc": (c_int, [c_void_p, c_i64, P(c_void_p)]),
+    "als_device_free": (c_int, [c_void_p, c_void_p]),
 }
 
 
@@ -436,6 +442,24 @@ class DeviceCSR:
         check(rc)
         return cls(ctx, h)
 
+    @classmethod
+    def from_device(cls, ctx, m):
+        """m: a CSR in CUDA memory (utils.is_device_csr: a CUDA torch.sparse_csr_tensor, or an object with shape and
+        indptr / indices / data exposing __cuda_array_interface__, like cupyx.scipy.sparse.csr_matrix), copied into a
+        device-resident CSR of the library (als_csr_upload_device) after the work its producer queued on the stream it
+        names.  Int32 / int64 indices and fp32 / fp64 values are narrowed on the device.  What als_csr_upload64 refuses,
+        and memory that is not on the context's device, raises ValueError."""
+        rows, cols, indptr, indices, data, owners = utils.device_csr_arrays(m)
+        stream = next(iter({a.stream for a in (indptr, indices, data) if a.stream}), 0)
+        h = c_void_p()
+        rc = ctx.lib.als_csr_upload_device(ctx.h, rows, cols, len(indices), indptr.ptr, indptr.itemsize, indices.ptr or None,
+                                           indices.itemsize, data.ptr or None, data.itemsize, 0, stream, ctypes.byref(h))
+        del owners  # the call has read the arrays
+        if rc == ALS_E_INVALID:
+            raise ValueError(ctx.lib.als_last_error().decode("utf-8", "replace"))
+        check(rc)
+        return cls(ctx, h)
+
     def column_counts(self):
         """int64 entries per column."""
         counts = np.zeros(self.shape3[1], dtype=np.int64)
@@ -560,6 +584,27 @@ class DeviceFactors:
         assert a.ndim == 2 and a.shape[1] == self.factors
         check(self.ctx.lib.als_factors_upload(self.ctx.h, self.h, ptr(a), int(row0), a.shape[0]))
 
+    @classmethod
+    def from_cuda(cls, ctx, obj, what="factors"):
+        """A new matrix filled device to device from a CUDA float32 2-D array (__cuda_array_interface__; rows may be
+        strided, like t[:, :f] of a wider tensor), after the work its producer queued on the stream it names.  ValueError
+        for what utils.parse_cai refuses and for memory that is not on the context's device."""
+        a = utils.cuda_array(obj, what, ("<f4",), 2)
+        f = cls(ctx, a.shape[0], a.shape[1])
+        try:
+            rc = ctx.lib.als_factors_import_device(ctx.h, f.h, a.ptr or None, a.ld, 0, a.shape[0], a.stream)
+            if rc == ALS_E_INVALID:
+                raise ValueError(ctx.lib.als_last_error().decode("utf-8", "replace"))
+            check(rc)
+        except BaseException:
+            f.close()
+            raise
+        return f
+
+    def snapshot(self):
+        """A DeviceSnapshot: a copy of this matrix in device memory of its own."""
+        return DeviceSnapshot(self)
+
     def fill_uniform(self, seed, scale):
         """factors = scale * U[0,1) generated on the device (the distribution of implicit/cpu/als.py:144-147)."""
         check(self.ctx.lib.als_factors_fill_uniform(self.ctx.h, self.h, int(seed), float(scale)))
@@ -584,6 +629,43 @@ class DeviceFactors:
         try:
             self.close()
         except Exception:
+            pass
+
+
+class DeviceSnapshot:
+    """A copy of a DeviceFactors matrix in device memory the library allocated for it alone, complete when it is made,
+    exposed through __cuda_array_interface__ version 3: shape (rows, factors), row stride the padded width (byte strides
+    (4 ld, 4)), '<f4', no stream to wait for.  torch.as_tensor(s, device="cuda") and cupy.asarray(s) keep the object,
+    and so its memory, alive; the memory is freed (cudaFree, after every stream's work) when the last reference dies.
+    Later changes of the matrix do not reach it."""
+
+    def __init__(self, factors):
+        ctx = factors.ctx
+        rows, f, ld = c_i64(), c_int(), c_int()
+        check(ctx.lib.als_factors_shape(factors.h, ctypes.byref(rows), ctypes.byref(f), ctypes.byref(ld)))
+        self.ctx, self.shape, self.ld = ctx, (rows.value, f.value), ld.value
+        self.ptr = c_void_p()
+        check(ctx.lib.als_device_alloc(ctx.h, 4 * self.ld * rows.value, ctypes.byref(self.ptr)))
+        try:
+            check(ctx.lib.als_factors_export_device(ctx.h, factors.h, self.ptr, self.ld, 0, rows.value))
+        except BaseException:
+            self.close()
+            raise
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": self.shape, "strides": (4 * self.ld, 4), "typestr": "<f4", "data": (self.ptr.value, False),
+                "version": 3, "stream": None}
+
+    def close(self):
+        if getattr(self, "ptr", None) and getattr(self.ctx, "h", None):
+            self.ctx.lib.als_device_free(self.ctx.h, self.ptr)
+        self.ptr = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # interpreter shutdown
             pass
 
 

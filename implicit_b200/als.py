@@ -17,7 +17,7 @@ from scipy.sparse import csr_matrix
 from . import _lib
 from .distributed import RowBlock
 from .utils import (BLOCK_FIELDS, ModelFitError, block_cuts, check_block_table, check_csr, check_random_state,
-                    column_splits, nnz_balanced_splits, splits_from_cuts)
+                    column_splits, is_device_csr, nnz_balanced_splits, splits_from_cuts)
 
 log = logging.getLogger("implicit")
 
@@ -117,6 +117,21 @@ class AlternatingLeastSquares:
     Parameters mirror implicit/als.py:7-19.  ``use_gpu`` must stay True and ``dtype`` float32: this
     package has no CPU path and computes in fp32.  New: ``device`` (CUDA ordinal) and
     ``process_group`` (implicit_b200.distributed.ProcessGroup) for row-sharded multi-GPU fits.
+
+    Inputs in CUDA memory: ``fit``, ``recommend`` (its liked filter and ``recalculate_user``), ``recalculate_*`` and
+    ``partial_fit_*`` also take a CSR whose arrays live on the model's device -- a CUDA ``torch.sparse_csr_tensor``, or any
+    object with ``shape`` and ``indptr`` / ``indices`` / ``data`` exposing ``__cuda_array_interface__`` (versions 2 and 3,
+    e.g. ``cupyx.scipy.sparse.csr_matrix``).  It is copied on the device into arrays the library owns (never aliased),
+    with int32 / int64 indices and float32 / float64 values, and gives bitwise the results of the same scipy CSR of
+    float32 values, entry for entry.  (A scipy CSR of other values is cast with ``astype``, which also merges its
+    duplicates and sorts its rows; a device CSR keeps its entries as they are.  In ``recalculate_*`` a device CSR is
+    scaled by ``alpha`` after the cast, a scipy one before it.)  ``user_factors`` /
+    ``item_factors`` take CUDA float32 2-D arrays too (rows may be strided), copied device to device; the numpy getters
+    download them lazily.  ``user_factors_device`` / ``item_factors_device`` hand out device snapshots of the factors.
+    Not covered, and refused with ValueError: device CSRs on a process group of several ranks (RowBlocks of device
+    arrays included), ``recommend(..., items=...)`` with a device liked filter, a device liked filter of 2^31 - 1 or
+    more nonzeros, and ``evaluation`` with device CSRs; DLPack is not read, and ``recommend`` returns numpy ids and
+    scores.
     """
 
     def __init__(
@@ -197,6 +212,9 @@ class AlternatingLeastSquares:
         return host
 
     def _set_host(self, side, value):
+        if value is not None and not isinstance(value, np.ndarray) and hasattr(value, "__cuda_array_interface__"):
+            self._set_device(side, value)
+            return
         if value is not None:
             value = np.ascontiguousarray(value, dtype=np.float32)
         if side == "user":
@@ -206,8 +224,41 @@ class AlternatingLeastSquares:
         self._host_fresh[side] = True
         self._dev_fresh[side] = False
 
+    def _set_device(self, side, value):
+        """Assignment of a CUDA float32 2-D array: the device replica is filled device to device and the host copy is
+        stale until a getter downloads it."""
+        d = _lib.DeviceFactors.from_cuda(self.ctx, value, f"{side}_factors")
+        if self._dev[side] is not None:
+            self._dev[side].close()
+        self._dev[side] = d
+        if side == "user":
+            self._user_factors, self._user_norms, self._XtX = None, None, None
+        else:
+            self._item_factors, self._item_norms, self._YtY = None, None, None
+        self._dev_fresh[side] = True
+        self._host_fresh[side] = False
+
+    def _factors_shape(self, side):
+        """The shape of one side's factors, from whichever copy is current (None: not set); downloads nothing."""
+        if not self._host_fresh[side] and self._dev[side] is not None:
+            return self._dev[side].rows, self._dev[side].factors
+        host = self._user_factors if side == "user" else self._item_factors
+        return None if host is None else host.shape
+
     user_factors = property(lambda self: self._get_host("user"), lambda self, v: self._set_host("user", v))
     item_factors = property(lambda self: self._get_host("item"), lambda self, v: self._set_host("item", v))
+
+    @property
+    def user_factors_device(self):
+        """A snapshot of the user factors in device memory of its own, exposing __cuda_array_interface__ version 3:
+        shape (users, factors), byte strides (4 ld, 4) with ld the padded width, '<f4'.  torch.as_tensor(...,
+        device="cuda") or cupy.asarray(...) keep it alive; a later fit or assignment does not change it."""
+        return self._device_factors("user").snapshot()
+
+    @property
+    def item_factors_device(self):
+        """The item factors' snapshot, like user_factors_device."""
+        return self._device_factors("item").snapshot()
 
     def _device_factors(self, side):
         """Device replica of one side, uploaded if the host copy is newer."""
@@ -235,12 +286,17 @@ class AlternatingLeastSquares:
 
     # ------------------------------------------------------------------ fit (implicit/cpu/als.py:98-202)
     def fit(self, user_items, show_progress=True, callback=None):
-        """Factorizes the user_items matrix (CSR, users x items, values = confidence).  On a process group of several
-        ranks, each rank may instead pass only its own rows, as a distributed.RowBlock."""
+        """Factorizes the user_items matrix (CSR, users x items, values = confidence; scipy, or in CUDA memory on one
+        GPU).  On a process group of several ranks, each rank may instead pass only its own rows, as a
+        distributed.RowBlock."""
         random_state = check_random_state(self.random_state)
         pg = self.process_group
         from_blocks = isinstance(user_items, RowBlock) and pg is not None and pg.world > 1
-        if from_blocks:
+        from_device = not isinstance(user_items, RowBlock) and is_device_csr(user_items)
+        if from_device and pg is not None and pg.world > 1:
+            raise ValueError("a CSR in CUDA memory is fitted on one GPU; on a process group of several ranks pass a "
+                             "scipy CSR or RowBlocks of scipy CSRs")
+        if from_blocks or from_device:
             Cui_host = None
         elif isinstance(user_items, RowBlock):
             Cui_host = user_items.whole()  # one rank: the block must be the whole matrix
@@ -259,6 +315,15 @@ class AlternatingLeastSquares:
         elif pg is not None and pg.world > 1:
             users, items, nnz = *Cui_host.shape, Cui_host.nnz
             Cui_s, Ciu_s, usplit, isplit = self._ingest_shards(Cui_host, row_cost)
+        elif from_device:
+            # copied on the device into the library's arrays and always device-resident (the host_csr rule is for
+            # host arrays); the same layout, so bitwise the factors of the same scipy CSR
+            Cui_s = _lib.DeviceCSR.from_device(ctx, user_items)
+            users, items, nnz = Cui_s.shape3
+            if self.alpha != 1.0:
+                Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
+            Ciu_s = Cui_s.transpose()
+            usplit = isplit = None
         else:
             users, items, nnz = *Cui_host.shape, Cui_host.nnz
             # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a
@@ -277,16 +342,16 @@ class AlternatingLeastSquares:
 
         # cpu/als.py:144-147: pre-set factors are kept, otherwise rng.random(...) * 0.01
         if self.process_group is not None and self.process_group.world > 1 and \
-                (self._get_host("user") is None or self._get_host("item") is None):
+                (self._factors_shape("user") is None or self._factors_shape("item") is None):
             # every rank must start from the same replicas: rank 0 draws a seed, everyone initialises from it
             seed = int(random_state.integers(1, 2**31 - 1)) if self.process_group.rank == 0 else 0
             seed = int(ctx.allreduce([float(seed)], "max")[0])
             random_state = np.random.default_rng(seed)
-        if self._get_host("user") is None:
+        if self._factors_shape("user") is None:
             self._set_host("user", random_state.random((users, self.factors), dtype=np.float32) * np.float32(0.01))
-        if self._get_host("item") is None:
+        if self._factors_shape("item") is None:
             self._set_host("item", random_state.random((items, self.factors), dtype=np.float32) * np.float32(0.01))
-        if self._user_factors.shape != (users, self.factors) or self._item_factors.shape != (items, self.factors):
+        if self._factors_shape("user") != (users, self.factors) or self._factors_shape("item") != (items, self.factors):
             raise ValueError("pre-set factors do not match the shape of user_items / the factors parameter")
         X = self._device_factors("user")
         Y = self._device_factors("item")
@@ -498,16 +563,24 @@ class AlternatingLeastSquares:
 
     # ------------------------------------------------------------------ recalculate / partial fit
     def _recalculate(self, ids, matrix, other_side, gram):
-        """implicit/cpu/als.py:204-265: Cholesky on purpose, with the cached Gramian of the other side."""
-        matrix = check_csr(matrix)
+        """implicit/cpu/als.py:204-265: Cholesky on purpose, with the cached Gramian of the other side.  A device CSR is
+        scaled by alpha on the device, after its values are cast to float32."""
+        device = is_device_csr(matrix)
+        if not device:
+            matrix = check_csr(matrix)
         n = 1 if np.isscalar(ids) else len(ids)
         if matrix.shape[0] != n:
             raise ValueError("user_items should have one row for every item in user")
-        if self.alpha != 1.0:
+        if self.alpha != 1.0 and not device:
             matrix = self.alpha * matrix
         ctx = self.ctx
         Y = self._device_factors(other_side)
-        C = _lib.DeviceCSR.upload(ctx, matrix.astype(np.float32))
+        if device:
+            C = _lib.DeviceCSR.from_device(ctx, matrix)
+            if self.alpha != 1.0:
+                C.scale(self.alpha)
+        else:
+            C = _lib.DeviceCSR.upload(ctx, matrix.astype(np.float32))
         out = _lib.DeviceFactors(ctx, n, self.factors)
         try:
             _lib.least_squares_with_gramian(ctx, gram, C, out, Y, self.regularization)
@@ -565,8 +638,9 @@ class AlternatingLeastSquares:
     # ------------------------------------------------------------------ recommend (cpu/matrix_factorization_base.py:35-96)
     def recommend(self, userid, user_items, N=10, filter_already_liked_items=True, filter_items=None,
                   recalculate_user=False, items=None):
+        device = is_device_csr(user_items)
         if filter_already_liked_items or recalculate_user:
-            if not isinstance(user_items, csr_matrix):
+            if not isinstance(user_items, csr_matrix) and not device:
                 raise ValueError("user_items needs to be a CSR sparse matrix")
             user_count = 1 if np.isscalar(userid) else len(userid)
             if user_items.shape[0] != user_count:
@@ -602,7 +676,15 @@ class AlternatingLeastSquares:
 
             fq = None
             batches = [(0, n_query)]
-            if filter_already_liked_items:
+            if filter_already_liked_items and device:
+                if items is not None:
+                    raise ValueError("recommend(..., items=...) filters liked items of a scipy CSR only, not of a CSR in "
+                                     "CUDA memory")
+                fq = _lib.DeviceCSR.from_device(ctx, user_items)  # unsorted rows are sorted on the device
+                tmp.append(fq)
+                if fq.shape3[2] > _LIKED_NNZ_MAX:
+                    raise ValueError(f"a liked filter in CUDA memory holds at most {_LIKED_NNZ_MAX} nonzeros")
+            elif filter_already_liked_items:
                 fq = user_items
                 if items is not None:
                     fq = _filter_items_from_sparse_matrix(items, fq)
@@ -623,7 +705,9 @@ class AlternatingLeastSquares:
                 if len(batches) > 1:
                     qr = query_rows[b0:b1] if query_rows is not None else np.arange(b0, b1)
                 liked = None
-                if fq is not None:
+                if device and fq is not None:
+                    liked = fq
+                elif fq is not None:
                     liked = _lib.DeviceCSR.upload(ctx, fq if len(batches) == 1 else fq[b0:b1])
                     tmp.append(liked)
                 parts.append(_lib.topk(ctx, item_handle, queries, int(N), query_rows=qr, n_query=b1 - b0,

@@ -657,31 +657,89 @@ ALS_API int als_host_free(void *ptr) {
   return ALS_OK;
 }
 
+// ---- device memory of the caller ------------------------------------------------------------------
+// ALS_E_INVALID unless p is device memory of ctx's device, or managed memory
+static int require_device_memory(als_ctx *ctx, const char *who, const char *what, const void *p) {
+  cudaPointerAttributes at;
+  const cudaError_t e = cudaPointerGetAttributes(&at, p);
+  cudaGetLastError();  // an unregistered host pointer may leave an error behind on older drivers
+  if (e == cudaSuccess && at.type == cudaMemoryTypeManaged) return ALS_OK;
+  if (e == cudaSuccess && at.type == cudaMemoryTypeDevice && at.device == ctx->device) return ALS_OK;
+  if (e == cudaSuccess && at.type == cudaMemoryTypeDevice)
+    set_error("%s: %s is memory of device %d, not of the context's device %d", who, what, at.device, ctx->device);
+  else
+    set_error("%s: %s is not device memory (a host pointer, or no CUDA allocation)", who, what);
+  return ALS_E_INVALID;
+}
+
+// ctx->stream continues after the work queued so far on the caller's stream (0: none)
+static int wait_for_producer(als_ctx *ctx, uint64_t producer_stream) {
+  if (!producer_stream) return ALS_OK;
+  cudaEvent_t ev;
+  ALS_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  cudaError_t e = cudaEventRecord(ev, (cudaStream_t)(uintptr_t)producer_stream);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev, 0);
+  cudaEventDestroy(ev);  // released once the wait has been satisfied
+  return e == cudaSuccess ? ALS_OK : cuda_fail(e, "ordering after the producer stream", __FILE__, __LINE__);
+}
+
 // ---- CSR ---------------------------------------------------------------------------------------
-// The one builder behind the three uploads: the checks, the rebase of a row shard (indptr[0] != 0), the arrays of the
-// residency, the copies and the layout.  An int32 indptr is als_csr_upload's: int32 limits on nnz too, and its int32
+// Where the arrays of an upload are: host memory (indptr of 4 bytes per entry for als_csr_upload, 8 for the 64-bit
+// entries; fp32 values) or, for als_csr_upload_device, device memory of any of the widths it takes.
+struct CsrArrays {
+  const void *indptr;
+  int indptr_bytes;
+  const void *indices;
+  int index_bytes;
+  const void *data;
+  int data_bytes;
+  bool device;
+};
+
+// The one builder behind the four uploads: the checks, the rebase of a row shard (indptr[0] != 0), the arrays of the
+// residency, the copies and the layout.  A host int32 indptr is als_csr_upload's: int32 limits on nnz too, and its int32
 // indices are copied as they are; the 64-bit entries narrow the indices while they are staged and refuse any outside
-// [0, cols).
-template <typename IP>
-static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const IP *indptr,
-                     const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  constexpr bool int32_entry = sizeof(IP) == sizeof(int32_t);
-  ALS_REQUIRE(ctx && out && indptr, "%s: NULL argument", who);
-  ALS_REQUIRE(index_bytes == 4 || index_bytes == 8, "%s: index_bytes must be 4 or 8, got %d", who, index_bytes);
+// [0, cols).  Device arrays are read by device kernels instead of the staging threads: the indptr comes to the host
+// (8 bytes per row, for the layout), the indices and values never do; the checks and their messages are the same.
+static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz,
+                     const CsrArrays &a, int64_t row_offset, als_csr **out) {
+  const bool int32_entry = !a.device && a.indptr_bytes == 4;
+  ALS_REQUIRE(ctx && out && a.indptr, "%s: NULL argument", who);
+  ALS_REQUIRE(a.index_bytes == 4 || a.index_bytes == 8, "%s: index_bytes must be 4 or 8, got %d", who, a.index_bytes);
+  ALS_REQUIRE(a.indptr_bytes == 4 || a.indptr_bytes == 8, "%s: indptr_bytes must be 4 or 8, got %d", who, a.indptr_bytes);
+  ALS_REQUIRE(a.data_bytes == 4 || a.data_bytes == 8, "%s: data_bytes must be 4 or 8, got %d", who, a.data_bytes);
   ALS_REQUIRE(rows >= 0 && cols >= 0 && nnz >= 0, "%s: negative shape", who);
   if (int32_entry)
     ALS_REQUIRE(nnz < (int64_t)INT32_MAX && rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX,
                 "%s: int32 CSR only (rows, cols, nnz < 2^31), like implicit/gpu/matrix.h:93-100", who);
   else
     ALS_REQUIRE(rows < (int64_t)INT32_MAX && cols < (int64_t)INT32_MAX, "%s: rows and cols must be < 2^31 - 1", who);
-  const int64_t base = indptr[0];
-  ALS_REQUIRE(base >= 0 && (int64_t)indptr[rows] - base == nnz, "%s: indptr[rows] - indptr[0] = %lld != nnz = %lld", who,
-              (long long)((int64_t)indptr[rows] - base), (long long)nnz);
-  ALS_REQUIRE(nnz == 0 || (indices && data), "%s: indices/data NULL with nnz > 0", who);
-  std::vector<int64_t> ip((size_t)rows + 1);
-  for (int64_t r = 0; r <= rows; ++r) ip[r] = (int64_t)indptr[r] - base;
-  for (int64_t r = 0; r < rows; ++r)
-    ALS_REQUIRE(ip[r + 1] >= ip[r], "%s: indptr is not monotone at row %lld", who, (long long)r);
+  std::vector<int64_t> ip;
+  int64_t base = 0, bad_row = -1;
+  if (a.device) {
+    ALS_CUDA(cudaSetDevice(ctx->device));
+    int rc = require_device_memory(ctx, who, "indptr", a.indptr);
+    if (rc == ALS_OK && nnz > 0 && a.indices) rc = require_device_memory(ctx, who, "indices", a.indices);
+    if (rc == ALS_OK && nnz > 0 && a.data) rc = require_device_memory(ctx, who, "data", a.data);
+    if (rc == ALS_OK) rc = device_indptr(ctx, a.indptr, a.indptr_bytes, rows, ip, &base, &bad_row);
+    if (rc != ALS_OK) return rc;
+  } else {
+    auto at = [&](int64_t r) -> int64_t {
+      return a.indptr_bytes == 8 ? ((const int64_t *)a.indptr)[r] : ((const int32_t *)a.indptr)[r];
+    };
+    base = at(0);
+    ip.resize((size_t)rows + 1);
+    for (int64_t r = 0; r <= rows; ++r) ip[r] = at(r) - base;
+    for (int64_t r = 0; r < rows && bad_row < 0; ++r)
+      if (ip[r + 1] < ip[r]) bad_row = r;
+  }
+  ALS_REQUIRE(base >= 0 && ip[rows] == nnz, "%s: indptr[rows] - indptr[0] = %lld != nnz = %lld", who, (long long)ip[rows],
+              (long long)nnz);
+  // device arrays are taken whole: nnz is their length, so a positive indptr[0] would read past their end
+  ALS_REQUIRE(!a.device || base == 0, "%s: indptr[0] = %lld, not 0: device arrays hold the matrix from its first entry",
+              who, (long long)base);
+  ALS_REQUIRE(nnz == 0 || (a.indices && a.data), "%s: indices/data NULL with nnz > 0", who);
+  ALS_REQUIRE(bad_row < 0, "%s: indptr is not monotone at row %lld", who, (long long)bad_row);
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
   als_csr *c = new als_csr();
@@ -691,20 +749,31 @@ static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int
   c->nnz = nnz;
   c->row_offset = row_offset;
   c->host = host;
-  const char *ix = (const char *)indices + base * index_bytes;
+  const char *ix = (const char *)a.indices + base * a.index_bytes;
+  const char *dv = (const char *)a.data + base * a.data_bytes;
   int64_t bad = -1;
   int rc = csr_alloc(ctx, c);
-  if (rc == ALS_OK)
+  if (rc == ALS_OK && a.device) {
+    rc = device_entries(ctx, c, ix, a.index_bytes, dv, a.data_bytes, &bad);
+  } else if (rc == ALS_OK) {
+    const float *data = (const float *)dv;
     rc = int32_entry ? h2d_copy(ctx, c->indices, ix, sizeof(int32_t) * nnz)
-                     : h2d_indices(ctx, c->indices, ix, index_bytes, nnz, cols, &bad, host);
-  if (rc == ALS_OK)
-    rc = host ? fill_host_values(ctx, c, c->data, nnz,
-                                 [&](float *v, int64_t i0, int64_t m) { memcpy(v, data + base + i0, sizeof(float) * m); })
-              : h2d_copy(ctx, c->data, data + base, sizeof(float) * nnz);
+                     : h2d_indices(ctx, c->indices, ix, a.index_bytes, nnz, cols, &bad, host);
+    if (rc == ALS_OK)
+      rc = host ? fill_host_values(ctx, c, c->data, nnz,
+                                   [&](float *v, int64_t i0, int64_t m) { memcpy(v, data + i0, sizeof(float) * m); })
+                : h2d_copy(ctx, c->data, data, sizeof(float) * nnz);
+  }
   if (rc == ALS_OK) rc = csr_layout(ctx, c, ip.data());
   if (rc != ALS_OK) {
     if (bad >= 0) {
-      const int64_t v = index_bytes == 8 ? ((const int64_t *)indices)[base + bad] : ((const int32_t *)indices)[base + bad];
+      int64_t v = 0;
+      if (a.device) {
+        if (cudaMemcpy(&v, ix + bad * a.index_bytes, a.index_bytes, cudaMemcpyDeviceToHost) != cudaSuccess) cudaGetLastError();
+        if (a.index_bytes == 4) v = (int32_t)v;  // little-endian: the low half
+      } else {
+        v = a.index_bytes == 8 ? ((const int64_t *)ix)[bad] : ((const int32_t *)ix)[bad];
+      }
       set_error("%s: indices[%lld] = %lld is outside [0, %lld)", who, (long long)(base + bad), (long long)v, (long long)cols);
     }
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -717,18 +786,32 @@ static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int
 
 ALS_API int als_csr_upload(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int32_t *indptr,
                            const int32_t *indices, const float *data, int64_t row_offset, als_csr **out) {
-  return csr_build("als_csr_upload", false, ctx, rows, cols, nnz, indptr, indices, 4, data, row_offset, out);
+  return csr_build("als_csr_upload", false, ctx, rows, cols, nnz, CsrArrays{indptr, 4, indices, 4, data, 4, false},
+                   row_offset, out);
 }
 
 // als_csr_upload_host64 keeps indices / data in page-locked host memory (always segmented) instead of uploading them
 ALS_API int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                              const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  return csr_build("als_csr_upload64", false, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+  return csr_build("als_csr_upload64", false, ctx, rows, cols, nnz,
+                   CsrArrays{indptr, 8, indices, index_bytes, data, 4, false}, row_offset, out);
 }
 
 ALS_API int als_csr_upload_host64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                                   const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out) {
-  return csr_build("als_csr_upload_host64", true, ctx, rows, cols, nnz, indptr, indices, index_bytes, data, row_offset, out);
+  return csr_build("als_csr_upload_host64", true, ctx, rows, cols, nnz,
+                   CsrArrays{indptr, 8, indices, index_bytes, data, 4, false}, row_offset, out);
+}
+
+ALS_API int als_csr_upload_device(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const void *indptr,
+                                  int indptr_bytes, const void *indices, int index_bytes, const void *data, int data_bytes,
+                                  int64_t row_offset, uint64_t producer_stream, als_csr **out) {
+  ALS_REQUIRE(ctx && out, "als_csr_upload_device: NULL argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const int rc = wait_for_producer(ctx, producer_stream);
+  if (rc != ALS_OK) return rc;
+  return csr_build("als_csr_upload_device", false, ctx, rows, cols, nnz,
+                   CsrArrays{indptr, indptr_bytes, indices, index_bytes, data, data_bytes, true}, row_offset, out);
 }
 
 ALS_API int als_csr_is_host(const als_csr *csr, int *host) {
@@ -1033,6 +1116,59 @@ ALS_API int als_factors_download(als_ctx *ctx, const als_factors *f, float *host
                                sizeof(float) * f->f, nrows, cudaMemcpyDeviceToHost, ctx->stream));
   }
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_factors_import_device(als_ctx *ctx, als_factors *f, const float *src, int64_t ld, int64_t row0,
+                                      int64_t nrows, uint64_t producer_stream) {
+  const char *who = "als_factors_import_device";
+  ALS_REQUIRE(ctx && f && (src || nrows == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(row0 >= 0 && nrows >= 0 && row0 + nrows <= f->rows, "%s: rows [%lld, %lld) out of range", who,
+              (long long)row0, (long long)(row0 + nrows));
+  ALS_REQUIRE(ld >= f->f, "%s: a row stride of %lld elements is shorter than a row of %d factors", who, (long long)ld, f->f);
+  if (nrows == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = require_device_memory(ctx, who, "src", src);
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc != ALS_OK) return rc;
+  float *dst = f->d + row0 * f->ld;
+  ALS_CUDA(cudaMemcpy2DAsync(dst, sizeof(float) * f->ld, src, sizeof(float) * ld, sizeof(float) * f->f, nrows,
+                             cudaMemcpyDeviceToDevice, ctx->stream));
+  if (f->ld > f->f)  // the padding columns read as zeros, as after als_factors_upload
+    ALS_CUDA(cudaMemset2DAsync(dst + f->f, sizeof(float) * f->ld, 0, sizeof(float) * (f->ld - f->f), nrows, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller may free or refill src once this returns
+  return ALS_OK;
+}
+
+ALS_API int als_factors_export_device(als_ctx *ctx, const als_factors *f, float *dst, int64_t ld, int64_t row0,
+                                      int64_t nrows) {
+  const char *who = "als_factors_export_device";
+  ALS_REQUIRE(ctx && f && (dst || nrows == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(row0 >= 0 && nrows >= 0 && row0 + nrows <= f->rows, "%s: rows [%lld, %lld) out of range", who,
+              (long long)row0, (long long)(row0 + nrows));
+  ALS_REQUIRE(ld >= f->f, "%s: a row stride of %lld elements is shorter than a row of %d factors", who, (long long)ld, f->f);
+  if (nrows == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const int rc = require_device_memory(ctx, who, "dst", dst);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpy2DAsync(dst, sizeof(float) * ld, f->d + row0 * f->ld, sizeof(float) * f->ld, sizeof(float) * f->f,
+                             nrows, cudaMemcpyDeviceToDevice, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // complete when this returns: any stream may read dst
+  return ALS_OK;
+}
+
+ALS_API int als_device_alloc(als_ctx *ctx, int64_t bytes, void **ptr) {
+  ALS_REQUIRE(ctx && ptr && bytes >= 0, "als_device_alloc: bad argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  ALS_CUDA(cudaMalloc(ptr, (size_t)std::max<int64_t>(bytes, 16)));
+  return ALS_OK;
+}
+
+ALS_API int als_device_free(als_ctx *ctx, void *ptr) {
+  ALS_REQUIRE(ctx, "als_device_free: ctx is NULL");
+  if (!ptr) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  ALS_CUDA(cudaFree(ptr));
   return ALS_OK;
 }
 

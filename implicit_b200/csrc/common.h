@@ -264,6 +264,16 @@ int csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t c
 int set_host_wmax(als_ctx *ctx, als_csr *c, unsigned wmax_bits, bool neg);
 // the same range folded over n values on the host
 void host_wmax(const float *v, int64_t n, unsigned *wmax_bits, bool *neg);
+// The device source of an upload (als_csr_upload_device), on ctx->stream.  device_indptr: the caller's device indptr
+// (4 or 8 bytes per entry) rebased to its first entry, copied to ip[0 .. rows] on the host (8 bytes per row), with
+// *base = indptr[0] and *bad_row the first row r with indptr[r + 1] < indptr[r] (else -1); synchronises.
+// device_entries: c->nnz indices (4 or 8 bytes, from the first nonzero) narrowed to int32 into c->indices and values
+// (fp32 or fp64) cast to fp32 into c->data; an index outside [0, c->cols) sets *bad_at to the first such position and
+// returns ALS_E_INVALID.  Synchronises: the caller's arrays have been read when it returns.
+int device_indptr(als_ctx *ctx, const void *indptr, int indptr_bytes, int64_t rows, std::vector<int64_t> &ip,
+                  int64_t *base, int64_t *bad_row);
+int device_entries(als_ctx *ctx, als_csr *c, const void *indices, int index_bytes, const void *data, int data_bytes,
+                   int64_t *bad_at);
 // synthetic inputs generated on the device (gen.cu)
 int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t nnz_target, uint64_t seed, als_csr **out);
 int factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale);

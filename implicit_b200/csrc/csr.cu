@@ -300,7 +300,108 @@ __global__ void concat_indptr_kernel(const int32_t *__restrict__ ip, int64_t row
   for (; r <= rows; r += (int64_t)gridDim.x * blockDim.x) out[r] = out_base + (ip[r] - f);
 }
 
+// ---- the device source of the one upload path (api.cu csr_build, als_csr_upload_device) ---------------------------
+// flags[0]: indptr[0]; flags[1]: the first row r with indptr[r + 1] < indptr[r]; flags[2]: the first position (from
+// indptr[0]) of an index outside [0, cols).  Rows and positions are folded with atomicMin from all ones (none).
+template <typename T>
+__global__ void indptr_rebase_kernel(const T *__restrict__ indptr, int64_t rows, long long *__restrict__ ip,
+                                     unsigned long long *flags) {
+  int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const long long base = (long long)indptr[0];
+  if (r == 0) flags[0] = (unsigned long long)base;
+  for (; r <= rows; r += stride) {
+    const long long v = (long long)indptr[r];
+    ip[r] = v - base;
+    if (r < rows && (long long)indptr[r + 1] < v) atomicMin(flags + 1, (unsigned long long)r);
+  }
+}
+
+// indices of 4 or 8 bytes -> int32, with the range check of the host staging (h2d_indices)
+template <typename T>
+__global__ void narrow_indices_kernel(const T *__restrict__ in, int64_t n, int64_t cols, int32_t *__restrict__ out,
+                                      unsigned long long *flags) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) {
+    const long long v = (long long)in[i];
+    if ((unsigned long long)v >= (unsigned long long)cols) atomicMin(flags + 2, (unsigned long long)i);
+    out[i] = (int32_t)v;
+  }
+}
+
+// fp64 values -> fp32, rounded to nearest like numpy's astype(np.float32)
+__global__ void narrow_values_kernel(const double *__restrict__ in, int64_t n, float *__restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) out[i] = (float)in[i];
+}
+
 }  // namespace
+
+int device_indptr(als_ctx *ctx, const void *indptr, int indptr_bytes, int64_t rows, std::vector<int64_t> &ip,
+                  int64_t *base, int64_t *bad_row) {
+  long long *ip_dev = nullptr;
+  unsigned long long *flags = nullptr;
+  int rc = dev_alloc(ctx, (void **)&ip_dev, sizeof(long long) * (rows + 1));
+  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&flags, 3 * sizeof(unsigned long long));
+  if (rc != ALS_OK) {
+    dev_free(ctx, ip_dev);
+    return rc;
+  }
+  ALS_CUDA(cudaMemsetAsync(flags, 0xff, 3 * sizeof(unsigned long long), ctx->stream));
+  const int blocks = (int)std::min<int64_t>((rows + 256) / 256, (int64_t)ctx->sm_count * 8);
+  if (indptr_bytes == 8)
+    indptr_rebase_kernel<<<blocks, 256, 0, ctx->stream>>>((const long long *)indptr, rows, ip_dev, flags);
+  else
+    indptr_rebase_kernel<<<blocks, 256, 0, ctx->stream>>>((const int32_t *)indptr, rows, ip_dev, flags);
+  ALS_CUDA(cudaGetLastError());
+  ctx->launches++;
+  unsigned long long f[2];
+  ip.assign((size_t)rows + 1, 0);
+  ALS_CUDA(cudaMemcpyAsync(ip.data(), ip_dev, sizeof(int64_t) * (rows + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaMemcpyAsync(f, flags, sizeof(f), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  dev_free(ctx, ip_dev);
+  dev_free(ctx, flags);
+  *base = (int64_t)f[0];
+  *bad_row = f[1] == ~0ull ? -1 : (int64_t)f[1];
+  return ALS_OK;
+}
+
+int device_entries(als_ctx *ctx, als_csr *c, const void *indices, int index_bytes, const void *data, int data_bytes,
+                   int64_t *bad_at) {
+  *bad_at = -1;
+  const int64_t n = c->nnz;
+  if (n == 0) return ALS_OK;
+  unsigned long long *flags = nullptr;
+  int rc = dev_alloc(ctx, (void **)&flags, 3 * sizeof(unsigned long long));
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemsetAsync(flags, 0xff, 3 * sizeof(unsigned long long), ctx->stream));
+  const int blocks = ctx->sm_count * 8;
+  if (index_bytes == 8)
+    narrow_indices_kernel<<<blocks, 256, 0, ctx->stream>>>((const long long *)indices, n, c->cols, c->indices, flags);
+  else
+    narrow_indices_kernel<<<blocks, 256, 0, ctx->stream>>>((const int32_t *)indices, n, c->cols, c->indices, flags);
+  ALS_CUDA(cudaGetLastError());
+  ctx->launches++;
+  if (data_bytes == 8) {
+    narrow_values_kernel<<<blocks, 256, 0, ctx->stream>>>((const double *)data, n, c->data);
+    ALS_CUDA(cudaGetLastError());
+    ctx->launches++;
+  } else {
+    ALS_CUDA(cudaMemcpyAsync(c->data, data, sizeof(float) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  unsigned long long bad = 0;
+  ALS_CUDA(cudaMemcpyAsync(&bad, flags + 2, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller's arrays have been read
+  dev_free(ctx, flags);
+  if (bad != ~0ull) {
+    *bad_at = (int64_t)bad;
+    return ALS_E_INVALID;
+  }
+  return ALS_OK;
+}
 
 int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch, bool with_data) {
   const std::vector<const als_csr *> segs = segments_of(C);

@@ -18,7 +18,7 @@ import time
 import numpy as np
 
 from . import _lib
-from .utils import check_csr
+from .utils import check_csr, is_device_csr
 
 _MAGIC = b"ALSB200\x01"
 _PORT_OFFSETS = (1, 2, 3, 5, 8, 13, 21, 34)
@@ -127,7 +127,10 @@ class RowBlock:
         self.user_items, self.first_row, self.users = user_items, first_row, users
 
     def csr(self):
-        """The block as a float32 scipy CSR, after checking its own shape."""
+        """The block as a float32 scipy CSR, after checking its own shape.  A block of device arrays is refused
+        (ValueError): RowBlocks take scipy CSRs."""
+        if is_device_csr(self.user_items):
+            raise ValueError("a RowBlock takes a scipy CSR: a CSR in CUDA memory is fitted on one GPU only")
         m = check_csr(self.user_items)
         if m.dtype != np.float32:
             m = m.astype(np.float32)  # cpu/als.py:129-130

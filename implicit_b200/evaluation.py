@@ -19,13 +19,21 @@ the whole matrices.  Any other model with a ``recommend`` method goes through th
 reference's contract (every eligible user leaves exactly K entries in the test matrix, train + test == input, a
 reserved share of users stays train-only, the same ValueErrors).  The reference draws its shuffle from numpy's
 global generator there (:128), so the split itself is seeded here and is not bit-comparable.
+
+Every function here takes scipy CSRs (or RowBlocks of them); a CSR in CUDA memory is refused with ValueError.
 """
 import numpy as np
 from scipy.sparse import csr_matrix
 
 from .als import AlternatingLeastSquares, _Ingest
 from .distributed import RowBlock
-from .utils import BLOCK_FIELDS, check_block_table, check_random_state
+from .utils import BLOCK_FIELDS, check_block_table, check_random_state, is_device_csr
+
+def _host_only(*matrices):
+    """ValueError for a CSR in CUDA memory, which evaluation does not read."""
+    if any(is_device_csr(m) for m in matrices):
+        raise ValueError("evaluation takes scipy CSRs: a CSR in CUDA memory is not supported here")
+
 
 #: users per ``recommend`` call (the reference uses 1000, evaluation.pyx:417; any value gives the same sums)
 BATCH = 16384
@@ -36,6 +44,7 @@ def train_test_split(ratings, train_percentage=0.8, random_state=None):
 
     One uniform draw per stored entry, in COO order: ``< train_percentage`` goes to train.  Negative
     test entries are dropped (:44-45)."""
+    _host_only(ratings)
     ratings = ratings.tocoo()
     rng = check_random_state(random_state)
     draw = rng.random(len(ratings.data))
@@ -54,6 +63,7 @@ def leave_k_out_split(ratings, K=1, train_only_size=0.0, random_state=None):
     """'Leave K out': every eligible user (more than K + 1 stored entries, evaluation.pyx:191) gives K randomly
     chosen entries to the test matrix; `train_only_size` is the fraction of users kept out of the test set
     (:194-198).  Returns (train, test) CSR matrices of the input's shape with train + test == ratings."""
+    _host_only(ratings)
     if K < 1:
         raise ValueError("The 'K' must be >= 1.")
     if not 0.0 <= train_only_size < 1.0:
@@ -111,6 +121,7 @@ def ranking_metrics_at_k(model, train_user_items, test_user_items, K=10, show_pr
     ``test_user_items`` may be ``distributed.RowBlock``s of the same rows on each rank; without one, or on one
     rank, a RowBlock must hold every row.
     """
+    _host_only(train_user_items, test_user_items)
     if isinstance(model, AlternatingLeastSquares):
         return _device_ranking_metrics(model, train_user_items, test_user_items, int(K), show_progress)
     if isinstance(train_user_items, RowBlock):

@@ -29,6 +29,119 @@ def check_csr(user_items):
     return user_items
 
 
+class CudaArray:
+    """One array of device memory, read from its __cuda_array_interface__ (parse_cai): the address, the shape, the item
+    size, the row stride in elements (2-D) and the stream its producer queued it on (0: no ordering needed)."""
+
+    def __init__(self, ptr, shape, itemsize, ld, stream):
+        self.ptr, self.shape, self.itemsize, self.ld, self.stream = ptr, shape, itemsize, ld, stream
+
+    def __len__(self):
+        return self.shape[0]
+
+
+def parse_cai(cai, what, typestrs, ndim):
+    """The CudaArray a __cuda_array_interface__ dict (version 2 or 3) describes, or ValueError, before its pointer is used:
+    a version other than 2 or 3, a mask, a typestr outside `typestrs`, a shape of other than `ndim` dimensions, strides
+    other than contiguous (1-D) or row-strided with unit column stride (2-D), or a stream entry of 0, which the interface
+    forbids.  Version 3's stream (1: the legacy default stream, 2: the per-thread one, else a cudaStream_t) is the stream
+    to order after; an absent or None stream needs no ordering.  Version 2 cannot name a stream: its arrays are ordered
+    after the legacy default stream, where PyTorch and CuPy queue their work unless told otherwise."""
+    if not isinstance(cai, dict):
+        raise ValueError(f"{what}: __cuda_array_interface__ is not a dict")
+    version = cai.get("version")
+    if version not in (2, 3):
+        raise ValueError(f"{what}: __cuda_array_interface__ version {version!r} is not supported (2 or 3)")
+    if cai.get("mask") is not None:
+        raise ValueError(f"{what}: masked arrays are not supported")
+    typestr = cai.get("typestr")
+    if typestr not in typestrs:
+        raise ValueError(f"{what}: typestr {typestr!r} is not one of {', '.join(typestrs)}")
+    itemsize = int(typestr[2:])
+    shape = cai.get("shape")
+    if not isinstance(shape, tuple) or len(shape) != ndim or not all(isinstance(n, int) and n >= 0 for n in shape):
+        raise ValueError(f"{what}: shape {shape!r} is not a {ndim}-D shape")
+    strides = cai.get("strides")
+    ld = shape[-1] if ndim == 2 else 1
+    if strides is not None:
+        if not isinstance(strides, tuple) or len(strides) != ndim or not all(isinstance(s, int) for s in strides):
+            raise ValueError(f"{what}: strides {strides!r} do not match the shape {shape!r}")
+        if ndim == 1 and shape[0] > 1 and strides[0] != itemsize:
+            raise ValueError(f"{what}: a 1-D array of stride {strides[0]} bytes is not contiguous")
+        if ndim == 2:
+            if shape[1] > 1 and strides[1] != itemsize:
+                raise ValueError(f"{what}: column stride {strides[1]} bytes: the rows must be contiguous")
+            if shape[0] > 1 and (strides[0] % itemsize or strides[0] < shape[1] * itemsize):
+                raise ValueError(f"{what}: row stride {strides[0]} bytes is not a whole number of elements at least a row "
+                                 f"of {shape[1]} long")
+            if shape[0] > 1:
+                ld = strides[0] // itemsize
+    data = cai.get("data")
+    if not isinstance(data, tuple) or len(data) != 2 or not isinstance(data[0], int):
+        raise ValueError(f"{what}: data {data!r} is not a (pointer, read-only) pair")
+    if data[0] == 0 and all(shape):
+        raise ValueError(f"{what}: NULL pointer for a non-empty array")
+    if version == 2:
+        stream = 1
+    else:
+        stream = cai.get("stream")
+        if stream is None:
+            stream = 0
+        elif not isinstance(stream, int) or stream == 0:
+            raise ValueError(f"{what}: stream {stream!r} is not a stream (0 is forbidden; None means no ordering)")
+    return CudaArray(int(data[0]), shape, itemsize, ld, int(stream))
+
+
+def cuda_array(obj, what, typestrs, ndim):
+    """parse_cai of obj.__cuda_array_interface__; ValueError when obj has none (host memory)."""
+    cai = getattr(obj, "__cuda_array_interface__", None)
+    if cai is None:
+        raise ValueError(f"{what}: {type(obj).__name__} does not expose __cuda_array_interface__ (not CUDA memory)")
+    return parse_cai(cai, what, typestrs, ndim)
+
+
+def _is_torch_sparse_csr(m):
+    return str(getattr(m, "layout", "")) == "torch.sparse_csr" and callable(getattr(m, "crow_indices", None))
+
+
+def is_device_csr(m):
+    """A CSR whose arrays are in CUDA memory: a torch.sparse_csr_tensor (by its layout name), or any object with `shape`
+    and indptr / indices / data attributes that expose __cuda_array_interface__ (cupyx.scipy.sparse.csr_matrix)."""
+    if _is_torch_sparse_csr(m):
+        return True
+    return hasattr(m, "shape") and all(hasattr(getattr(m, a, None), "__cuda_array_interface__")
+                                       for a in ("indptr", "indices", "data"))
+
+
+INDEX_TYPESTRS = ("<i4", "<i8")
+VALUE_TYPESTRS = ("<f4", "<f8")
+
+
+def device_csr_arrays(m):
+    """(rows, cols, indptr, indices, data, owners) of a device CSR (is_device_csr): the three CudaArrays and the objects
+    that own their memory, to be held until the upload returns.  ValueError for what parse_cai refuses, for arrays whose
+    lengths do not fit the shape and for arrays that name different streams."""
+    if _is_torch_sparse_csr(m):
+        owners = (m.crow_indices(), m.col_indices(), m.values())
+    else:
+        owners = (m.indptr, m.indices, m.data)
+    shape = tuple(int(n) for n in m.shape)
+    if len(shape) != 2:
+        raise ValueError(f"a device CSR must be 2-D, got shape {shape}")
+    rows, cols = shape
+    indptr = cuda_array(owners[0], "indptr", INDEX_TYPESTRS, 1)
+    indices = cuda_array(owners[1], "indices", INDEX_TYPESTRS, 1)
+    data = cuda_array(owners[2], "data", VALUE_TYPESTRS, 1)
+    if len(indptr) != rows + 1:
+        raise ValueError(f"indptr has {len(indptr)} entries, the {rows} rows need {rows + 1}")
+    if len(indices) != len(data):
+        raise ValueError(f"indices has {len(indices)} entries and data {len(data)}")
+    streams = {a.stream for a in (indptr, indices, data) if a.stream}
+    if len(streams) > 1:
+        raise ValueError("the arrays of a device CSR name different streams")
+    return rows, cols, indptr, indices, data, owners
+
+
 def check_random_state(random_state):
     """implicit/utils.py:65-83: int / None / RandomState / Generator -> np.random.Generator."""
     if isinstance(random_state, np.random.RandomState):

@@ -119,6 +119,19 @@ int als_csr_upload64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, cons
  * als_csr_slice_rows and als_topk's `liked` refuse it (ALS_E_UNSUPPORTED). */
 int als_csr_upload_host64(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const int64_t *indptr,
                           const void *indices, int index_bytes, const float *data, int64_t row_offset, als_csr **out);
+/* The arguments and refusals of als_csr_upload64, with every array in device memory of the context's device (or managed
+ * memory): indptr of indptr_bytes = 4 or 8, indices of index_bytes = 4 or 8, values of data_bytes = 4 (fp32) or 8 (fp64,
+ * rounded to fp32).  The arrays are taken whole: indices / data hold exactly nnz entries and indptr[0] must be 0 (a row
+ * shard is rows of its own arrays, with row_offset its first row).  The copy is ordered after the work queued so far on producer_stream (a cudaStream_t as an integer;
+ * 0: none).  Device kernels narrow the indices and values into arrays the library owns, and check every index and the
+ * indptr; a refusal names the position als_csr_upload64 names for the same input, in the same words.  Only the indptr
+ * comes to the host (8 bytes per row, for the layout and the schedule).  The caller's memory is never aliased: it has been
+ * read when the call returns.  The CSR is device-resident and segmented above the segment cap like als_csr_upload64's.
+ * Refuses pointers that are not device memory of the context's device (ALS_E_INVALID).  (No reference equivalent; the
+ * reference's GPU Matrix wraps __cuda_array_interface__ memory, implicit/gpu/_cuda.pyx:97-103.) */
+int als_csr_upload_device(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz, const void *indptr, int indptr_bytes,
+                          const void *indices, int index_bytes, const void *data, int data_bytes, int64_t row_offset,
+                          uint64_t producer_stream, als_csr **out);
 /* *host = 1 for a host-resident CSR (als_csr_upload_host64 or its transpose), else 0. */
 int als_csr_is_host(const als_csr *csr, int *host);
 /* Number of row-block segments of the device layout (1 for a CSR within the segment cap). */
@@ -180,6 +193,18 @@ int als_factors_create(als_ctx *ctx, int64_t rows, int factors, als_factors **ou
 /* host[nrows, factors] (row-major, unpadded) <-> device rows [row0, row0 + nrows). */
 int als_factors_upload(als_ctx *ctx, als_factors *f, const float *host, int64_t row0, int64_t nrows);
 int als_factors_download(als_ctx *ctx, const als_factors *f, float *host, int64_t row0, int64_t nrows);
+/* Strided fp32 device memory <-> device rows [row0, row0 + nrows): row r of the caller's matrix starts ld >= factors
+ * elements after row r - 1 (so t[:, :factors] of a wider row-major matrix is taken as it is).  Import zeroes the padding
+ * columns [factors, stride) like als_factors_upload, after the work queued so far on producer_stream (0: none); export
+ * writes the factors columns only.  Both refuse memory that is not device memory of the context's device (managed memory
+ * is taken), and both synchronise: src has been read, and dst written, when they return. */
+int als_factors_import_device(als_ctx *ctx, als_factors *f, const float *src, int64_t ld, int64_t row0, int64_t nrows,
+                              uint64_t producer_stream);
+int als_factors_export_device(als_ctx *ctx, const als_factors *f, float *dst, int64_t ld, int64_t row0, int64_t nrows);
+/* Device memory of the context's device that the caller owns (the factor snapshots of the Python layer): cudaMalloc /
+ * cudaFree.  cudaFree waits for the device, so work of any stream that still reads the block finishes first. */
+int als_device_alloc(als_ctx *ctx, int64_t bytes, void **ptr);
+int als_device_free(als_ctx *ctx, void *ptr);
 int als_factors_shape(const als_factors *f, int64_t *rows, int *factors, int *stride);
 /* *has_nan = 1 if any element is NaN (device-side scan).  Replaces the host np.isnan pass of
  * RecommenderBase._check_factors, implicit/recommender_base.py:218-223. */
