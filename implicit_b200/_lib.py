@@ -105,6 +105,16 @@ SIGNATURES = {
     "als_factors_export_device": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64]),
     "als_device_alloc": (c_int, [c_void_p, c_i64, P(c_void_p)]),
     "als_device_free": (c_int, [c_void_p, c_void_p]),
+    "als_topk_into": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_int, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_int, c_i64, c_void_p, c_int, ctypes.c_uint64, c_void_p, c_void_p,
+                              P(c_int)]),
+    "als_factors_gather_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, P(c_void_p),
+                                        P(c_int)]),
+    "als_device_upload": (c_int, [c_void_p, c_void_p, c_void_p, c_i64]),
+    "als_device_download": (c_int, [c_void_p, c_void_p, c_void_p, c_i64]),
+    "als_factors_row_norms": (c_int, [c_void_p, c_void_p, c_f32, c_void_p]),
+    "als_ids_sort": (c_int, [c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, c_void_p]),
+    "als_csr_restrict_columns": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, P(c_void_p)]),
 }
 
 
@@ -460,6 +470,15 @@ class DeviceCSR:
         check(rc)
         return cls(ctx, h)
 
+    def restrict_columns(self, subset):
+        """The liked CSR remapped onto the positions of `subset` (a utils.CudaArray sorted ascending), the device
+        counterpart of als._filter_items_from_sparse_matrix (als_csr_restrict_columns)."""
+        h = c_void_p()
+        _check_input(self.ctx, self.ctx.lib.als_csr_restrict_columns(self.ctx.h, self.h, subset.ptr or None,
+                                                                     subset.itemsize, len(subset), subset.stream,
+                                                                     ctypes.byref(h)))
+        return DeviceCSR(self.ctx, h)
+
     def column_counts(self):
         """int64 entries per column."""
         counts = np.zeros(self.shape3[1], dtype=np.int64)
@@ -603,7 +622,29 @@ class DeviceFactors:
 
     def snapshot(self):
         """A DeviceSnapshot: a copy of this matrix in device memory of its own."""
-        return DeviceSnapshot(self)
+        return DeviceSnapshot.of_factors(self)
+
+    @classmethod
+    def gather_rows(cls, ctx, src, rows):
+        """A new matrix of the rows src[rows] (rows: a utils.CudaArray of int32 / int64 ids), after the work its producer
+        queued on the stream it names.  None when some id is outside [0, src.rows) (nothing is created); ValueError for
+        memory that is not on the context's device."""
+        h, bad = c_void_p(), c_int(0)
+        rc = ctx.lib.als_factors_gather_rows(ctx.h, src.h, rows.ptr or None, rows.itemsize, len(rows), rows.stream,
+                                             ctypes.byref(h), ctypes.byref(bad))
+        if bad.value:
+            return None
+        _check_input(ctx, rc)
+        f = cls.__new__(cls)
+        f.ctx, f.h, f.rows, f.factors = ctx, h, len(rows), src.factors
+        return f
+
+    def row_norms(self, zero_value=1e-10):
+        """A DeviceSnapshot [rows] '<f4' of the row norms, bitwise np.linalg.norm(F, axis=-1) with zeros written as
+        float32(zero_value) (the `n[n == 0] = 1e-10` of the user_norms / item_norms properties)."""
+        out = DeviceSnapshot(self.ctx, (self.rows,), "<f4")
+        check(self.ctx.lib.als_factors_row_norms(self.ctx.h, self.h, float(zero_value), out.ptr))
+        return out
 
     def fill_uniform(self, seed, scale):
         """factors = scale * U[0,1) generated on the device (the distribution of implicit/cpu/als.py:144-147)."""
@@ -633,28 +674,57 @@ class DeviceFactors:
 
 
 class DeviceSnapshot:
-    """A copy of a DeviceFactors matrix in device memory the library allocated for it alone, complete when it is made,
-    exposed through __cuda_array_interface__ version 3: shape (rows, factors), row stride the padded width (byte strides
-    (4 ld, 4)), '<f4', no stream to wait for.  torch.as_tensor(s, device="cuda") and cupy.asarray(s) keep the object,
-    and so its memory, alive; the memory is freed (cudaFree, after every stream's work) when the last reference dies.
-    Later changes of the matrix do not reach it."""
+    """A 1-D or 2-D array in device memory the library allocated for it alone (als_device_alloc), complete when it is
+    handed out, exposed through __cuda_array_interface__ version 3: `shape`, `typestr`, rows `ld` elements apart (2-D),
+    no stream to wait for.  The factor snapshots (of_factors) are '<f4' rows of the padded width; the outputs of the
+    device serving calls are contiguous ids and scores.  torch.as_tensor(s, device="cuda") and cupy.asarray(s) keep the
+    object, and so its memory, alive; the memory is freed (cudaFree, after every stream's work) when the last reference
+    dies, and outlives the model and the context object that made it."""
 
-    def __init__(self, factors):
+    def __init__(self, ctx, shape, typestr, ld=None):
+        self.ctx, self.shape, self.typestr = ctx, tuple(int(n) for n in shape), typestr
+        self.itemsize = int(typestr[2:])
+        self.ld = self.shape[-1] if ld is None else int(ld)
+        count = self.shape[0] * (self.ld if len(self.shape) == 2 else 1)
+        self.ptr = c_void_p()
+        check(ctx.lib.als_device_alloc(ctx.h, self.itemsize * count, ctypes.byref(self.ptr)))
+
+    @classmethod
+    def of_factors(cls, factors):
+        """A copy of a DeviceFactors matrix: shape (rows, factors), row stride the padded width."""
         ctx = factors.ctx
         rows, f, ld = c_i64(), c_int(), c_int()
         check(ctx.lib.als_factors_shape(factors.h, ctypes.byref(rows), ctypes.byref(f), ctypes.byref(ld)))
-        self.ctx, self.shape, self.ld = ctx, (rows.value, f.value), ld.value
-        self.ptr = c_void_p()
-        check(ctx.lib.als_device_alloc(ctx.h, 4 * self.ld * rows.value, ctypes.byref(self.ptr)))
+        s = cls(ctx, (rows.value, f.value), "<f4", ld.value)
         try:
-            check(ctx.lib.als_factors_export_device(ctx.h, factors.h, self.ptr, self.ld, 0, rows.value))
+            check(ctx.lib.als_factors_export_device(ctx.h, factors.h, s.ptr, s.ld, 0, rows.value))
         except BaseException:
-            self.close()
+            s.close()
             raise
+        return s
+
+    @classmethod
+    def from_host(cls, ctx, a):
+        """A 1-D copy of the contiguous numpy array a ('<i4', '<i8' or '<f4')."""
+        a = np.ascontiguousarray(a)
+        s = cls(ctx, a.shape, a.dtype.str)
+        try:
+            check(ctx.lib.als_device_upload(ctx.h, s.ptr, ptr(a) if a.size else None, a.nbytes))
+        except BaseException:
+            s.close()
+            raise
+        return s
+
+    def cuda(self, row0=0):
+        """This array from row `row0` on as a utils.CudaArray (no stream to wait for)."""
+        step = self.itemsize * (self.ld if len(self.shape) == 2 else 1)
+        return utils.CudaArray(self.ptr.value + step * row0, (self.shape[0] - row0,) + self.shape[1:], self.itemsize,
+                               self.ld, 0)
 
     @property
     def __cuda_array_interface__(self):
-        return {"shape": self.shape, "strides": (4 * self.ld, 4), "typestr": "<f4", "data": (self.ptr.value, False),
+        strides = (self.itemsize * self.ld, self.itemsize) if len(self.shape) == 2 else None
+        return {"shape": self.shape, "strides": strides, "typestr": self.typestr, "data": (self.ptr.value, False),
                 "version": 3, "stream": None}
 
     def close(self):
@@ -667,6 +737,31 @@ class DeviceSnapshot:
             self.close()
         except Exception:  # interpreter shutdown
             pass
+
+
+def _check_input(ctx, rc):
+    """check(), with ALS_E_INVALID (a refused argument) raised as ValueError."""
+    if rc == ALS_E_INVALID:
+        raise ValueError(ctx.lib.als_last_error().decode("utf-8", "replace"))
+    check(rc)
+
+
+def ids_download(ctx, ids):
+    """The utils.CudaArray ids as a numpy array of their width (int32 / int64)."""
+    out = np.empty(len(ids), dtype=np.int32 if ids.itemsize == 4 else np.int64)
+    _check_input(ctx, ctx.lib.als_device_download(ctx.h, ptr(out) if out.size else None, ids.ptr or None, out.nbytes))
+    return out
+
+
+def ids_sort(ctx, ids):
+    """A DeviceSnapshot of the utils.CudaArray ids sorted ascending on the device, of the same width."""
+    out = DeviceSnapshot(ctx, ids.shape, f"<i{ids.itemsize}")
+    try:
+        _check_input(ctx, ctx.lib.als_ids_sort(ctx.h, ids.ptr or None, ids.itemsize, len(ids), ids.stream, out.ptr))
+    except BaseException:
+        out.close()
+        raise
+    return out
 
 
 # ---- the native operator interface, named like the reference's (implicit/cpu/_als.pyx, topk.pyx) ----
@@ -773,6 +868,31 @@ def topk(ctx, items, queries, k, query_rows=None, n_query=None, item_norms=None,
                            liked.h if liked is not None else None, ptr(fl), 0 if fl is None else len(fl),
                            ptr(ids), ptr(scores)))
     return ids, scores
+
+
+def topk_into(ctx, items, queries, k, n_query, ids, scores, query_rows=None, query_row0=0, item_norms=None,
+              query_norms=None, liked=None, filter_items=None, id_map=None, stream=0):
+    """als_topk_into: the top-k of topk() written to the device arrays ids / scores (utils.CudaArrays of n_query rows of
+    k), every other id or norm array a utils.CudaArray too (query_rows None: rows [query_row0, query_row0 + n_query) of
+    queries).  Returns 0, or the bits of the device ids that were out of range (1: query_rows, 2: filter_items), in
+    which case nothing was written."""
+    def arr(a):
+        return (a.ptr or None, a.itemsize) if a is not None else (None, 4)
+
+    qr, qb = arr(query_rows)
+    fl, fb = arr(filter_items)
+    mp, mb = arr(id_map)
+    bad = c_int(0)
+    rc = ctx.lib.als_topk_into(ctx.h, items.h, queries.h, qr, qb, int(query_row0), int(n_query), int(k),
+                               item_norms.ptr if item_norms is not None else None,
+                               query_norms.ptr if query_norms is not None else None,
+                               liked.h if liked is not None else None, fl, fb,
+                               0 if filter_items is None else len(filter_items), mp, mb, int(stream), ids.ptr or None,
+                               scores.ptr or None, ctypes.byref(bad))
+    if bad.value:
+        return bad.value
+    _check_input(ctx, rc)
+    return 0
 
 
 def ranking_metrics(ctx, items, queries, k, query_rows, test, gain, gain_sum, liked=None):

@@ -16,8 +16,9 @@ from scipy.sparse import csr_matrix
 
 from . import _lib
 from .distributed import RowBlock
+from .utils import CudaArray
 from .utils import (BLOCK_FIELDS, ModelFitError, block_cuts, check_block_table, check_csr, check_random_state,
-                    column_splits, is_device_csr, nnz_balanced_splits, splits_from_cuts)
+                    column_splits, cuda_ids, is_cuda_array, is_device_csr, nnz_balanced_splits, splits_from_cuts)
 
 log = logging.getLogger("implicit")
 
@@ -128,10 +129,15 @@ class AlternatingLeastSquares:
     scaled by ``alpha`` after the cast, a scipy one before it.)  ``user_factors`` /
     ``item_factors`` take CUDA float32 2-D arrays too (rows may be strided), copied device to device; the numpy getters
     download them lazily.  ``user_factors_device`` / ``item_factors_device`` hand out device snapshots of the factors.
+    Serving on the device: when the ids argument of ``recommend`` / ``rank_items`` (``userid``), ``similar_items``
+    (``itemid``) or ``similar_users`` (``userid``) is a 1-D int32 / int64 CUDA array, the call runs on the device and
+    returns ``(ids, scores)`` as CUDA arrays (``__cuda_array_interface__`` v3, shape (n, N), complete when returned,
+    outliving the model), bitwise the host path's for the same values.  ``filter_items``, ``items`` and the
+    ``similar_*`` subsets may then be host or CUDA arrays, and no factor matrix is downloaded (norms and subsets are
+    computed on the device).  Other ids take the host path, unchanged.
     Not covered, and refused with ValueError: device CSRs on a process group of several ranks (RowBlocks of device
-    arrays included), ``recommend(..., items=...)`` with a device liked filter, a device liked filter of 2^31 - 1 or
-    more nonzeros, and ``evaluation`` with device CSRs; DLPack is not read, and ``recommend`` returns numpy ids and
-    scores.
+    arrays included), a device liked filter of 2^31 - 1 or more nonzeros, and ``evaluation`` with device CSRs; DLPack is
+    not read.
     """
 
     def __init__(
@@ -183,6 +189,7 @@ class AlternatingLeastSquares:
         self._dev_fresh = {"user": False, "item": False}   # device replica matches the host copy
         self._host_fresh = {"user": True, "item": True}    # host copy matches the device replica
         self._user_norms = self._item_norms = None
+        self._dev_norms = {"user": None, "item": None}  # DeviceSnapshots of the norms the device serving path reads
         self._YtY = self._XtX = None
 
     # ------------------------------------------------------------------ device plumbing
@@ -221,6 +228,7 @@ class AlternatingLeastSquares:
             self._user_factors, self._user_norms, self._XtX = value, None, None
         else:
             self._item_factors, self._item_norms, self._YtY = value, None, None
+        self._dev_norms[side] = None
         self._host_fresh[side] = True
         self._dev_fresh[side] = False
 
@@ -235,6 +243,7 @@ class AlternatingLeastSquares:
             self._user_factors, self._user_norms, self._XtX = None, None, None
         else:
             self._item_factors, self._item_norms, self._YtY = None, None, None
+        self._dev_norms[side] = None
         self._dev_fresh[side] = True
         self._host_fresh[side] = False
 
@@ -279,6 +288,7 @@ class AlternatingLeastSquares:
     def _mark_device_updated(self, side):
         self._dev_fresh[side] = True
         self._host_fresh[side] = False
+        self._dev_norms[side] = None
         if side == "user":
             self._user_norms = self._XtX = None
         else:
@@ -356,6 +366,7 @@ class AlternatingLeastSquares:
         X = self._device_factors("user")
         Y = self._device_factors("item")
         self._user_norms = self._item_norms = self._YtY = self._XtX = None  # cpu/als.py:152-154
+        self._dev_norms = {"user": None, "item": None}
 
         self._p2p = False
         if usplit is not None and os.environ.get("ALS_B200_NO_P2P") != "1":
@@ -565,10 +576,18 @@ class AlternatingLeastSquares:
     def _recalculate(self, ids, matrix, other_side, gram):
         """implicit/cpu/als.py:204-265: Cholesky on purpose, with the cached Gramian of the other side.  A device CSR is
         scaled by alpha on the device, after its values are cast to float32."""
+        out = self._recalculate_device(1 if np.isscalar(ids) else len(ids), matrix, other_side, gram)
+        try:
+            res = out.download()
+        finally:
+            out.close()
+        return res[0] if np.isscalar(ids) else res
+
+    def _recalculate_device(self, n, matrix, other_side, gram):
+        """The n rows _recalculate returns, left on the device: a DeviceFactors the caller closes."""
         device = is_device_csr(matrix)
         if not device:
             matrix = check_csr(matrix)
-        n = 1 if np.isscalar(ids) else len(ids)
         if matrix.shape[0] != n:
             raise ValueError("user_items should have one row for every item in user")
         if self.alpha != 1.0 and not device:
@@ -584,11 +603,12 @@ class AlternatingLeastSquares:
         out = _lib.DeviceFactors(ctx, n, self.factors)
         try:
             _lib.least_squares_with_gramian(ctx, gram, C, out, Y, self.regularization)
-            res = out.download()
+        except BaseException:
+            out.close()
+            raise
         finally:
             C.close()
-            out.close()
-        return res[0] if np.isscalar(ids) else res
+        return out
 
     def recalculate_user(self, userid, user_items):
         return self._recalculate(userid, user_items, "item", self.YtY)
@@ -638,6 +658,11 @@ class AlternatingLeastSquares:
     # ------------------------------------------------------------------ recommend (cpu/matrix_factorization_base.py:35-96)
     def recommend(self, userid, user_items, N=10, filter_already_liked_items=True, filter_items=None,
                   recalculate_user=False, items=None):
+        """cpu/matrix_factorization_base.py:35-96.  With userid a 1-D int32 / int64 CUDA array the call runs on the
+        device and returns (ids, scores) in CUDA memory (see _recommend_device)."""
+        if is_cuda_array(userid):
+            return self._recommend_device(userid, user_items, N, filter_already_liked_items, filter_items,
+                                          recalculate_user, items)
         device = is_device_csr(user_items)
         if filter_already_liked_items or recalculate_user:
             if not isinstance(user_items, csr_matrix) and not device:
@@ -774,7 +799,12 @@ class AlternatingLeastSquares:
             self._item_norms = n
         return self._item_norms
 
-    def _similar(self, side, ids_in, N, recalculated, filter_ids, subset):
+    def _similar(self, side, ids_in, N, recalculate, filter_ids, subset):
+        """recalculate: (item_users,) for similar_items(recalculate_item=True), else None.  With ids_in a 1-D int32 /
+        int64 CUDA array the call runs on the device (_similar_device)."""
+        if is_cuda_array(ids_in):
+            return self._similar_device(side, ids_in, N, recalculate, filter_ids, subset)
+        recalculated = None if recalculate is None else self.recalculate_item(ids_in, recalculate[0])
         ctx = self.ctx
         handle = self._device_factors(side)
         norms = self.user_norms if side == "user" else self.item_norms
@@ -821,9 +851,183 @@ class AlternatingLeastSquares:
             ids = subset[ids]
         return ids, scores
 
+    # ------------------------------------------------------------------ serving from CUDA ids
+    def _device_norms(self, side):
+        """The row norms of one side on the device (a DeviceSnapshot, bitwise the user_norms / item_norms properties),
+        cached until the factors change; never downloads the factors."""
+        if self._dev_norms[side] is None:
+            self._dev_norms[side] = self._device_factors(side).row_norms()
+        return self._dev_norms[side]
+
+    def _device_ids(self, ids, what, tmp, sort=False):
+        """The utils.CudaArray of an ids argument of a device call: a 1-D int32 / int64 CUDA array as it is (sorted into a
+        copy when `sort`), or host ids (list, numpy) uploaded, sorted first when `sort`.  Uploads and sorted copies are
+        appended to `tmp`.  Host ids keep numpy's dtype (np.array of a list of ints is int64); other than int32 / int64
+        they are refused with ValueError."""
+        if is_cuda_array(ids):
+            a = cuda_ids(ids, what)
+            if not sort:
+                return a
+            s = _lib.ids_sort(self.ctx, a)
+            tmp.append(s)
+            return s.cuda()
+        a = np.array(ids).ravel()
+        if a.size == 0 and a.dtype == np.float64:
+            a = a.astype(np.int64)  # np.array([]) of an empty list
+        if a.dtype not in (np.int32, np.int64):
+            raise ValueError(f"{what}: ids of dtype {a.dtype} (a call with ids in CUDA memory takes int32 or int64)")
+        if sort:
+            a.sort()
+        s = _lib.DeviceSnapshot.from_host(self.ctx, a)
+        tmp.append(s)
+        return s.cuda()
+
+    @staticmethod
+    def _one_stream(*arrays):
+        """The producer stream the CUDA arrays of one call name (0: none); ValueError when they name different ones."""
+        streams = {a.stream for a in arrays if a is not None and a.stream}
+        if len(streams) > 1:
+            raise ValueError("the CUDA arrays of one call name different producer streams")
+        return streams.pop() if streams else 0
+
+    def _recommend_device(self, userid, user_items, N, filter_already_liked_items, filter_items, recalculate_user,
+                          items):
+        """recommend() for userid in CUDA memory: the checks, the liked batches and the top-k of the host path, with the
+        ids, the subset, the liked remap and the outputs on the device, and no factor matrix downloaded.  Returns (ids,
+        scores), DeviceSnapshots of shape (len(userid), N): int32 ids (the subset's dtype with `items`), float32 scores,
+        bitwise the host path's for the same values.  filter_items / items may be host or CUDA arrays; user_items a
+        scipy or device CSR."""
+        ctx = self.ctx
+        uid = cuda_ids(userid, "userid")
+        n_query = len(uid)
+        device = is_device_csr(user_items)
+        if filter_already_liked_items or recalculate_user:
+            if not isinstance(user_items, csr_matrix) and not device:
+                raise ValueError("user_items needs to be a CSR sparse matrix")
+            if user_items.shape[0] != n_query:
+                raise ValueError("user_items must contain 1 row for every user in userids")
+        tmp = []
+        try:
+            query_rows = None
+            if recalculate_user:
+                queries = self._recalculate_device(n_query, user_items, "item", self.YtY)
+                tmp.append(queries)
+            else:
+                queries, query_rows = self._device_factors("user"), uid
+            item_handle = self._device_factors("item")
+            subset = None
+            if items is not None:
+                N = min(N, _ids_len(items, "items"))
+                if filter_items is not None and _ids_len(filter_items, "filter_items"):
+                    raise ValueError("Can't set both items and filter_items in recommend call")
+                if _ids_len(items, "items") == 0:
+                    raise ValueError("zero-size array to reduction operation maximum which has no identity")
+                subset = self._device_ids(items, "items", tmp, sort=True)
+                item_handle = _lib.DeviceFactors.gather_rows(ctx, item_handle, subset)
+                if item_handle is None:
+                    raise IndexError("Some itemids in the items parameter in are not in the model")
+                tmp.append(item_handle)
+
+            fq = None
+            batches = [(0, n_query)]
+            if filter_already_liked_items and device:
+                fq = _lib.DeviceCSR.from_device(ctx, user_items)  # unsorted rows are sorted on the device
+                tmp.append(fq)
+                if fq.shape3[2] > _LIKED_NNZ_MAX:
+                    raise ValueError(f"a liked filter in CUDA memory holds at most {_LIKED_NNZ_MAX} nonzeros")
+                if subset is not None:
+                    fq = fq.restrict_columns(subset)
+                    tmp.append(fq)
+            elif filter_already_liked_items:
+                fq = user_items
+                if subset is not None:  # the remap of the host path; only the subset's ids come to the host
+                    fq = _filter_items_from_sparse_matrix(_lib.ids_download(ctx, subset), fq)
+                if not fq.has_sorted_indices:
+                    fq = fq.sorted_indices()
+                if fq.nnz > _LIKED_NNZ_MAX:
+                    batches = liked_batches(fq.indptr, _LIKED_NNZ_MAX)
+
+            fl = None
+            if filter_items is not None:
+                fl = self._device_ids(filter_items, "filter_items", tmp)
+            stream = self._one_stream(uid, fl, subset)
+            N = int(N)
+            ids = _lib.DeviceSnapshot(ctx, (n_query, N), f"<i{4 if subset is None else subset.itemsize}")
+            scores = _lib.DeviceSnapshot(ctx, (n_query, N), "<f4")
+            for b0, b1 in batches:
+                liked = None
+                if device and fq is not None:
+                    liked = fq
+                elif fq is not None:
+                    liked = _lib.DeviceCSR.upload(ctx, fq if len(batches) == 1 else fq[b0:b1])
+                    tmp.append(liked)
+                qr = None if query_rows is None else _slice(query_rows, b0, b1)
+                bad = _lib.topk_into(ctx, item_handle, queries, N, b1 - b0, ids.cuda(b0), scores.cuda(b0),
+                                     query_rows=qr, query_row0=b0 if qr is None and len(batches) > 1 else 0,
+                                     liked=liked, filter_items=fl, id_map=subset, stream=stream)
+                if bad & 1:
+                    raise IndexError("userid out of range")
+                if bad:
+                    raise IndexError("filter_items contains ids that are not in the model")
+                if liked is not None and not device:
+                    liked.close()
+        finally:
+            for t in tmp:
+                t.close()
+        return ids, scores
+
+    def _similar_device(self, side, ids_in, N, recalculate, filter_ids, subset):
+        """_similar for ids in CUDA memory: the host path's top-k with the norms computed on the device (bitwise the
+        user_norms / item_norms properties), a subset gathered on the device (kept unsorted, duplicates included, and
+        N not clamped, as on the host) and the query norms divided out in the top-k's epilogue.  Returns DeviceSnapshots
+        (ids, scores) of shape (len(ids_in), N), like _recommend_device.  An id of filter_ids outside the model raises
+        IndexError (the host path ignores it)."""
+        ctx = self.ctx
+        what = f"{side}id"
+        qa = cuda_ids(ids_in, what)
+        tmp = []
+        try:
+            handle = self._device_factors(side)
+            if recalculate is not None:
+                queries = self._recalculate_device(len(qa), recalculate[0], "user", self.XtX)
+                tmp.append(queries)
+                query_rows, qnorms = None, queries.row_norms()
+                tmp.append(qnorms)
+            else:
+                queries, query_rows, qnorms = handle, qa, self._device_norms(side)
+            target, tnorms, sub = handle, self._device_norms(side), None
+            if subset is not None:
+                if filter_ids is not None and _ids_len(filter_ids, f"filter_{side}s"):
+                    raise ValueError("Can't set both a subset and a filter in a similar_* call")
+                if _ids_len(subset, "items" if side == "item" else "users") == 0:
+                    raise ValueError("zero-size array to reduction operation maximum which has no identity")
+                sub = self._device_ids(subset, "items" if side == "item" else "users", tmp)
+                target = _lib.DeviceFactors.gather_rows(ctx, handle, sub)
+                if target is None:
+                    raise IndexError("Some ids in the subset parameter are not in the model")
+                tmp.append(target)
+                tnorms = target.row_norms()  # bitwise the norms of those rows
+                tmp.append(tnorms)
+            fl = None
+            if filter_ids is not None:
+                fl = self._device_ids(filter_ids, f"filter_{side}s", tmp)
+            stream = self._one_stream(qa, fl, sub)
+            N = int(N)
+            ids = _lib.DeviceSnapshot(ctx, (len(qa), N), f"<i{4 if sub is None else sub.itemsize}")
+            scores = _lib.DeviceSnapshot(ctx, (len(qa), N), "<f4")
+            bad = _lib.topk_into(ctx, target, queries, N, len(qa), ids.cuda(), scores.cuda(), query_rows=query_rows,
+                                 item_norms=tnorms, query_norms=qnorms, filter_items=fl, id_map=sub, stream=stream)
+            if bad & 1:
+                raise IndexError(f"{what} out of range")
+            if bad:
+                raise IndexError(f"filter_{side}s contains ids that are not in the model")
+        finally:
+            for t in tmp:
+                t.close()
+        return ids, scores
+
     def similar_items(self, itemid, N=10, recalculate_item=False, item_users=None, filter_items=None, items=None):
-        rec = self.recalculate_item(itemid, item_users) if recalculate_item else None
-        return self._similar("item", itemid, N, rec, filter_items, items)
+        return self._similar("item", itemid, N, (item_users,) if recalculate_item else None, filter_items, items)
 
     def similar_users(self, userid, N=10, filter_users=None, users=None):
         return self._similar("user", userid, N, None, filter_users, users)
@@ -866,12 +1070,13 @@ class AlternatingLeastSquares:
         state = dict(self.__dict__)
         state["_user_factors"] = self.user_factors
         state["_item_factors"] = self.item_factors
-        state.update(_ctx=None, process_group=None, _dev={"user": None, "item": None},
+        state.update(_ctx=None, process_group=None, _dev={"user": None, "item": None}, _dev_norms={"user": None, "item": None},
                      _dev_fresh={"user": False, "item": False}, _host_fresh={"user": True, "item": True})
         return state
 
     def __setstate__(self, state):
         self.__dict__.update(state)
+        self.__dict__.setdefault("_dev_norms", {"user": None, "item": None})
 
 
 def _filter_items_from_sparse_matrix(items, query_items):
@@ -885,3 +1090,13 @@ def _filter_items_from_sparse_matrix(items, query_items):
     out = coo.tocsr()
     # the reference keeps the original column count; positions index the subset, so shrink to it
     return csr_matrix((out.data, out.indices, out.indptr), shape=(out.shape[0], len(items)))
+
+
+def _slice(a, b0, b1):
+    """Entries [b0, b1) of a 1-D utils.CudaArray."""
+    return CudaArray(a.ptr + b0 * a.itemsize, (b1 - b0,), a.itemsize, 1, a.stream)
+
+
+def _ids_len(ids, what):
+    """The number of ids of a host or CUDA ids argument."""
+    return len(cuda_ids(ids, what)) if is_cuda_array(ids) else int(np.asarray(ids).size)

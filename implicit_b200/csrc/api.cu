@@ -1533,3 +1533,163 @@ ALS_API int als_ranking_metrics(als_ctx *ctx, const als_factors *items, const al
   ALS_CUDA(cudaSetDevice(ctx->device));
   return launch_ranking_metrics(ctx, items, queries, query_rows, n_query, k, liked, test, gain_host, gain_sum_host, sums);
 }
+
+// ---- serving from device ids (serve.cu) ------------------------------------------------------------------------
+// ORs `bit` into the flag of ids outside [0, limit) and reads it back: 0 when every id is in range
+static int device_ids_out_of_range(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t limit, int *bad) {
+  *bad = 0;
+  if (n == 0) return ALS_OK;
+  int *flag = reinterpret_cast<int *>(ctx->counters + kCtrIdsBad);
+  ALS_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+  const int rc = stage_ids(ctx, ids, bytes, n, limit, nullptr, flag, 1);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(bad, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_device_upload(als_ctx *ctx, void *dst, const void *src, int64_t bytes) {
+  const char *who = "als_device_upload";
+  ALS_REQUIRE(ctx && ((dst && src) || bytes == 0) && bytes >= 0, "%s: bad argument", who);
+  if (bytes == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const int rc = require_device_memory(ctx, who, "dst", dst);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_device_download(als_ctx *ctx, void *dst, const void *src, int64_t bytes) {
+  const char *who = "als_device_download";
+  ALS_REQUIRE(ctx && ((dst && src) || bytes == 0) && bytes >= 0, "%s: bad argument", who);
+  if (bytes == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const int rc = require_device_memory(ctx, who, "src", src);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_ids_sort(als_ctx *ctx, const void *ids, int id_bytes, int64_t n, uint64_t producer_stream, void *sorted) {
+  const char *who = "als_ids_sort";
+  ALS_REQUIRE(ctx && ((ids && sorted) || n == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(id_bytes == 4 || id_bytes == 8, "%s: id_bytes must be 4 or 8, got %d", who, id_bytes);
+  ALS_REQUIRE(n >= 0, "%s: negative length", who);
+  if (n == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = require_device_memory(ctx, who, "ids", ids);
+  if (rc == ALS_OK) rc = require_device_memory(ctx, who, "sorted", sorted);
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc == ALS_OK) rc = sort_ids(ctx, ids, id_bytes, n, sorted);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_factors_gather_rows(als_ctx *ctx, const als_factors *src, const void *rows, int row_bytes, int64_t n,
+                                    uint64_t producer_stream, als_factors **out, int *bad) {
+  const char *who = "als_factors_gather_rows";
+  ALS_REQUIRE(ctx && src && out && bad && (rows || n == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(row_bytes == 4 || row_bytes == 8, "%s: row_bytes must be 4 or 8, got %d", who, row_bytes);
+  ALS_REQUIRE(n >= 0, "%s: negative length", who);
+  *out = nullptr;
+  *bad = 0;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = n ? require_device_memory(ctx, who, "rows", rows) : ALS_OK;
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc == ALS_OK) rc = device_ids_out_of_range(ctx, rows, row_bytes, n, src->rows, bad);
+  if (rc != ALS_OK) return rc;
+  ALS_REQUIRE(!*bad, "%s: rows holds ids outside [0, %lld)", who, (long long)src->rows);
+  als_factors *f = nullptr;
+  if ((rc = als_factors_create(ctx, n, src->f, &f)) != ALS_OK) return rc;
+  rc = launch_gather_rows(ctx, src, rows, row_bytes, n, f);
+  if (rc == ALS_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+    rc = cuda_fail(cudaGetLastError(), "als_factors_gather_rows", __FILE__, __LINE__);
+  if (rc != ALS_OK) {
+    als_factors_destroy(f);
+    return rc;
+  }
+  *out = f;
+  return ALS_OK;
+}
+
+ALS_API int als_factors_row_norms(als_ctx *ctx, const als_factors *f, float zero_value, float *norms) {
+  const char *who = "als_factors_row_norms";
+  ALS_REQUIRE(ctx && f && (norms || f->rows == 0), "%s: NULL argument", who);
+  if (f->rows == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = require_device_memory(ctx, who, "norms", norms);
+  if (rc == ALS_OK) rc = launch_row_norms(ctx, f, zero_value, norms);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
+}
+
+ALS_API int als_csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int subset_bytes, int64_t m,
+                                     uint64_t producer_stream, als_csr **out) {
+  const char *who = "als_csr_restrict_columns";
+  ALS_REQUIRE(ctx && liked && out && (subset || m == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(subset_bytes == 4 || subset_bytes == 8, "%s: subset_bytes must be 4 or 8, got %d", who, subset_bytes);
+  ALS_REQUIRE(m >= 0 && m < (int64_t)INT32_MAX, "%s: a subset of %lld ids", who, (long long)m);
+  ALS_REQUIRE(!liked->host && liked->segs.empty() && !liked->sched_pending,
+              "%s: the liked CSR must be one device-resident CSR of fewer than 2^31 - 1 nonzeros", who);
+  *out = nullptr;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = m ? require_device_memory(ctx, who, "subset", subset) : ALS_OK;
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc != ALS_OK) return rc;
+  int64_t *indptr = nullptr, nnz = 0;
+  int32_t *indices = nullptr;
+  float *data = nullptr;
+  rc = csr_restrict_columns(ctx, liked, subset, subset_bytes, m, &indptr, &indices, &data, &nnz);
+  // the remapped entries go through the one upload path, like every other CSR
+  if (rc == ALS_OK)
+    rc = csr_build(who, false, ctx, liked->rows, m, nnz, CsrArrays{indptr, 8, indices, 4, data, 4, true}, 0, out);
+  dev_free(ctx, indptr);
+  dev_free(ctx, indices);
+  dev_free(ctx, data);
+  return rc;
+}
+
+ALS_API int als_topk_into(als_ctx *ctx, const als_factors *items, const als_factors *queries, const void *query_rows,
+                          int query_row_bytes, int64_t query_row0, int64_t n_query, int k, const float *item_norms,
+                          const float *query_norms, const als_csr *liked, const void *filter_items, int filter_bytes,
+                          int64_t n_filter, const void *id_map, int map_bytes, uint64_t producer_stream, void *ids,
+                          float *scores, int *bad) {
+  const char *who = "als_topk_into";
+  ALS_REQUIRE(ctx && items && queries && bad, "%s: NULL argument", who);
+  *bad = 0;
+  const bool outputs = n_query > 0 && k > 0;
+  ALS_REQUIRE((ids && scores) || !outputs, "%s: NULL outputs", who);
+  ALS_REQUIRE(filter_items || n_filter == 0, "%s: NULL filter_items", who);
+  ALS_REQUIRE(query_row_bytes == 4 || query_row_bytes == 8, "%s: query_row_bytes must be 4 or 8, got %d", who, query_row_bytes);
+  ALS_REQUIRE(filter_bytes == 4 || filter_bytes == 8, "%s: filter_bytes must be 4 or 8, got %d", who, filter_bytes);
+  ALS_REQUIRE(map_bytes == 4 || map_bytes == 8, "%s: map_bytes must be 4 or 8, got %d", who, map_bytes);
+  ALS_REQUIRE(n_filter >= 0 && query_row0 >= 0, "%s: negative n_filter or query_row0", who);
+  ALS_REQUIRE(!query_rows || query_row0 == 0, "%s: query_row0 = %lld with query_rows", who, (long long)query_row0);
+  int rc = check_topk(who, items, queries, n_query, k, liked);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  const struct {
+    const void *p;
+    const char *name;
+    bool read;
+  } mem[] = {{query_rows, "query_rows", query_rows && n_query > 0},  {item_norms, "item_norms", item_norms && items->rows > 0},
+             {query_norms, "query_norms", query_norms && outputs}, {filter_items, "filter_items", n_filter > 0},
+             {id_map, "id_map", id_map && outputs},                 {ids, "ids", outputs},
+             {scores, "scores", outputs}};
+  for (const auto &a : mem)
+    if (a.read && (rc = require_device_memory(ctx, who, a.name, a.p)) != ALS_OK) return rc;
+  if ((rc = wait_for_producer(ctx, producer_stream)) != ALS_OK) return rc;
+  const TopkIds rows{query_rows, query_rows ? n_query : 0, query_row_bytes, true, query_row0};
+  const TopkIds filter{filter_items, n_filter, filter_bytes, true, 0};
+  TopkDevice t;
+  rc = topk_device(ctx, items, queries, rows, n_query, k, item_norms, true, liked, filter, &t);
+  *bad = t.bad;
+  if (rc == ALS_OK && outputs) rc = launch_topk_epilogue(ctx, t, n_query, k, id_map, map_bytes, query_norms, ids, scores);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // complete when this returns: any stream may read ids / scores
+  return ALS_OK;
+}

@@ -201,6 +201,7 @@ enum { kProfGramian = 0, kProfCholesky = 1, kProfCholFinish = 2, kProfCg = 3, kP
 enum {
   kCtrMain = 0, kCtrFinish = 1, kCtrDeferredCount = 2, kCtrDeferredWork = 3, kCtrWhitenOk = 4, kCtrHasNan = 5, kCtrYAbsMax = 6,
   kCtrChunks = 7,
+  kCtrIdsBad = 14,  // out-of-range bits of the device ids of a top-k (serve.cu stage_ids)
   kCtrShort = 8 /* +0..5: one per short-row size class */
 };
 // size classes of the short-row path: als_csr::le_begin[i] is the first work item of at most kShortThresholds[i] nonzeros
@@ -328,16 +329,47 @@ int launch_topk_tc(als_ctx *ctx, const float *items, int64_t n_items, const floa
 int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
                 int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
                 const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host);
+// Ids handed to the top-k: a host int32 array (als_topk, checked by its caller), or a device array of 4- or 8-byte ids
+// (als_topk_into), narrowed into the top-k's staging and range-checked on the device.  A NULL `p` with first > 0 stands
+// for the rows [first, first + n) (a batch of als_topk_into's queries without query rows).
+struct TopkIds {
+  const void *p = nullptr;
+  int64_t n = 0;
+  int bytes = 4;
+  bool device = false;
+  int64_t first = 0;
+};
 // The top-k of launch_topk left on the device: ids and scores [n_query, k_eff] in ctx->scratch, valid until the next call
-// that uses the scratch.  k_eff = min(k, items); 0 (and NULL arrays) when there is nothing to rank.
+// that uses the scratch.  k_eff = min(k, items); 0 (and NULL arrays) when there is nothing to rank.  query_rows: the int32
+// query rows the kernels read (NULL: rows 0, 1, ...).  bad: which device ids were out of range when topk_device refused
+// them (kBadQueryRows, kBadFilter), before any top-k launch.
 struct TopkDevice {
   int32_t *ids = nullptr;
   float *scores = nullptr;
   int k_eff = 0;
+  const int32_t *query_rows = nullptr;
+  int bad = 0;
 };
-int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
-                int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
-                const int32_t *filter_items, int64_t n_filter, TopkDevice *out);
+enum { kBadQueryRows = 1, kBadFilter = 2 };
+// item_norms: [items] fp32, in host memory, or in device memory when norms_on_device
+int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const TopkIds &query_rows,
+                int64_t n_query, int k, const float *item_norms, bool norms_on_device, const als_csr *liked,
+                const TopkIds &filter, TopkDevice *out);
+// serve.cu: the device side of als_topk_into and its helpers (als_b200.h).
+// stage_ids: n ids of `bytes` each -> int32 out (may be NULL: check only); an id outside [0, limit) ORs `bit` into *flag
+int stage_ids(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t limit, int32_t *out, int *flag, int bit);
+int stage_iota(als_ctx *ctx, int32_t *out, int64_t n, int64_t first);
+// t's [n_query, k_eff] -> ids / scores [n_query, k]: zero tail, ids = map[id] (map_bytes wide, else int32), scores /=
+// qnorm[query row]
+int launch_topk_epilogue(als_ctx *ctx, const TopkDevice &t, int64_t n_query, int k, const void *map, int map_bytes,
+                         const float *qnorm, void *ids, float *scores);
+int launch_row_norms(als_ctx *ctx, const als_factors *F, float zero_value, float *out);
+int launch_gather_rows(als_ctx *ctx, const als_factors *src, const void *rows, int bytes, int64_t n, als_factors *dst);
+int sort_ids(als_ctx *ctx, const void *in, int bytes, int64_t n, void *out);
+// the liked CSR remapped onto positions of the sorted subset[m]: device indptr (int64, rows + 1), indices and values
+// (1) from the pool, *nnz entries; the caller frees them
+int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m, int64_t **indptr,
+                         int32_t **indices, float **data, int64_t *nnz);
 // (indptr, indices) of a device CSR with every row in ascending column order: checked once on the device, and a CSR with
 // an unsorted row gets a sorted copy (indptr rebased to 0) kept with the handle (topk.cu)
 int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, const int32_t **indices);

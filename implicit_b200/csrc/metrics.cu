@@ -114,8 +114,11 @@ int launch_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_fac
   const int32_t *t_indptr = nullptr, *t_indices = nullptr;
   int rc = rows_in_order(ctx, test, &t_indptr, &t_indices);
   if (rc != ALS_OK) return rc;
+  TopkIds rows;
+  rows.p = query_rows;
+  rows.n = query_rows ? n_query : 0;
   TopkDevice t;
-  if ((rc = topk_device(ctx, items, queries, query_rows, n_query, k, nullptr, liked, nullptr, 0, &t)) != ALS_OK) return rc;
+  if ((rc = topk_device(ctx, items, queries, rows, n_query, k, nullptr, false, liked, TopkIds(), &t)) != ALS_OK) return rc;
   // the ids stay in ctx->scratch: what this pass needs comes from the pool
   const int grid = (int)ceil_div(n_query, kRowsPerCta);
   double *buf = nullptr;

@@ -593,13 +593,33 @@ int run_topk_f(als_ctx *ctx, const TopkArgs &a) {
 
 }  // namespace
 
-int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
-                int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
-                const int32_t *filter_items, int64_t n_filter, TopkDevice *out) {
+int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const TopkIds &query_rows,
+                int64_t n_query, int k, const float *item_norms, bool norms_on_device, const als_csr *liked,
+                const TopkIds &filter, TopkDevice *out) {
   *out = TopkDevice();
   if (items->ld != queries->ld) {
     set_error("topk: items and queries strides differ");
     return ALS_E_INVALID;
+  }
+  const int64_t n_filter = filter.n;
+  // device ids are checked before anything else, whether or not there is anything to rank (one flag readback)
+  if ((query_rows.device && query_rows.p) || (filter.device && n_filter)) {
+    int *flag = reinterpret_cast<int *>(ctx->counters + kCtrIdsBad);
+    ALS_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+    int rc = ALS_OK;
+    if (query_rows.device && query_rows.p)
+      rc = stage_ids(ctx, query_rows.p, query_rows.bytes, n_query, queries->rows, nullptr, flag, kBadQueryRows);
+    if (rc == ALS_OK && filter.device) rc = stage_ids(ctx, filter.p, filter.bytes, n_filter, items->rows, nullptr, flag, kBadFilter);
+    if (rc != ALS_OK) return rc;
+    int bad = 0;
+    ALS_CUDA(cudaMemcpyAsync(&bad, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (bad) {
+      out->bad = bad;
+      set_error("topk: %s holds ids outside [0, %lld)", (bad & kBadQueryRows) ? "query_rows" : "filter_items",
+                (long long)((bad & kBadQueryRows) ? queries->rows : items->rows));
+      return ALS_E_INVALID;
+    }
   }
   if (n_query == 0 || k == 0) return ALS_OK;
   const int64_t I = items->rows;
@@ -607,6 +627,12 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
   if (n_query >= INT32_MAX || I >= INT32_MAX) {
     set_error("topk: too many rows");
     return ALS_E_UNSUPPORTED;
+  }
+  const bool has_rows = query_rows.p || query_rows.first > 0;
+  if (!query_rows.p && query_rows.first + n_query > queries->rows) {
+    set_error("topk: %lld queries requested from a matrix of %lld rows", (long long)(query_rows.first + n_query),
+              (long long)queries->rows);
+    return ALS_E_INVALID;
   }
   // The output row stride is k; admission is clamped to the number of items (the k-list can never
   // hold more than I entries), which leaves the tail zero exactly like the reference.
@@ -620,13 +646,13 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
     return o;
   };
   const int64_t o_ids = take(out_elems * 4), o_sc = take(out_elems * 4);
-  const int64_t o_qr = take(query_rows ? n_query * 4 : 0);
-  const int64_t o_nrm = take(item_norms_host ? I * 4 : 0);
+  const int64_t o_qr = take(has_rows ? n_query * 4 : 0);
+  const int64_t o_nrm = take(item_norms && !norms_on_device ? I * 4 : 0);
   const int64_t o_mask = take(n_filter ? I : 0);
   const int64_t o_fl = take(n_filter * 4);
   // Large batches at 64 padded factors go to the wgmma kernel (topk_tc.cu).  It skips filtered items instead of
   // keeping them at -FLT_MAX, which is the same thing as long as every row has k unfiltered items left.
-  const bool use_tc = !ctx->knobs.topk_legacy && topk_tc_eligible(items->ld, n_query, I, k_eff, item_norms_host != nullptr) &&
+  const bool use_tc = !ctx->knobs.topk_legacy && topk_tc_eligible(items->ld, n_query, I, k_eff, item_norms != nullptr) &&
                       (!liked || !liked->sched_pending) &&
                       I - n_filter - (liked ? liked->max_row_nnz : 0) >= k_eff;
   const int64_t o_tc = take(use_tc ? topk_tc_scratch_bytes(n_query, I) : 0);
@@ -635,22 +661,29 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
   char *base = (char *)ctx->scratch;
   ALS_CUDA(cudaMemsetAsync(base + o_ids, 0, out_elems * 4, ctx->stream));
   ALS_CUDA(cudaMemsetAsync(base + o_sc, 0, out_elems * 4, ctx->stream));
-  if (query_rows) {
+  int32_t *qr = (int32_t *)(base + o_qr);
+  if (query_rows.p && query_rows.device) {
+    if ((rc = stage_ids(ctx, query_rows.p, query_rows.bytes, n_query, queries->rows, qr, nullptr, 0)) != ALS_OK) return rc;
+  } else if (query_rows.p) {
+    const int32_t *h = (const int32_t *)query_rows.p;
     for (int64_t q = 0; q < n_query; ++q)
-      if (query_rows[q] < 0 || query_rows[q] >= queries->rows) {
-        set_error("topk: query row %d out of range", query_rows[q]);
+      if (h[q] < 0 || h[q] >= queries->rows) {
+        set_error("topk: query row %d out of range", h[q]);
         return ALS_E_INVALID;
       }
-    ALS_CUDA(cudaMemcpyAsync(base + o_qr, query_rows, n_query * 4, cudaMemcpyHostToDevice, ctx->stream));
-  } else if (n_query > queries->rows) {
-    set_error("topk: %lld queries requested from a matrix of %lld rows", (long long)n_query, (long long)queries->rows);
-    return ALS_E_INVALID;
+    ALS_CUDA(cudaMemcpyAsync(qr, h, n_query * 4, cudaMemcpyHostToDevice, ctx->stream));
+  } else if (has_rows) {
+    if ((rc = stage_iota(ctx, qr, n_query, query_rows.first)) != ALS_OK) return rc;
   }
-  if (item_norms_host)
-    ALS_CUDA(cudaMemcpyAsync(base + o_nrm, item_norms_host, I * 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (item_norms && !norms_on_device)
+    ALS_CUDA(cudaMemcpyAsync(base + o_nrm, item_norms, I * 4, cudaMemcpyHostToDevice, ctx->stream));
   if (n_filter) {
     ALS_CUDA(cudaMemsetAsync(base + o_mask, 0, I, ctx->stream));
-    ALS_CUDA(cudaMemcpyAsync(base + o_fl, filter_items, n_filter * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (filter.device)
+      rc = stage_ids(ctx, filter.p, filter.bytes, n_filter, I, (int32_t *)(base + o_fl), nullptr, 0);
+    else
+      ALS_CUDA(cudaMemcpyAsync(base + o_fl, filter.p, n_filter * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (rc != ALS_OK) return rc;
     mask_scatter_kernel<<<(unsigned)ceil_div(n_filter, 256), 256, 0, ctx->stream>>>(
         (uint8_t *)(base + o_mask), (const int32_t *)(base + o_fl), n_filter, (int)I);
     ALS_CUDA(cudaGetLastError());
@@ -660,11 +693,11 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
   a.items = items->d;
   a.n_items = (int)I;
   a.queries = queries->d;
-  a.query_rows = query_rows ? (const int32_t *)(base + o_qr) : nullptr;
+  a.query_rows = has_rows ? qr : nullptr;
   a.n_query = (int)n_query;
   a.k = k_eff;
   a.k_out = k;
-  a.norms = item_norms_host ? (const float *)(base + o_nrm) : nullptr;
+  a.norms = !item_norms ? nullptr : norms_on_device ? item_norms : (const float *)(base + o_nrm);
   a.mask = n_filter ? (const uint8_t *)(base + o_mask) : nullptr;
   a.liked_indptr = nullptr;
   a.liked_indices = nullptr;
@@ -699,6 +732,7 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
   out->ids = a.ids;
   out->scores = a.scores;
   out->k_eff = k_eff;
+  out->query_rows = a.query_rows;
   return ALS_OK;
 }
 
@@ -709,8 +743,13 @@ int launch_topk(als_ctx *ctx, const als_factors *items, const als_factors *queri
     memset(ids_host, 0, sizeof(int32_t) * n_query * k);  // topk.pyx:20-21
     memset(scores_host, 0, sizeof(float) * n_query * k);
   }
+  TopkIds rows, filter;
+  rows.p = query_rows;
+  rows.n = query_rows ? n_query : 0;
+  filter.p = filter_items;
+  filter.n = n_filter;
   TopkDevice t;
-  int rc = topk_device(ctx, items, queries, query_rows, n_query, k, item_norms_host, liked, filter_items, n_filter, &t);
+  int rc = topk_device(ctx, items, queries, rows, n_query, k, item_norms_host, false, liked, filter, &t);
   if (rc != ALS_OK || t.k_eff == 0) return rc;
   // outputs: device [n_query, k_eff] -> host [n_query, k]
   ALS_CUDA(cudaMemcpy2DAsync(ids_host, sizeof(int32_t) * k, t.ids, sizeof(int32_t) * t.k_eff, sizeof(int32_t) * t.k_eff,

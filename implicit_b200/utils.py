@@ -100,6 +100,21 @@ def cuda_array(obj, what, typestrs, ndim):
     return parse_cai(cai, what, typestrs, ndim)
 
 
+def is_cuda_array(obj):
+    """True when obj exposes __cuda_array_interface__ (a CUDA torch tensor, a CuPy array, ...): recommend, rank_items
+    and similar_* take their device path for ids given this way."""
+    return not isinstance(obj, np.ndarray) and hasattr(obj, "__cuda_array_interface__")
+
+
+ID_TYPESTRS = ("<i4", "<i8")
+
+
+def cuda_ids(obj, what):
+    """The CudaArray of a 1-D int32 / int64 array of ids in CUDA memory; ValueError, naming `what`, for another typestr
+    (float ids), another number of dimensions and whatever parse_cai refuses."""
+    return cuda_array(obj, what, ID_TYPESTRS, 1)
+
+
 def _is_torch_sparse_csr(m):
     return str(getattr(m, "layout", "")) == "torch.sparse_csr" and callable(getattr(m, "crow_indices", None))
 

@@ -285,6 +285,52 @@ int als_calculate_loss(als_ctx *ctx, const als_csr *C, const als_factors *X, con
 int als_topk(als_ctx *ctx, const als_factors *items, const als_factors *queries, const int32_t *query_rows,
              int64_t n_query, int k, const float *item_norms_host, const als_csr *liked,
              const int32_t *filter_items, int64_t n_filter, int32_t *ids_host, float *scores_host);
+/* ---- serving from device ids: CUDA ids in, CUDA ids and scores out ------------------------------------------------
+ * Every array below is device memory of the context's device (or managed memory); anything else is refused with
+ * ALS_E_INVALID, naming the argument.  Ids are int32 (4 bytes) or int64 (8 bytes).  Each call is ordered after the
+ * work queued so far on producer_stream (a cudaStream_t as an integer; 0: none) and has read its inputs and completed
+ * its outputs when it returns (it synchronises).
+ *
+ * als_topk_into: the top-k of als_topk, written to ids / scores [n_query, k] that the caller allocated (als_device_alloc),
+ * the tail past the items zero as in als_topk.  query_rows [n_query] (NULL: rows [query_row0, query_row0 + n_query) of
+ * queries), item_norms [items rows] (NULL: none) and filter_items [n_filter] are device arrays; the query rows and the
+ * filter are range-checked on the device before any top-k launch, and an id outside [0, queries rows) / [0, items rows)
+ * returns ALS_E_INVALID with *bad = 1 (query_rows) | 2 (filter_items), nothing written.  One epilogue kernel reads the
+ * top-k's scratch output and writes the caller's arrays: with id_map (NULL: none) each id becomes id_map[id], and ids
+ * holds map_bytes per entry (else int32); with query_norms (NULL: none) each score becomes score / query_norms[r], r the
+ * query's row of queries (fp32 division, as numpy's scores / norm[:, None]).  Shares als_topk's checks and top-k driver,
+ * so the same inputs give bitwise als_topk's ids and scores. */
+int als_topk_into(als_ctx *ctx, const als_factors *items, const als_factors *queries, const void *query_rows,
+                  int query_row_bytes, int64_t query_row0, int64_t n_query, int k, const float *item_norms,
+                  const float *query_norms, const als_csr *liked, const void *filter_items, int filter_bytes,
+                  int64_t n_filter, const void *id_map, int map_bytes, uint64_t producer_stream, void *ids, float *scores,
+                  int *bad);
+/* A new factor matrix (*out) of the rows src[rows[i]], i < n, its padding columns zero (the wgmma top-k reads them).
+ * rows are range-checked on the device first: an id outside [0, src rows) returns ALS_E_INVALID with *bad = 1 and
+ * creates nothing. */
+int als_factors_gather_rows(als_ctx *ctx, const als_factors *src, const void *rows, int row_bytes, int64_t n,
+                            uint64_t producer_stream, als_factors **out, int *bad);
+/* norms[r] = the fp32 norm of row r of f, bitwise numpy's np.linalg.norm(F, axis=-1): sqrt of numpy's pairwise float32
+ * sum of the squares of exactly f->f elements (never the padding), every step rounded on its own; a zero norm is
+ * written as zero_value (1e-10 for similar_items, implicit/cpu/matrix_factorization_base.py). */
+int als_factors_row_norms(als_ctx *ctx, const als_factors *f, float zero_value, float *norms);
+/* bytes of host memory copied to dst, device memory of the context's device (the host ids of a call whose other ids
+ * are in CUDA memory). */
+int als_device_upload(als_ctx *ctx, void *dst, const void *src, int64_t bytes);
+/* bytes of device memory src (of the context's device) copied to the host: the sorted subset of a call whose liked
+ * filter is a scipy CSR, remapped on the host. */
+int als_device_download(als_ctx *ctx, void *dst, const void *src, int64_t bytes);
+/* sorted[n] = ids[n] in ascending order (CUB radix sort; equal to numpy's sort of the same integers). */
+int als_ids_sort(als_ctx *ctx, const void *ids, int id_bytes, int64_t n, uint64_t producer_stream, void *sorted);
+/* The liked CSR remapped onto a column subset, as recommend(..., items=subset) remaps a scipy liked filter
+ * (_filter_items_from_sparse_matrix): *out has liked's rows and m columns, and row r holds, sorted and once each, the
+ * positions in subset[m] (ascending; searched like numpy's searchsorted(side="left")) of the columns of row r that
+ * are in the subset and whose stored value is not 0.  Values are 1 (a liked filter reads positions only).  Built on
+ * the device -- count, scan, scatter, a CUB segmented sort and unique per row -- and laid out by the one upload path
+ * (the layout and max_row_nnz of the scipy remap uploaded with als_csr_upload).  liked must be one device-resident
+ * CSR (not segmented, not host-resident). */
+int als_csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int subset_bytes, int64_t m,
+                             uint64_t producer_stream, als_csr **out);
 /* Ranking metrics at k of the top-k above, without its ids leaving the device: the ids als_topk would return (no item
  * norms, no filter_items; ranks past the items are id 0) are scored against `test`, a CSR over the query rows of the
  * withheld items (any order within a row, repeats and stored zeros allowed; sorted on the device like `liked`).  Per
