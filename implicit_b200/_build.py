@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libals_b200.so")
-SOURCES = ["api.cu", "csr.cu", "gen.cu", "gramian.cu", "cholesky.cu", "cholesky_tc.cu", "cholesky_short.cu", "dense.cu", "cholesky_wide.cu", "cholesky_xwide.cu", "cg.cu", "loss.cu", "topk.cu", "topk_tc.cu", "metrics.cu", "serve.cu", "comm.cu"]
+SOURCES = ["api.cu", "csr.cu", "gen.cu", "gramian.cu", "cholesky.cu", "cholesky_tc.cu", "cholesky_short.cu", "dense.cu", "cholesky_wide.cu", "cholesky_xwide.cu", "cg.cu", "loss.cu", "topk.cu", "topk_tc.cu", "metrics.cu", "serve.cu", "refit.cu", "comm.cu"]
 HEADERS = [os.path.join(CSRC, "common.h"), os.path.join(CSRC, "cholesky_device.cuh"), os.path.join(CSRC, "sm90.cuh"),
            os.path.join(HERE, "..", "include", "als_b200.h")]
 

@@ -115,6 +115,9 @@ SIGNATURES = {
     "als_factors_row_norms": (c_int, [c_void_p, c_void_p, c_f32, c_void_p]),
     "als_ids_sort": (c_int, [c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, c_void_p]),
     "als_csr_restrict_columns": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, P(c_void_p)]),
+    "als_ids_range": (c_int, [c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, P(c_i64), P(c_i64)]),
+    "als_factors_grow": (c_int, [c_void_p, c_void_p, c_i64]),
+    "als_factors_scatter_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_i64, ctypes.c_uint64, c_void_p]),
 }
 
 
@@ -639,6 +642,20 @@ class DeviceFactors:
         f.ctx, f.h, f.rows, f.factors = ctx, h, len(rows), src.factors
         return f
 
+    def grow(self, rows):
+        """Grows the matrix to `rows` rows on the device (als_factors_grow): the old rows are kept, the new ones are zero.
+        ValueError, the matrix unchanged, for more rows than the device's memory holds."""
+        rows = min(int(rows), 2**63 - 1)  # max id + 1 of int64 ids: past any device, and still an int64
+        _check_input(self.ctx, self.ctx.lib.als_factors_grow(self.ctx.h, self.h, rows))
+        self.rows = int(rows)
+
+    def scatter_rows(self, ids, src):
+        """self[ids] = src on the device (als_factors_scatter_rows): ids a utils.CudaArray of src.rows int32 / int64
+        ids inside the matrix, read after the work its producer queued on the stream it names; of a repeated id the last
+        occurrence wins, as in numpy."""
+        _check_input(self.ctx, self.ctx.lib.als_factors_scatter_rows(self.ctx.h, self.h, ids.ptr or None, ids.itemsize,
+                                                                     len(ids), ids.stream, src.h))
+
     def row_norms(self, zero_value=1e-10):
         """A DeviceSnapshot [rows] '<f4' of the row norms, bitwise np.linalg.norm(F, axis=-1) with zeros written as
         float32(zero_value) (the `n[n == 0] = 1e-10` of the user_norms / item_norms properties)."""
@@ -762,6 +779,15 @@ def ids_sort(ctx, ids):
         out.close()
         raise
     return out
+
+
+def ids_range(ctx, ids):
+    """(min, max) of the utils.CudaArray ids, read after the work its producer queued on the stream it names: one pass and
+    one 16-byte read-back (als_ids_range).  (0, -1) for no ids."""
+    lo, hi = c_i64(), c_i64()
+    _check_input(ctx, ctx.lib.als_ids_range(ctx.h, ids.ptr or None, ids.itemsize, len(ids), ids.stream, ctypes.byref(lo),
+                                            ctypes.byref(hi)))
+    return lo.value, hi.value
 
 
 # ---- the native operator interface, named like the reference's (implicit/cpu/_als.pyx, topk.pyx) ----

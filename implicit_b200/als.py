@@ -135,9 +135,16 @@ class AlternatingLeastSquares:
     outliving the model), bitwise the host path's for the same values.  ``filter_items``, ``items`` and the
     ``similar_*`` subsets may then be host or CUDA arrays, and no factor matrix is downloaded (norms and subsets are
     computed on the device).  Other ids take the host path, unchanged.
+    Refitting on the device: when ``userids`` / ``itemids`` of ``partial_fit_users`` / ``partial_fit_items`` is a 1-D
+    int32 / int64 CUDA array, the rows are solved, the factor matrix grown (new rows zero) and the rows stored on the
+    device, the last occurrence of a repeated id winning as in numpy; no factor matrix crosses PCIe and the host copy is
+    downloaded only when a getter asks for it.  The factors are bitwise those of the numpy call where it succeeds: with
+    numpy ids, a call that adds no new rows raises ("assignment destination is read-only", the getters hand out
+    read-only views), where the CUDA-id call stores the rows.  A max id whose rows would not fit in the device's memory
+    is refused with ValueError (the numpy call raises MemoryError).
     Not covered, and refused with ValueError: device CSRs on a process group of several ranks (RowBlocks of device
-    arrays included), a device liked filter of 2^31 - 1 or more nonzeros, and ``evaluation`` with device CSRs; DLPack is
-    not read.
+    arrays included), CUDA ids in ``partial_fit_*`` there too, a negative CUDA id in ``partial_fit_*``, a device liked
+    filter of 2^31 - 1 or more nonzeros, and ``evaluation`` with device CSRs; DLPack is not read.
     """
 
     def __init__(
@@ -617,7 +624,11 @@ class AlternatingLeastSquares:
         return self._recalculate(itemid, item_users, "user", self.XtX)
 
     def partial_fit_users(self, userids, user_items):
-        """implicit/cpu/als.py:267-307"""
+        """implicit/cpu/als.py:267-307.  With userids a 1-D int32 / int64 CUDA array the rows are refitted in place on
+        the device (_partial_fit_device)."""
+        if is_cuda_array(userids):
+            return self._partial_fit_device("user", userids, user_items,
+                                            "user_items must contain 1 row for every user in userids")
         if len(userids) != user_items.shape[0]:
             raise ValueError("user_items must contain 1 row for every user in userids")
         user_factors = self.recalculate_user(userids, user_items)
@@ -630,7 +641,10 @@ class AlternatingLeastSquares:
         self.user_factors = host
 
     def partial_fit_items(self, itemids, item_users):
-        """implicit/cpu/als.py:309-349"""
+        """implicit/cpu/als.py:309-349.  With itemids a 1-D int32 / int64 CUDA array, as partial_fit_users."""
+        if is_cuda_array(itemids):
+            return self._partial_fit_device("item", itemids, item_users,
+                                            "item_users must contain 1 row for every user in itemids")
         if len(itemids) != item_users.shape[0]:
             raise ValueError("item_users must contain 1 row for every user in itemids")
         item_factors = self.recalculate_item(itemids, item_users)
@@ -641,6 +655,45 @@ class AlternatingLeastSquares:
             host = np.concatenate([host, np.zeros((max_itemid - items + 1, factors), dtype=self.dtype)])
         host[itemids] = item_factors
         self.item_factors = host
+
+    def _partial_fit_device(self, side, ids_in, matrix, count_message):
+        """partial_fit_* for ids in CUDA memory: the rows are recalculated on the device (the same solve, with the same
+        cached Gramian, as the host path), the device replica grows to max(ids) + 1 rows if it must (new rows zero) and
+        takes the rows at their ids, the last occurrence of a repeated id winning, as numpy's host[ids] = rows does.  No
+        factor matrix crosses PCIe: one pass over the ids reads back their min and max, and the host copy is downloaded
+        only if a getter asks for it.  ValueError, before anything is written: a process group of several ranks, ids
+        that are not 1-D int32 / int64, a row count other than len(ids), a negative id; and, after the solve, no ids at
+        all (like the host path's max() of no ids) and a max id whose rows would not fit in the device's memory."""
+        what = f"{side}ids"
+        pg = self.process_group
+        if pg is not None and pg.world > 1:
+            raise ValueError(f"{what} in CUDA memory refit {side}s on one GPU; on a process group of several ranks pass "
+                             f"{what} as a host array")
+        ids = cuda_ids(ids_in, what)
+        if len(ids) != matrix.shape[0]:
+            raise ValueError(count_message)
+        ctx = self.ctx
+        lo, hi = _lib.ids_range(ctx, ids)
+        if lo < 0:
+            raise ValueError(f"{what} holds a negative id ({lo})")
+        other = "item" if side == "user" else "user"
+        rows = self._recalculate_device(len(ids), matrix, other, self.YtY if side == "user" else self.XtX)
+        grown = False
+        try:
+            if not len(ids):
+                raise ValueError(f"{what} is empty: no rows to refit")
+            F = self._device_factors(side)
+            if hi >= F.rows:
+                F.grow(hi + 1)  # ValueError, F unchanged, past the device's memory
+                grown = True
+            F.scatter_rows(ids, rows)
+        except BaseException:
+            if grown:  # the replica has rows the host copy lacks: it is the current copy from here on
+                self._mark_device_updated(side)
+            raise
+        finally:
+            rows.close()
+        self._mark_device_updated(side)
 
     @property
     def YtY(self):

@@ -1693,3 +1693,67 @@ ALS_API int als_topk_into(als_ctx *ctx, const als_factors *items, const als_fact
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // complete when this returns: any stream may read ids / scores
   return ALS_OK;
 }
+
+// ---- refitting rows in place from device ids (refit.cu) ----------------------------------------------------------
+ALS_API int als_ids_range(als_ctx *ctx, const void *ids, int id_bytes, int64_t n, uint64_t producer_stream,
+                          int64_t *min_id, int64_t *max_id) {
+  const char *who = "als_ids_range";
+  ALS_REQUIRE(ctx && min_id && max_id && (ids || n == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(id_bytes == 4 || id_bytes == 8, "%s: id_bytes must be 4 or 8, got %d", who, id_bytes);
+  ALS_REQUIRE(n >= 0, "%s: negative length", who);
+  *min_id = 0;
+  *max_id = -1;
+  if (n == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = require_device_memory(ctx, who, "ids", ids);
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc == ALS_OK) rc = ids_range(ctx, ids, id_bytes, n, min_id, max_id);
+  return rc;
+}
+
+ALS_API int als_factors_grow(als_ctx *ctx, als_factors *f, int64_t rows) {
+  const char *who = "als_factors_grow";
+  ALS_REQUIRE(ctx && f, "%s: NULL argument", who);
+  ALS_REQUIRE(rows >= f->rows, "%s: %lld rows would shrink a matrix of %lld", who, (long long)rows, (long long)f->rows);
+  ALS_REQUIRE(f->pooled && f->n_peers == 0, "%s: the matrix is shared with other ranks", who);
+  if (rows == f->rows) return ALS_OK;
+  const int64_t row_bytes = sizeof(float) * (int64_t)f->ld;
+  // checked before the product is formed: a row count whose bytes overflow int64 or exceed the device's memory (a
+  // hashed 64-bit id, say) is refused, never allocated short
+  ALS_REQUIRE(rows <= ctx->mem_bytes / row_bytes, "%s: %lld rows of %lld bytes are more than the device's %lld bytes", who,
+              (long long)rows, (long long)row_bytes, (long long)ctx->mem_bytes);
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  float *d = nullptr;
+  const int rc = dev_alloc(ctx, (void **)&d, row_bytes * rows);
+  if (rc != ALS_OK) return rc;
+  cudaError_t e = f->rows ? cudaMemcpyAsync(d, f->d, row_bytes * f->rows, cudaMemcpyDeviceToDevice, ctx->stream)
+                          : cudaSuccess;
+  // the new rows, padding included, are zero: np.concatenate([host, np.zeros(...)]) uploaded
+  if (e == cudaSuccess) e = cudaMemsetAsync(d + f->rows * f->ld, 0, row_bytes * (rows - f->rows), ctx->stream);
+  if (e != cudaSuccess) {
+    dev_free(ctx, d);
+    return cuda_fail(e, "als_factors_grow", __FILE__, __LINE__);
+  }
+  dev_free(ctx, f->d);  // stream-ordered: after the copy has read it
+  f->d = d;
+  f->rows = rows;
+  return ALS_OK;
+}
+
+ALS_API int als_factors_scatter_rows(als_ctx *ctx, als_factors *dst, const void *ids, int id_bytes, int64_t n,
+                                     uint64_t producer_stream, const als_factors *src) {
+  const char *who = "als_factors_scatter_rows";
+  ALS_REQUIRE(ctx && dst && src && (ids || n == 0), "%s: NULL argument", who);
+  ALS_REQUIRE(id_bytes == 4 || id_bytes == 8, "%s: id_bytes must be 4 or 8, got %d", who, id_bytes);
+  ALS_REQUIRE(n == src->rows, "%s: %lld ids for %lld rows", who, (long long)n, (long long)src->rows);
+  ALS_REQUIRE(src->f == dst->f, "%s: rows of %d factors into a matrix of %d", who, src->f, dst->f);
+  ALS_REQUIRE(dst->n_peers == 0, "%s: the matrix is shared with other ranks", who);
+  if (n == 0) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  int rc = require_device_memory(ctx, who, "ids", ids);
+  if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
+  if (rc == ALS_OK) rc = scatter_rows(ctx, dst, ids, id_bytes, n, src);
+  if (rc != ALS_OK) return rc;
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // the ids have been read: the caller may free or refill them
+  return ALS_OK;
+}

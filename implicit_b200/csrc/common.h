@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <functional>
 #include <string>
 #include <vector>
@@ -355,6 +356,10 @@ enum { kBadQueryRows = 1, kBadFilter = 2 };
 int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queries, const TopkIds &query_rows,
                 int64_t n_query, int k, const float *item_norms, bool norms_on_device, const als_csr *liked,
                 const TopkIds &filter, TopkDevice *out);
+// the grid of a grid-stride loop of 256-thread blocks over `threads` elements: at most 16 blocks per SM
+static inline int grid_for(als_ctx *ctx, int64_t threads) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(threads, 256), (int64_t)ctx->sm_count * 16));
+}
 // serve.cu: the device side of als_topk_into and its helpers (als_b200.h).
 // stage_ids: n ids of `bytes` each -> int32 out (may be NULL: check only); an id outside [0, limit) ORs `bit` into *flag
 int stage_ids(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t limit, int32_t *out, int *flag, int bit);
@@ -370,6 +375,12 @@ int sort_ids(als_ctx *ctx, const void *in, int bytes, int64_t n, void *out);
 // (1) from the pool, *nnz entries; the caller frees them
 int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m, int64_t **indptr,
                          int32_t **indices, float **data, int64_t *nnz);
+// refit.cu: the device side of partial_fit_* with CUDA ids (als_ids_range, als_factors_scatter_rows).
+// ids_range: min and max of n ids of `bytes` each (n = 0: 0 and -1); synchronises
+int ids_range(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t *min_id, int64_t *max_id);
+// dst[ids[i]] = src[i] for i < n (src->rows = n, the same width), the last occurrence of a repeated id winning; ids
+// outside [0, dst->rows) are skipped
+int scatter_rows(als_ctx *ctx, als_factors *dst, const void *ids, int bytes, int64_t n, const als_factors *src);
 // (indptr, indices) of a device CSR with every row in ascending column order: checked once on the device, and a CSR with
 // an unsorted row gets a sorted copy (indptr rebased to 0) kept with the handle (topk.cu)
 int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, const int32_t **indices);

@@ -191,10 +191,6 @@ __global__ void restrict_unique_kernel(const int64_t *__restrict__ off, int64_t 
   }
 }
 
-int grid_for(als_ctx *ctx, int64_t threads) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(threads, 256), (int64_t)ctx->sm_count * 16));
-}
-
 // exclusive scan of counts[0, rows) into off[0, rows]; counts[rows] must be 0
 int scan_counts(als_ctx *ctx, int64_t *counts, int64_t rows, int64_t *off) {
   size_t tmp_bytes = 0;

@@ -350,6 +350,30 @@ int als_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_factor
                         int64_t n_query, int k, const als_csr *liked, const als_csr *test, const double *gain_host,
                         const double *gain_sum_host, double *sums /* [6] */);
 
+/* ---- refitting rows in place from device ids ----------------------------------------------------------------------
+ * The device side of partial_fit_users / partial_fit_items (implicit/cpu/als.py:267-349) for ids in CUDA memory: the
+ * factor matrix grows and takes the recalculated rows where it lives, and no factor matrix crosses PCIe.  Ids and
+ * producer_stream as in the serving calls above.
+ *
+ * *min_id / *max_id = the smallest and largest of ids[n] (n = 0: 0 and -1), in one pass and one 16-byte read-back
+ * (synchronises): the caller refuses a negative id and grows the matrix to max + 1 rows, the max(userids) of
+ * implicit/cpu/als.py:301-302. */
+int als_ids_range(als_ctx *ctx, const void *ids, int id_bytes, int64_t n, uint64_t producer_stream, int64_t *min_id,
+                  int64_t *max_id);
+/* f grows to `rows` rows (not fewer than it has) in a new allocation of the same padded row stride: the old rows are
+ * copied device to device and rows [old rows, rows) are zero, padding included -- np.concatenate([factors,
+ * np.zeros(...)]) of implicit/cpu/als.py:302-305, uploaded.  The old and the new matrix are both allocated while the
+ * copy runs.  Refused with ALS_E_INVALID, f unchanged: a matrix shared with other ranks (exported over CUDA IPC), and a
+ * row count whose bytes would exceed the device's memory (so no byte count overflows, whatever id asked for it). */
+int als_factors_grow(als_ctx *ctx, als_factors *f, int64_t rows);
+/* dst[ids[i]] = src[i] for i < n (src has n rows and dst's width), with the semantics of numpy's factors[ids] = rows
+ * (implicit/cpu/als.py:308, 345): of an id that repeats, the last occurrence wins, deterministically.  The (id,
+ * position) pairs are radix-sorted (stable) and only the last pair of each id writes its row: the `factors` columns
+ * from src, the padding columns as zeros.  Rows no id names keep their bits; an id outside [0, dst rows) is skipped,
+ * never written (als_ids_range gives the caller the range to grow to).  Synchronises. */
+int als_factors_scatter_rows(als_ctx *ctx, als_factors *dst, const void *ids, int id_bytes, int64_t n,
+                             uint64_t producer_stream, const als_factors *src);
+
 /* ---- multi-GPU (one process per GPU; NCCL over NVLink/NVSwitch) -------------------------------- */
 /* The reference has no multi-GPU path (`// TODO: multi-gpu support`, implicit/gpu/als.cu:169). */
 #define ALS_COMM_ID_BYTES 128
