@@ -105,6 +105,8 @@ SIGNATURES = {
     "als_factors_export_device": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64]),
     "als_device_alloc": (c_int, [c_void_p, c_i64, P(c_void_p)]),
     "als_device_free": (c_int, [c_void_p, c_void_p]),
+    "als_pool_alloc": (c_int, [c_void_p, c_i64, P(c_void_p)]),
+    "als_pool_free": (c_int, [c_void_p, c_void_p]),
     "als_topk_into": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_int, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_int, c_i64, c_void_p, c_int, ctypes.c_uint64, c_void_p, c_void_p,
                               P(c_int)]),
@@ -696,15 +698,17 @@ class DeviceSnapshot:
     no stream to wait for.  The factor snapshots (of_factors) are '<f4' rows of the padded width; the outputs of the
     device serving calls are contiguous ids and scores.  torch.as_tensor(s, device="cuda") and cupy.asarray(s) keep the
     object, and so its memory, alive; the memory is freed (cudaFree, after every stream's work) when the last reference
-    dies, and outlives the model and the context object that made it."""
+    dies, and outlives the model and the context object that made it.  `pooled`: a temporary of the library's own calls
+    (als_pool_alloc), read only on the context's stream and closed by the caller; no wait for the device to free it."""
 
-    def __init__(self, ctx, shape, typestr, ld=None):
-        self.ctx, self.shape, self.typestr = ctx, tuple(int(n) for n in shape), typestr
+    def __init__(self, ctx, shape, typestr, ld=None, pooled=False):
+        self.ctx, self.shape, self.typestr, self.pooled = ctx, tuple(int(n) for n in shape), typestr, pooled
         self.itemsize = int(typestr[2:])
         self.ld = self.shape[-1] if ld is None else int(ld)
         count = self.shape[0] * (self.ld if len(self.shape) == 2 else 1)
         self.ptr = c_void_p()
-        check(ctx.lib.als_device_alloc(ctx.h, self.itemsize * count, ctypes.byref(self.ptr)))
+        alloc = ctx.lib.als_pool_alloc if pooled else ctx.lib.als_device_alloc
+        check(alloc(ctx.h, self.itemsize * count, ctypes.byref(self.ptr)))
 
     @classmethod
     def of_factors(cls, factors):
@@ -721,10 +725,10 @@ class DeviceSnapshot:
         return s
 
     @classmethod
-    def from_host(cls, ctx, a):
+    def from_host(cls, ctx, a, pooled=False):
         """A 1-D copy of the contiguous numpy array a ('<i4', '<i8' or '<f4')."""
         a = np.ascontiguousarray(a)
-        s = cls(ctx, a.shape, a.dtype.str)
+        s = cls(ctx, a.shape, a.dtype.str, pooled=pooled)
         try:
             check(ctx.lib.als_device_upload(ctx.h, s.ptr, ptr(a) if a.size else None, a.nbytes))
         except BaseException:
@@ -746,7 +750,7 @@ class DeviceSnapshot:
 
     def close(self):
         if getattr(self, "ptr", None) and getattr(self.ctx, "h", None):
-            self.ctx.lib.als_device_free(self.ctx.h, self.ptr)
+            (self.ctx.lib.als_pool_free if self.pooled else self.ctx.lib.als_device_free)(self.ctx.h, self.ptr)
         self.ptr = None
 
     def __del__(self):
@@ -771,8 +775,8 @@ def ids_download(ctx, ids):
 
 
 def ids_sort(ctx, ids):
-    """A DeviceSnapshot of the utils.CudaArray ids sorted ascending on the device, of the same width."""
-    out = DeviceSnapshot(ctx, ids.shape, f"<i{ids.itemsize}")
+    """A pooled DeviceSnapshot of the utils.CudaArray ids sorted ascending on the device, of the same width."""
+    out = DeviceSnapshot(ctx, ids.shape, f"<i{ids.itemsize}", pooled=True)
     try:
         _check_input(ctx, ctx.lib.als_ids_sort(ctx.h, ids.ptr or None, ids.itemsize, len(ids), ids.stream, out.ptr))
     except BaseException:

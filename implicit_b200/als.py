@@ -129,12 +129,15 @@ class AlternatingLeastSquares:
     scaled by ``alpha`` after the cast, a scipy one before it.)  ``user_factors`` /
     ``item_factors`` take CUDA float32 2-D arrays too (rows may be strided), copied device to device; the numpy getters
     download them lazily.  ``user_factors_device`` / ``item_factors_device`` hand out device snapshots of the factors.
-    Serving on the device: when the ids argument of ``recommend`` / ``rank_items`` (``userid``), ``similar_items``
-    (``itemid``) or ``similar_users`` (``userid``) is a 1-D int32 / int64 CUDA array, the call runs on the device and
-    returns ``(ids, scores)`` as CUDA arrays (``__cuda_array_interface__`` v3, shape (n, N), complete when returned,
-    outliving the model), bitwise the host path's for the same values.  ``filter_items``, ``items`` and the
-    ``similar_*`` subsets may then be host or CUDA arrays, and no factor matrix is downloaded (norms and subsets are
-    computed on the device).  Other ids take the host path, unchanged.
+    Serving: ``recommend`` / ``rank_items``, ``similar_items`` and ``similar_users`` run on the device whatever their
+    ids, and no factor matrix is downloaded (norms and subsets are computed on the device).  When the ids argument
+    (``userid`` / ``itemid``) is a 1-D int32 / int64 CUDA array, ``(ids, scores)`` come back as CUDA arrays
+    (``__cuda_array_interface__`` v3, shape (n, N), complete when returned, outliving the model), and ``filter_items``,
+    ``items`` and the ``similar_*`` subsets may be host or CUDA arrays.  Host ids (scalars, lists, numpy arrays) are
+    checked and converted as numpy does, in the same order and with the same errors, uploaded, and the results come
+    back as numpy arrays (1-D for a scalar id), bitwise those of the CUDA-id call for the same values.  A host-id
+    ``similar_*`` call therefore neither downloads device-resident factors nor fills the ``user_norms`` /
+    ``item_norms`` caches.
     Refitting on the device: when ``userids`` / ``itemids`` of ``partial_fit_users`` / ``partial_fit_items`` is a 1-D
     int32 / int64 CUDA array, the rows are solved, the factor matrix grown (new rows zero) and the rows stored on the
     device, the last occurrence of a repeated id winning as in numpy; no factor matrix crosses PCIe and the host copy is
@@ -626,35 +629,27 @@ class AlternatingLeastSquares:
     def partial_fit_users(self, userids, user_items):
         """implicit/cpu/als.py:267-307.  With userids a 1-D int32 / int64 CUDA array the rows are refitted in place on
         the device (_partial_fit_device)."""
-        if is_cuda_array(userids):
-            return self._partial_fit_device("user", userids, user_items,
-                                            "user_items must contain 1 row for every user in userids")
-        if len(userids) != user_items.shape[0]:
-            raise ValueError("user_items must contain 1 row for every user in userids")
-        user_factors = self.recalculate_user(userids, user_items)
-        host = self.user_factors
-        users, factors = host.shape
-        max_userid = max(userids)
-        if max_userid >= users:
-            host = np.concatenate([host, np.zeros((max_userid - users + 1, factors), dtype=self.dtype)])
-        host[userids] = user_factors
-        self.user_factors = host
+        self._partial_fit("user", userids, user_items, "user_items must contain 1 row for every user in userids")
 
     def partial_fit_items(self, itemids, item_users):
         """implicit/cpu/als.py:309-349.  With itemids a 1-D int32 / int64 CUDA array, as partial_fit_users."""
-        if is_cuda_array(itemids):
-            return self._partial_fit_device("item", itemids, item_users,
-                                            "item_users must contain 1 row for every user in itemids")
-        if len(itemids) != item_users.shape[0]:
-            raise ValueError("item_users must contain 1 row for every user in itemids")
-        item_factors = self.recalculate_item(itemids, item_users)
-        host = self.item_factors
-        items, factors = host.shape
-        max_itemid = max(itemids)
-        if max_itemid >= items:
-            host = np.concatenate([host, np.zeros((max_itemid - items + 1, factors), dtype=self.dtype)])
-        host[itemids] = item_factors
-        self.item_factors = host
+        self._partial_fit("item", itemids, item_users, "item_users must contain 1 row for every user in itemids")
+
+    def _partial_fit(self, side, ids, matrix, count_message):
+        """partial_fit_* of one side: host ids with numpy's semantics (negative ids index from the end, the factors grow
+        to max(ids) + 1 rows), CUDA ids on the device."""
+        if is_cuda_array(ids):
+            return self._partial_fit_device(side, ids, matrix, count_message)
+        if len(ids) != matrix.shape[0]:
+            raise ValueError(count_message)
+        rows = getattr(self, f"recalculate_{side}")(ids, matrix)
+        host = self._get_host(side)
+        n, factors = host.shape
+        max_id = max(ids)
+        if max_id >= n:
+            host = np.concatenate([host, np.zeros((max_id - n + 1, factors), dtype=self.dtype)])
+        host[ids] = rows
+        self._set_host(side, host)
 
     def _partial_fit_device(self, side, ids_in, matrix, count_message):
         """partial_fit_* for ids in CUDA memory: the rows are recalculated on the device (the same solve, with the same
@@ -711,61 +706,98 @@ class AlternatingLeastSquares:
     # ------------------------------------------------------------------ recommend (cpu/matrix_factorization_base.py:35-96)
     def recommend(self, userid, user_items, N=10, filter_already_liked_items=True, filter_items=None,
                   recalculate_user=False, items=None):
-        """cpu/matrix_factorization_base.py:35-96.  With userid a 1-D int32 / int64 CUDA array the call runs on the
-        device and returns (ids, scores) in CUDA memory (see _recommend_device)."""
+        """cpu/matrix_factorization_base.py:35-96.  With userid a 1-D int32 / int64 CUDA array, (ids, scores) come back
+        in CUDA memory (see _recommend).  Host ids are checked here as numpy checks them and in the same order, uploaded
+        as int64, and the results downloaded: numpy arrays, 1-D for a scalar id, the ids in the dtype of np.array(items)
+        with `items`."""
         if is_cuda_array(userid):
-            return self._recommend_device(userid, user_items, N, filter_already_liked_items, filter_items,
-                                          recalculate_user, items)
-        device = is_device_csr(user_items)
+            return self._recommend(userid, user_items, N, filter_already_liked_items, filter_items, recalculate_user,
+                                   items)
+        self._check_user_items(user_items, 1 if np.isscalar(userid) else len(userid), filter_already_liked_items,
+                               recalculate_user)
+        rows = np.atleast_1d(np.asarray(userid)).astype(np.int64)
+        if not recalculate_user and rows.size and (rows.min() < 0 or rows.max() >= self._device_factors("user").rows):
+            raise IndexError("userid out of range")
+        subset = None
+        if items is not None:
+            if filter_items:  # numpy's own ValueError for an array of several ids
+                raise ValueError("Can't set both items and filter_items in recommend call")
+            subset = _host_subset(items, self._device_factors("item").rows,
+                                  "Some itemids in the items parameter in are not in the model")
+            if filter_already_liked_items and is_device_csr(user_items):
+                raise ValueError("recommend(..., items=...) filters liked items of a scipy CSR only, not of a CSR in "
+                                 "CUDA memory")
+        n_items = self._device_factors("item").rows if subset is None else len(subset)
+        if filter_items is not None:
+            filter_items = np.asarray(filter_items).ravel()
+            if filter_items.size and (filter_items.min() < 0 or filter_items.max() >= n_items):
+                raise IndexError("filter_items contains ids that are not in the model")
+            filter_items = filter_items.astype(np.int64)
+        if N < 0:  # numpy's, from the output allocation of the host top-k
+            raise ValueError("negative dimensions are not allowed")
+        if filter_already_liked_items and subset is None and user_items.shape[1] != n_items:
+            raise _lib.AlsError(_lib.ALS_E_INVALID, f"als_topk: liked has {user_items.shape[1]} columns for {n_items} items")
+        out = self._recommend(rows, user_items, N, filter_already_liked_items, filter_items, recalculate_user,
+                              None if subset is None else subset.astype(np.int64), host=True)
+        return _to_host(self.ctx, out, np.isscalar(userid), None if subset is None else subset.dtype)
+
+    @staticmethod
+    def _check_user_items(user_items, n_query, filter_already_liked_items, recalculate_user):
         if filter_already_liked_items or recalculate_user:
-            if not isinstance(user_items, csr_matrix) and not device:
+            if not isinstance(user_items, csr_matrix) and not is_device_csr(user_items):
                 raise ValueError("user_items needs to be a CSR sparse matrix")
-            user_count = 1 if np.isscalar(userid) else len(userid)
-            if user_items.shape[0] != user_count:
+            if user_items.shape[0] != n_query:
                 raise ValueError("user_items must contain 1 row for every user in userids")
 
+    def _recommend(self, userid, user_items, N, filter_already_liked_items, filter_items, recalculate_user, items,
+                   host=False):
+        """recommend() on the device: the ids, the subset, the liked remap and the outputs stay there, and no factor
+        matrix is downloaded.  userid, filter_items and items are host or CUDA arrays (_device_ids); user_items a scipy or
+        device CSR.  Returns (ids, scores), DeviceSnapshots of shape (len(userid), N): int32 ids (the subset's dtype with
+        `items`), float32 scores.  `host`: called by the host adapter, which has made numpy's checks of items and
+        filter_items (a filter numpy finds false may come with items) and downloads and frees the outputs at once (they
+        are pooled)."""
         ctx = self.ctx
         tmp = []
         try:
+            uid = self._device_ids(userid, "userid", tmp)
+            n_query = len(uid)
+            device = is_device_csr(user_items)
+            self._check_user_items(user_items, n_query, filter_already_liked_items, recalculate_user)
+            query_rows = None
             if recalculate_user:
-                q = np.atleast_2d(self.recalculate_user(userid, user_items))
-                queries = _lib.DeviceFactors.from_host(ctx, q)
+                queries = self._recalculate_device(n_query, user_items, "item", self.YtY)
                 tmp.append(queries)
-                query_rows, n_query = None, q.shape[0]
             else:
-                queries = self._device_factors("user")
-                query_rows = np.atleast_1d(np.asarray(userid)).astype(np.int64)
-                if query_rows.size and (query_rows.min() < 0 or query_rows.max() >= queries.rows):
-                    raise IndexError("userid out of range")
-                n_query = len(query_rows)
-
+                queries, query_rows = self._device_factors("user"), uid
             item_handle = self._device_factors("item")
-            n_items_model = item_handle.rows
+            subset = None
             if items is not None:
-                N = min(N, len(items))
-                if filter_items:
+                N = min(N, _ids_len(items, "items"))
+                if not host and filter_items is not None and _ids_len(filter_items, "filter_items"):
                     raise ValueError("Can't set both items and filter_items in recommend call")
-                items = np.array(items)
-                items.sort()
-                if items.max() >= n_items_model or items.min() < 0:
+                if _ids_len(items, "items") == 0:
+                    raise ValueError("zero-size array to reduction operation maximum which has no identity")
+                subset = self._device_ids(items, "items", tmp, sort=True)
+                item_handle = _lib.DeviceFactors.gather_rows(ctx, item_handle, subset)
+                if item_handle is None:
                     raise IndexError("Some itemids in the items parameter in are not in the model")
-                item_handle = _lib.DeviceFactors.from_host(ctx, self.item_factors[items])
                 tmp.append(item_handle)
 
             fq = None
             batches = [(0, n_query)]
             if filter_already_liked_items and device:
-                if items is not None:
-                    raise ValueError("recommend(..., items=...) filters liked items of a scipy CSR only, not of a CSR in "
-                                     "CUDA memory")
                 fq = _lib.DeviceCSR.from_device(ctx, user_items)  # unsorted rows are sorted on the device
                 tmp.append(fq)
                 if fq.shape3[2] > _LIKED_NNZ_MAX:
                     raise ValueError(f"a liked filter in CUDA memory holds at most {_LIKED_NNZ_MAX} nonzeros")
+                if subset is not None:
+                    fq = fq.restrict_columns(subset)
+                    tmp.append(fq)
             elif filter_already_liked_items:
                 fq = user_items
-                if items is not None:
-                    fq = _filter_items_from_sparse_matrix(items, fq)
+                if subset is not None:  # liked ids remapped to positions in the subset; only its ids come to the host
+                    fq = _filter_items_from_sparse_matrix(_lib.ids_download(ctx, subset), fq)
                 if not fq.has_sorted_indices:
                     fq = fq.sorted_indices()
                 if fq.nnz > _LIKED_NNZ_MAX:
@@ -773,35 +805,31 @@ class AlternatingLeastSquares:
 
             fl = None
             if filter_items is not None:
-                fl = np.asarray(filter_items).ravel()
-                if fl.size and (fl.min() < 0 or fl.max() >= item_handle.rows):
-                    raise IndexError("filter_items contains ids that are not in the model")
-
-            parts = []
+                fl = self._device_ids(filter_items, "filter_items", tmp)
+            stream = self._one_stream(uid, fl, subset)
+            N = int(N)
+            ids = _lib.DeviceSnapshot(ctx, (n_query, N), f"<i{4 if subset is None else subset.itemsize}", pooled=host)
+            scores = _lib.DeviceSnapshot(ctx, (n_query, N), "<f4", pooled=host)
             for b0, b1 in batches:
-                qr = query_rows
-                if len(batches) > 1:
-                    qr = query_rows[b0:b1] if query_rows is not None else np.arange(b0, b1)
                 liked = None
                 if device and fq is not None:
                     liked = fq
                 elif fq is not None:
                     liked = _lib.DeviceCSR.upload(ctx, fq if len(batches) == 1 else fq[b0:b1])
                     tmp.append(liked)
-                parts.append(_lib.topk(ctx, item_handle, queries, int(N), query_rows=qr, n_query=b1 - b0,
-                                       liked=liked, filter_items=fl))
-                if liked is not None:
+                qr = None if query_rows is None else _slice(query_rows, b0, b1)
+                bad = _lib.topk_into(ctx, item_handle, queries, N, b1 - b0, ids.cuda(b0), scores.cuda(b0),
+                                     query_rows=qr, query_row0=b0 if qr is None and len(batches) > 1 else 0,
+                                     liked=liked, filter_items=fl, id_map=subset, stream=stream)
+                if bad & 1:
+                    raise IndexError("userid out of range")
+                if bad:
+                    raise IndexError("filter_items contains ids that are not in the model")
+                if liked is not None and not device:
                     liked.close()
-            ids, scores = parts[0] if len(parts) == 1 else (np.concatenate([p[0] for p in parts]),
-                                                             np.concatenate([p[1] for p in parts]))
         finally:
             for t in tmp:
                 t.close()
-
-        if np.isscalar(userid):
-            ids, scores = ids[0], scores[0]
-        if items is not None:
-            ids = items[ids]
         return ids, scores
 
     def _ranking_sums(self, userids, user_items, test_items, K, gain, gain_sum):
@@ -852,59 +880,7 @@ class AlternatingLeastSquares:
             self._item_norms = n
         return self._item_norms
 
-    def _similar(self, side, ids_in, N, recalculate, filter_ids, subset):
-        """recalculate: (item_users,) for similar_items(recalculate_item=True), else None.  With ids_in a 1-D int32 /
-        int64 CUDA array the call runs on the device (_similar_device)."""
-        if is_cuda_array(ids_in):
-            return self._similar_device(side, ids_in, N, recalculate, filter_ids, subset)
-        recalculated = None if recalculate is None else self.recalculate_item(ids_in, recalculate[0])
-        ctx = self.ctx
-        handle = self._device_factors(side)
-        norms = self.user_norms if side == "user" else self.item_norms
-        host = self.user_factors if side == "user" else self.item_factors
-        tmp = []
-        try:
-            if recalculated is not None:
-                factor = recalculated
-                if np.isscalar(ids_in):
-                    norm = np.linalg.norm(factor)
-                    norm = norm if norm != 0 else 1e-10
-                else:
-                    norm = np.linalg.norm(factor, axis=1)
-                    norm[norm == 0] = 1e-10
-                queries = _lib.DeviceFactors.from_host(ctx, np.atleast_2d(factor))
-                tmp.append(queries)
-                query_rows, n_query = None, queries.rows
-            else:
-                norm = norms[ids_in]
-                queries = handle
-                query_rows = np.atleast_1d(np.asarray(ids_in)).astype(np.int64)
-                n_query = len(query_rows)
-            target, tnorms = handle, norms
-            if subset is not None:
-                if filter_ids:
-                    raise ValueError("Can't set both a subset and a filter in a similar_* call")
-                subset = np.array(subset)
-                if subset.max() >= host.shape[0] or subset.min() < 0:
-                    raise IndexError("Some ids in the subset parameter are not in the model")
-                target = _lib.DeviceFactors.from_host(ctx, host[subset])
-                tmp.append(target)
-                tnorms = norms[subset]
-            ids, scores = _lib.topk(ctx, target, queries, int(N), query_rows=query_rows, n_query=n_query,
-                                    item_norms=tnorms, filter_items=filter_ids)
-        finally:
-            for t in tmp:
-                t.close()
-        if np.isscalar(ids_in):
-            ids, scores = ids[0], scores[0]
-            scores = scores / np.float32(norm)
-        else:
-            scores = scores / np.asarray(norm, dtype=np.float32)[:, None]
-        if subset is not None:
-            ids = subset[ids]
-        return ids, scores
-
-    # ------------------------------------------------------------------ serving from CUDA ids
+    # ------------------------------------------------------------------ serving on the device
     def _device_norms(self, side):
         """The row norms of one side on the device (a DeviceSnapshot, bitwise the user_norms / item_norms properties),
         cached until the factors change; never downloads the factors."""
@@ -915,8 +891,8 @@ class AlternatingLeastSquares:
     def _device_ids(self, ids, what, tmp, sort=False):
         """The utils.CudaArray of an ids argument of a device call: a 1-D int32 / int64 CUDA array as it is (sorted into a
         copy when `sort`), or host ids (list, numpy) uploaded, sorted first when `sort`.  Uploads and sorted copies are
-        appended to `tmp`.  Host ids keep numpy's dtype (np.array of a list of ints is int64); other than int32 / int64
-        they are refused with ValueError."""
+        pooled temporaries, appended to `tmp`.  Host ids keep numpy's dtype (np.array of a list of ints is int64); other
+        than int32 / int64 they are refused with ValueError."""
         if is_cuda_array(ids):
             a = cuda_ids(ids, what)
             if not sort:
@@ -931,7 +907,7 @@ class AlternatingLeastSquares:
             raise ValueError(f"{what}: ids of dtype {a.dtype} (a call with ids in CUDA memory takes int32 or int64)")
         if sort:
             a.sort()
-        s = _lib.DeviceSnapshot.from_host(self.ctx, a)
+        s = _lib.DeviceSnapshot.from_host(self.ctx, a, pooled=True)
         tmp.append(s)
         return s.cuda()
 
@@ -943,114 +919,62 @@ class AlternatingLeastSquares:
             raise ValueError("the CUDA arrays of one call name different producer streams")
         return streams.pop() if streams else 0
 
-    def _recommend_device(self, userid, user_items, N, filter_already_liked_items, filter_items, recalculate_user,
-                          items):
-        """recommend() for userid in CUDA memory: the checks, the liked batches and the top-k of the host path, with the
-        ids, the subset, the liked remap and the outputs on the device, and no factor matrix downloaded.  Returns (ids,
-        scores), DeviceSnapshots of shape (len(userid), N): int32 ids (the subset's dtype with `items`), float32 scores,
-        bitwise the host path's for the same values.  filter_items / items may be host or CUDA arrays; user_items a
-        scipy or device CSR."""
-        ctx = self.ctx
-        uid = cuda_ids(userid, "userid")
-        n_query = len(uid)
-        device = is_device_csr(user_items)
-        if filter_already_liked_items or recalculate_user:
-            if not isinstance(user_items, csr_matrix) and not device:
-                raise ValueError("user_items needs to be a CSR sparse matrix")
-            if user_items.shape[0] != n_query:
-                raise ValueError("user_items must contain 1 row for every user in userids")
-        tmp = []
-        try:
-            query_rows = None
-            if recalculate_user:
-                queries = self._recalculate_device(n_query, user_items, "item", self.YtY)
-                tmp.append(queries)
-            else:
-                queries, query_rows = self._device_factors("user"), uid
-            item_handle = self._device_factors("item")
-            subset = None
-            if items is not None:
-                N = min(N, _ids_len(items, "items"))
-                if filter_items is not None and _ids_len(filter_items, "filter_items"):
-                    raise ValueError("Can't set both items and filter_items in recommend call")
-                if _ids_len(items, "items") == 0:
-                    raise ValueError("zero-size array to reduction operation maximum which has no identity")
-                subset = self._device_ids(items, "items", tmp, sort=True)
-                item_handle = _lib.DeviceFactors.gather_rows(ctx, item_handle, subset)
-                if item_handle is None:
-                    raise IndexError("Some itemids in the items parameter in are not in the model")
-                tmp.append(item_handle)
+    def _similar_host(self, side, ids_in, N, recalculate, filter_ids, subset):
+        """_similar for host ids, checked as numpy checks them and in the same order, uploaded as int64, the results
+        downloaded (numpy arrays, 1-D for a scalar id, the ids in the dtype of np.array(subset)).  Without a recalculation
+        an id past the rows raises numpy's IndexError and a negative one AlsError (when anything is ranked); filter ids
+        outside the rows ranked are ignored."""
+        rows = self._device_factors(side).rows
+        if recalculate is None:
+            _index_check(rows, ids_in)
+        if subset is not None:
+            if filter_ids:  # numpy's own ValueError for an array of several ids
+                raise ValueError("Can't set both a subset and a filter in a similar_* call")
+            subset = _host_subset(subset, rows, "Some ids in the subset parameter are not in the model")
+        if N < 0:  # numpy's, from the output allocation of the host top-k
+            raise ValueError("negative dimensions are not allowed")
+        query_rows = np.atleast_1d(np.asarray(ids_in)).astype(np.int64)
+        negative = query_rows < 0
+        if recalculate is None and negative.any() and N > 0:
+            raise _lib.AlsError(_lib.ALS_E_INVALID, f"topk: query row {query_rows[negative][0]} out of range")
+        query_rows[negative] += rows  # N == 0: nothing is ranked, and numpy indexed the norms from the end
+        if filter_ids is not None:
+            targets = rows if subset is None else len(subset)
+            filter_ids = np.asarray(filter_ids).ravel().astype(np.int32)
+            filter_ids = filter_ids[(filter_ids >= 0) & (filter_ids < targets)]
+        out = self._similar(side, query_rows, N, recalculate, filter_ids,
+                            None if subset is None else subset.astype(np.int64), scalar=np.isscalar(ids_in), host=True)
+        return _to_host(self.ctx, out, np.isscalar(ids_in), None if subset is None else subset.dtype)
 
-            fq = None
-            batches = [(0, n_query)]
-            if filter_already_liked_items and device:
-                fq = _lib.DeviceCSR.from_device(ctx, user_items)  # unsorted rows are sorted on the device
-                tmp.append(fq)
-                if fq.shape3[2] > _LIKED_NNZ_MAX:
-                    raise ValueError(f"a liked filter in CUDA memory holds at most {_LIKED_NNZ_MAX} nonzeros")
-                if subset is not None:
-                    fq = fq.restrict_columns(subset)
-                    tmp.append(fq)
-            elif filter_already_liked_items:
-                fq = user_items
-                if subset is not None:  # the remap of the host path; only the subset's ids come to the host
-                    fq = _filter_items_from_sparse_matrix(_lib.ids_download(ctx, subset), fq)
-                if not fq.has_sorted_indices:
-                    fq = fq.sorted_indices()
-                if fq.nnz > _LIKED_NNZ_MAX:
-                    batches = liked_batches(fq.indptr, _LIKED_NNZ_MAX)
-
-            fl = None
-            if filter_items is not None:
-                fl = self._device_ids(filter_items, "filter_items", tmp)
-            stream = self._one_stream(uid, fl, subset)
-            N = int(N)
-            ids = _lib.DeviceSnapshot(ctx, (n_query, N), f"<i{4 if subset is None else subset.itemsize}")
-            scores = _lib.DeviceSnapshot(ctx, (n_query, N), "<f4")
-            for b0, b1 in batches:
-                liked = None
-                if device and fq is not None:
-                    liked = fq
-                elif fq is not None:
-                    liked = _lib.DeviceCSR.upload(ctx, fq if len(batches) == 1 else fq[b0:b1])
-                    tmp.append(liked)
-                qr = None if query_rows is None else _slice(query_rows, b0, b1)
-                bad = _lib.topk_into(ctx, item_handle, queries, N, b1 - b0, ids.cuda(b0), scores.cuda(b0),
-                                     query_rows=qr, query_row0=b0 if qr is None and len(batches) > 1 else 0,
-                                     liked=liked, filter_items=fl, id_map=subset, stream=stream)
-                if bad & 1:
-                    raise IndexError("userid out of range")
-                if bad:
-                    raise IndexError("filter_items contains ids that are not in the model")
-                if liked is not None and not device:
-                    liked.close()
-        finally:
-            for t in tmp:
-                t.close()
-        return ids, scores
-
-    def _similar_device(self, side, ids_in, N, recalculate, filter_ids, subset):
-        """_similar for ids in CUDA memory: the host path's top-k with the norms computed on the device (bitwise the
-        user_norms / item_norms properties), a subset gathered on the device (kept unsorted, duplicates included, and
-        N not clamped, as on the host) and the query norms divided out in the top-k's epilogue.  Returns DeviceSnapshots
-        (ids, scores) of shape (len(ids_in), N), like _recommend_device.  An id of filter_ids outside the model raises
-        IndexError (the host path ignores it)."""
+    def _similar(self, side, ids_in, N, recalculate, filter_ids, subset, scalar=False, host=False):
+        """similar_* on the device: the norms computed there (bitwise the user_norms / item_norms properties), a subset
+        gathered there (kept unsorted, duplicates included, and N not clamped) and the query norms divided out in the
+        top-k's epilogue.  ids_in, filter_ids and subset are host or CUDA arrays (_device_ids); recalculate is
+        (item_users,) for similar_items(recalculate_item=True), else None, and `scalar` a recalculation of one host id,
+        whose norm numpy takes as a dot product.  Returns DeviceSnapshots (ids, scores) of shape (len(ids_in), N); `host`
+        as for _recommend.  An id of filter_ids outside the model raises IndexError."""
         ctx = self.ctx
         what = f"{side}id"
-        qa = cuda_ids(ids_in, what)
         tmp = []
         try:
+            qa = self._device_ids(ids_in, what, tmp)
             handle = self._device_factors(side)
             if recalculate is not None:
                 queries = self._recalculate_device(len(qa), recalculate[0], "user", self.XtX)
                 tmp.append(queries)
-                query_rows, qnorms = None, queries.row_norms()
+                if scalar:
+                    norm = np.linalg.norm(queries.download()[0])
+                    qnorms = _lib.DeviceSnapshot.from_host(ctx, np.array([norm if norm != 0 else 1e-10], np.float32),
+                                                           pooled=True)
+                else:
+                    qnorms = queries.row_norms()
                 tmp.append(qnorms)
+                query_rows = None
             else:
                 queries, query_rows, qnorms = handle, qa, self._device_norms(side)
             target, tnorms, sub = handle, self._device_norms(side), None
             if subset is not None:
-                if filter_ids is not None and _ids_len(filter_ids, f"filter_{side}s"):
+                if not host and filter_ids is not None and _ids_len(filter_ids, f"filter_{side}s"):
                     raise ValueError("Can't set both a subset and a filter in a similar_* call")
                 if _ids_len(subset, "items" if side == "item" else "users") == 0:
                     raise ValueError("zero-size array to reduction operation maximum which has no identity")
@@ -1066,8 +990,8 @@ class AlternatingLeastSquares:
                 fl = self._device_ids(filter_ids, f"filter_{side}s", tmp)
             stream = self._one_stream(qa, fl, sub)
             N = int(N)
-            ids = _lib.DeviceSnapshot(ctx, (len(qa), N), f"<i{4 if sub is None else sub.itemsize}")
-            scores = _lib.DeviceSnapshot(ctx, (len(qa), N), "<f4")
+            ids = _lib.DeviceSnapshot(ctx, (len(qa), N), f"<i{4 if sub is None else sub.itemsize}", pooled=host)
+            scores = _lib.DeviceSnapshot(ctx, (len(qa), N), "<f4", pooled=host)
             bad = _lib.topk_into(ctx, target, queries, N, len(qa), ids.cuda(), scores.cuda(), query_rows=query_rows,
                                  item_norms=tnorms, query_norms=qnorms, filter_items=fl, id_map=sub, stream=stream)
             if bad & 1:
@@ -1080,10 +1004,12 @@ class AlternatingLeastSquares:
         return ids, scores
 
     def similar_items(self, itemid, N=10, recalculate_item=False, item_users=None, filter_items=None, items=None):
-        return self._similar("item", itemid, N, (item_users,) if recalculate_item else None, filter_items, items)
+        serve = self._similar if is_cuda_array(itemid) else self._similar_host
+        return serve("item", itemid, N, (item_users,) if recalculate_item else None, filter_items, items)
 
     def similar_users(self, userid, N=10, filter_users=None, users=None):
-        return self._similar("user", userid, N, None, filter_users, users)
+        serve = self._similar if is_cuda_array(userid) else self._similar_host
+        return serve("user", userid, N, None, filter_users, users)
 
     # ------------------------------------------------------------------ persistence (cpu/als.py:458-477, recommender_base.py:173-202)
     def save(self, fileobj_or_path):
@@ -1153,3 +1079,32 @@ def _slice(a, b0, b1):
 def _ids_len(ids, what):
     """The number of ids of a host or CUDA ids argument."""
     return len(cuda_ids(ids, what)) if is_cuda_array(ids) else int(np.asarray(ids).size)
+
+
+def _index_check(rows, ids):
+    """Raises the IndexError numpy raises when `ids` index an array of `rows` rows, if any: ids past the rows, float
+    ids."""
+    np.broadcast_to(np.int8(0), (rows,))[ids]
+
+
+def _host_subset(ids, rows, message):
+    """np.array(ids) of a host subset, checked in numpy's order: ValueError when it is empty (its max), IndexError(message)
+    for ids outside [0, rows), then numpy's IndexError for ids that cannot index (_index_check)."""
+    a = np.array(ids)
+    if a.max() >= rows or a.min() < 0:
+        raise IndexError(message)
+    _index_check(rows, a)
+    return a
+
+
+def _to_host(ctx, out, scalar, ids_dtype=None):
+    """The (ids, scores) DeviceSnapshots of a serving call as numpy arrays, the snapshots freed: 1-D for a scalar id, the
+    ids cast to `ids_dtype` (a host subset's own dtype, which holds every id of the subset)."""
+    ids, scores = (_lib.ids_download(ctx, CudaArray(s.ptr.value, (s.shape[0] * s.shape[1],), s.itemsize, 1, 0))
+                   .reshape(s.shape) for s in out)
+    for s in out:
+        s.close()
+    scores = scores.view(np.float32)
+    if ids_dtype is not None:
+        ids = ids.astype(ids_dtype, copy=False)
+    return (ids[0], scores[0]) if scalar else (ids, scores)

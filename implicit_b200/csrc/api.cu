@@ -1172,6 +1172,20 @@ ALS_API int als_device_free(als_ctx *ctx, void *ptr) {
   return ALS_OK;
 }
 
+ALS_API int als_pool_alloc(als_ctx *ctx, int64_t bytes, void **ptr) {
+  ALS_REQUIRE(ctx && ptr && bytes >= 0, "als_pool_alloc: bad argument");
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  return dev_alloc(ctx, ptr, bytes);
+}
+
+ALS_API int als_pool_free(als_ctx *ctx, void *ptr) {
+  ALS_REQUIRE(ctx, "als_pool_free: ctx is NULL");
+  if (!ptr) return ALS_OK;
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  dev_free(ctx, ptr);
+  return ALS_OK;
+}
+
 ALS_API int als_factors_has_nan(als_ctx *ctx, const als_factors *f, int *has_nan) {
   ALS_REQUIRE(ctx && f && has_nan, "als_factors_has_nan: NULL argument");
   ALS_CUDA(cudaSetDevice(ctx->device));

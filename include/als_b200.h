@@ -205,6 +205,11 @@ int als_factors_export_device(als_ctx *ctx, const als_factors *f, float *dst, in
  * cudaFree.  cudaFree waits for the device, so work of any stream that still reads the block finishes first. */
 int als_device_alloc(als_ctx *ctx, int64_t bytes, void **ptr);
 int als_device_free(als_ctx *ctx, void *ptr);
+/* Device memory from the context's stream-ordered pool (cudaMallocAsync / cudaFreeAsync on its stream), for
+ * temporaries that only the library's calls on this context read: the free is ordered after the work queued so far on
+ * the context's stream, not after other streams' work, and does not wait for the device. */
+int als_pool_alloc(als_ctx *ctx, int64_t bytes, void **ptr);
+int als_pool_free(als_ctx *ctx, void *ptr);
 int als_factors_shape(const als_factors *f, int64_t *rows, int *factors, int *stride);
 /* *has_nan = 1 if any element is NaN (device-side scan).  Replaces the host np.isnan pass of
  * RecommenderBase._check_factors, implicit/recommender_base.py:218-223. */

@@ -1,6 +1,7 @@
-"""recommend, rank_items and similar_* with their ids in CUDA memory: the call runs on the device and hands back CUDA
-arrays, bitwise the host path's ids and scores for the same values (numpy ids, a scipy liked filter of the same float32
-entries).  PyTorch plays the producer; the package itself never imports it.
+"""recommend, rank_items and similar_* with their ids in CUDA memory: the call hands back CUDA arrays, bitwise the ids
+and scores of the same call with numpy ids (which goes through the host adapter; a scipy liked filter of the same
+float32 entries).  tests/test_gpu_serving_golden.py ties the numpy-id calls to recorded results.  PyTorch plays the
+producer; the package itself never imports it.
 """
 import gc
 import os

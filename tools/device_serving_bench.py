@@ -9,9 +9,8 @@ them over.  Timed, each call from its inputs where a user would hold them to its
 them, ending in a device synchronise (host clock):
   recommend  67,584 users, k = 10, their liked rows as a scipy CSR.  numpy: numpy ids in, numpy (ids, scores) out.
              torch: torch ids in, the CUDA outputs wrapped by torch.as_tensor.
-  similar    similar_items of 10,000 items, N = 10.  "first": the first call after the factors were assigned (the numpy
-             path downloads the item factors and computes the norms on the host; the torch path computes them on the
-             device), re-assigned before every rep; "steady": the call again, norms cached.
+  similar    similar_items of 10,000 items, N = 10.  "first": the first call after the factors were assigned (both
+             compute the norms on the device), re-assigned before every rep; "steady": the call again, norms cached.
 Every path is warmed up once; the paths alternate --reps times and the medians are reported in ms, with the card name
 and power limit read in the same run, as one JSON line (and DIR/device_serving_bench.json).  Each pair of paths must
 give bitwise the same ids and scores.
