@@ -38,28 +38,21 @@ void dev_free(als_ctx *ctx, void *ptr) {
   if (ptr) cudaFreeAsync(ptr, ctx->stream);
 }
 
-// Builds the schedule of a device-transposed CSR from the indptr copy that csr_transpose left in flight, or the
-// schedules of a CSR laid out without them from its device indptrs.
+// Builds the schedules of a CSR laid out without them (csr_layout's schedule = false) from its device indptrs.
 int ensure_schedule(als_ctx *ctx, als_csr *csr) {
-  if (csr->sched_lazy) {
-    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::vector<int32_t> ip;
-    csr->max_row_nnz = 0;
-    for (const als_csr *S : segments_of(csr)) {
-      ip.resize((size_t)S->rows + 1);
-      ALS_CUDA(cudaMemcpy(ip.data(), S->indptr, sizeof(int32_t) * ip.size(), cudaMemcpyDeviceToHost));
-      int rc = build_schedule(ctx, const_cast<als_csr *>(S), ip.data());
-      if (rc != ALS_OK) return rc;
-      csr->max_row_nnz = std::max(csr->max_row_nnz, S->max_row_nnz);
-    }
-    csr->sched_lazy = false;
-    return ALS_OK;
+  if (!csr->sched_lazy) return ALS_OK;
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  std::vector<int32_t> ip;
+  csr->max_row_nnz = 0;
+  for (const als_csr *S : segments_of(csr)) {
+    ip.resize((size_t)S->rows + 1);
+    ALS_CUDA(cudaMemcpy(ip.data(), S->indptr, sizeof(int32_t) * ip.size(), cudaMemcpyDeviceToHost));
+    int rc = build_schedule(ctx, const_cast<als_csr *>(S), ip.data());
+    if (rc != ALS_OK) return rc;
+    csr->max_row_nnz = std::max(csr->max_row_nnz, S->max_row_nnz);
   }
-  if (!csr->sched_pending) return ALS_OK;
-  ALS_CUDA(cudaEventSynchronize(ctx->sched_ev));
-  csr->sched_pending = false;
-  ctx->sched_owner = nullptr;
-  return build_schedule(ctx, csr, ctx->sched_pinned);
+  csr->sched_lazy = false;
+  return ALS_OK;
 }
 
 int ensure_scratch(als_ctx *ctx, int64_t bytes) {
@@ -297,8 +290,8 @@ int build_schedule(als_ctx *ctx, als_csr *csr, const int32_t *indptr) {
   }
   csr->n_finish = (int64_t)fin.size();
   csr->n_slots = slots;
-  // The lists are allocated and uploaded on the copy stream: when the schedule of a transposed matrix is built
-  // lazily, a half-iteration is already running on the compute stream and must not delay them (nor they it).
+  // The lists are allocated and uploaded on the copy stream: when the schedule of a transposed matrix is built, its
+  // sort is still running on the compute stream and must not delay them (nor they it).
   cudaStream_t up = ctx->copy;
   int rc;
   if (csr->n_work) {
@@ -424,7 +417,6 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->class_fork, cudaEventDisableTiming));
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
   ALS_CUDA(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
-  ALS_CUDA(cudaEventCreateWithFlags(&ctx->sched_ev, cudaEventDisableTiming));
   for (int k = 0; k < 2; ++k) {
     ALS_CUDA(cudaEventCreateWithFlags(&ctx->ring_loaded[k], cudaEventDisableTiming));
     ALS_CUDA(cudaEventCreateWithFlags(&ctx->ring_free[k], cudaEventDisableTiming));
@@ -526,8 +518,6 @@ ALS_API int als_ctx_destroy(als_ctx *ctx) {
     }
     cudaEventDestroy(ctx->stage_ready);
   }
-  if (ctx->sched_pinned) cudaFreeHost(ctx->sched_pinned);
-  cudaEventDestroy(ctx->sched_ev);
   for (int k = 0; k < 2; ++k) {
     cudaEventDestroy(ctx->ring_loaded[k]);
     cudaEventDestroy(ctx->ring_free[k]);
@@ -1021,10 +1011,6 @@ ALS_API int als_csr_destroy(als_csr *csr) {
   als_ctx *ctx = csr->ctx;
   if (ctx) {
     cudaSetDevice(ctx->device);
-    if (ctx->sched_owner == csr) {  // its indptr copy may still be in flight into the shared pinned buffer
-      cudaEventSynchronize(ctx->sched_ev);
-      ctx->sched_owner = nullptr;
-    }
     // stream-ordered frees: everything queued so far on the compute stream (which every other stream is joined
     // into before an entry point returns) still sees the arrays
     if (csr->owns && csr->host) {
@@ -1292,7 +1278,7 @@ static int check_half(const char *who, als_ctx *ctx, const als_csr *C, const als
               (long long)Y->rows);
   ALS_REQUIRE(C->row_offset + C->rows <= X->rows, "%s: C rows [%lld, %lld) exceed X's %lld rows", who,
               (long long)C->row_offset, (long long)(C->row_offset + C->rows), (long long)X->rows);
-  return ensure_schedule(ctx, const_cast<als_csr *>(C));  // a device-transposed matrix sorts its rows at first use
+  return ensure_schedule(ctx, const_cast<als_csr *>(C));
 }
 
 ALS_API int als_gramian_read(als_ctx *ctx, const als_factors *Y, float *G_host) {
@@ -1647,7 +1633,7 @@ ALS_API int als_csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const v
   ALS_REQUIRE(ctx && liked && out && (subset || m == 0), "%s: NULL argument", who);
   ALS_REQUIRE(subset_bytes == 4 || subset_bytes == 8, "%s: subset_bytes must be 4 or 8, got %d", who, subset_bytes);
   ALS_REQUIRE(m >= 0 && m < (int64_t)INT32_MAX, "%s: a subset of %lld ids", who, (long long)m);
-  ALS_REQUIRE(!liked->host && liked->segs.empty() && !liked->sched_pending,
+  ALS_REQUIRE(!liked->host && liked->segs.empty(),
               "%s: the liked CSR must be one device-resident CSR of fewer than 2^31 - 1 nonzeros", who);
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));

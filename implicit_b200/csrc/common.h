@@ -115,11 +115,6 @@ struct als_ctx {
   cudaStream_t stage_stream[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t stage_ev[4][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
   cudaEvent_t stage_ready = nullptr;
-  // a transposed CSR whose schedule has not been built yet (csr.cu): its indptr lands here, asynchronously
-  struct als_csr *sched_owner = nullptr;
-  int32_t *sched_pinned = nullptr;
-  int64_t sched_pinned_cap = 0;
-  cudaEvent_t sched_ev = nullptr;
   // the two-slot device ring that streams the segments of a host-resident CSR (csr.cu for_each_segment): a slot is
   // loaded (ring_loaded, on the copy stream) and free again once every launch that read it has finished (ring_free)
   cudaEvent_t ring_loaded[2] = {nullptr, nullptr}, ring_free[2] = {nullptr, nullptr};
@@ -161,7 +156,6 @@ struct als_csr {
   unsigned *wmax_dev = nullptr;  // device: [0] bits of max | |c| - 1 | over the values, [1] != 0 when some |c| < 1 (cholesky.cu), computed lazily
   bool wmax_valid = false;
   bool neg_w_known = false, has_neg_w = false;  // host copy of wmax_dev[1]: weights |c| - 1 < 0 exist (then no wgmma long-row path)
-  bool sched_pending = false;  // transposed on the device: the schedule is built at first use (ensure_schedule)
   // laid out without schedules (the pieces of a sharded transpose, which are only copied): ensure_schedule builds them
   // from the device indptrs at the first solve
   bool sched_lazy = false;

@@ -22,38 +22,7 @@ __global__ void iota_kernel(int32_t *v, int64_t n) {
   for (; i < n; i += stride) v[i] = (int32_t)i;
 }
 
-// For each sorted entry j: the row of the original entry e = perm[j] (binary search in indptr) and its value.
-__global__ void gather_transposed_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ indptr,
-                                         int rows, const float *__restrict__ data, int64_t nnz,
-                                         int32_t *__restrict__ out_indices, float *__restrict__ out_data) {
-  int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (; j < nnz; j += stride) {
-    const int32_t e = perm[j];
-    int lo = 0, hi = rows;  // largest r with indptr[r] <= e
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (indptr[mid] <= e) lo = mid; else hi = mid;
-    }
-    out_indices[j] = lo;
-    out_data[j] = data[e];
-  }
-}
-
-// out_indptr[c] = first position j with sorted_cols[j] >= c
-__global__ void indptr_from_sorted_kernel(const int32_t *__restrict__ sorted_cols, int64_t nnz, int cols,
-                                          int32_t *__restrict__ out_indptr) {
-  int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c > cols) return;
-  int64_t lo = 0, hi = nnz;  // first j in [0, nnz] with key >= c
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (sorted_cols[mid] < c) lo = mid + 1; else hi = mid;
-  }
-  out_indptr[c] = (int32_t)lo;
-}
-
-// ---- the transpose of a CSR held as row-block segments, device- or host-resident --------------------------------
+// ---- the transpose of a CSR, device- or host-resident, in one segment or many ------------------------------------
 // Peak memory of a device-resident transpose: input + output + O(piece).  Output positions are 64-bit: a column histogram over all segments, scanned
 // into the output indptr, gives every column its range; the input is then sorted in row pieces of bounded nnz, in row
 // order, each piece stably by column, and every entry goes to out_indptr[c] + (entries of column c in earlier pieces)
@@ -77,10 +46,11 @@ __device__ __forceinline__ int64_t first_of_key(const int32_t *__restrict__ keys
 
 // sorted entry j of a piece (perm[j]: its position after the piece's first nonzero, keys[j]: its column) -> its place
 // in the output.  indptr: the piece's rows in the segment's indptr (indptr[0] is the piece's first nonzero).  Only the
-// columns [c0, c1) are written, to out + (output position - out_base): a window of a host-resident output.
+// columns [c0, c1) are written, to out + (output position - out_base): a window of a host-resident output.  When the
+// piece is the whole input, j itself is the output position (next[c] is then the first j of column c).
 __global__ void scatter_piece_kernel(const int32_t *__restrict__ perm, const int32_t *__restrict__ keys, int64_t n,
                                      const int32_t *__restrict__ indptr, int rows, int64_t row0,
-                                     const float *__restrict__ data, const long long *__restrict__ next,
+                                     const float *__restrict__ data, const long long *__restrict__ next, bool whole,
                                      int32_t *__restrict__ out_indices, float *__restrict__ out_data, int32_t c0, int32_t c1,
                                      int64_t out_base) {
   int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -94,7 +64,7 @@ __global__ void scatter_piece_kernel(const int32_t *__restrict__ perm, const int
       const int mid = (lo + hi) >> 1;
       if (indptr[mid] - base <= e) lo = mid; else hi = mid;
     }
-    const int64_t dst = next[c] + (j - first_of_key(keys, n, c)) - out_base;
+    const int64_t dst = (whole ? j : next[c] + (j - first_of_key(keys, n, c))) - out_base;
     out_indices[dst] = (int32_t)(row0 + lo);
     out_data[dst] = data[e];
   }
@@ -133,8 +103,11 @@ int column_histogram(als_ctx *ctx, const als_csr *in, unsigned long long *count)
 
 // Writes the transpose of `in` into t->indices / t->data (t->rows, t->nnz and the arrays set) and its indptr, as
 // positions into them, into ip[0 .. cols]; the caller lays t out.  index_base is added to every output index: 0 numbers
-// the rows of `in` from its first row, in->row_offset gives the global rows of a shard.
-int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t index_base, std::vector<int64_t> &ip) {
+// the rows of `in` from its first row, in->row_offset gives the global rows of a shard.  Pieces hold at most piece_nnz
+// nonzeros unless a single row is longer.  It returns with the sorts and scatters still running, so that the caller's
+// host work (the layout and schedule of t) overlaps them.
+int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t index_base, int64_t piece_nnz,
+                        std::vector<int64_t> &ip) {
   const int64_t cols = in->cols;
   int end_bit = 1;
   while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
@@ -156,22 +129,26 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
   ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   dev_free(ctx, out_ip);
-  // pieces: whole rows of one segment, at most kPieceNnz nonzeros unless a single row is longer, cut from the segment
-  // indptrs (on the device for either residency)
+  // pieces: whole rows of one segment, cut from the segment indptrs (on the device for either residency)
   const std::vector<const als_csr *> segs = segments_of(in);
   struct Piece { int64_t r0, r1, b0, n; };
   std::vector<std::vector<Piece>> pieces(segs.size());
-  int64_t max_piece = 1, max_seg = 1;
+  int64_t max_piece = 1, max_seg = 1, npieces = 0;
   for (size_t s = 0; s < segs.size(); ++s) {
     const als_csr *S = segs[s];
-    std::vector<int32_t> sip((size_t)S->rows + 1);
-    ALS_CUDA(cudaMemcpy(sip.data(), S->indptr, sizeof(int32_t) * (S->rows + 1), cudaMemcpyDeviceToHost));
-    for (int64_t a = 0; a < S->rows;) {
-      int64_t b = std::upper_bound(sip.begin() + a + 1, sip.end(), (int64_t)sip[a] + kPieceNnz) - sip.begin() - 1;
+    // a segment of at most piece_nnz nonzeros is one piece, for which the first position is all of the indptr needed
+    std::vector<int32_t> sip(S->nnz > piece_nnz ? (size_t)S->rows + 1 : 1);
+    ALS_CUDA(cudaMemcpy(sip.data(), S->indptr, sizeof(int32_t) * sip.size(), cudaMemcpyDeviceToHost));
+    if (sip.size() == 1 && S->rows) pieces[s].push_back(Piece{0, S->rows, sip[0], S->nnz});
+    for (int64_t a = 0; sip.size() > 1 && a < S->rows;) {
+      int64_t b = std::upper_bound(sip.begin() + a + 1, sip.end(), (int64_t)sip[a] + piece_nnz) - sip.begin() - 1;
       b = std::max(b, a + 1);
       pieces[s].push_back(Piece{a, b, sip[a], (int64_t)sip[b] - sip[a]});
-      max_piece = std::max(max_piece, pieces[s].back().n);
       a = b;
+    }
+    for (const Piece &pc : pieces[s]) {
+      max_piece = std::max(max_piece, pc.n);
+      npieces += pc.n > 0;
     }
     max_seg = std::max(max_seg, S->nnz);
   }
@@ -218,7 +195,9 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
   for (const auto &w : windows) {
     const int64_t c0 = w.first, c1 = w.second, wn = ip[c1] - ip[c0];
     if (wn == 0) continue;
-    ALS_CUDA(cudaMemcpyAsync(next, ip.data(), sizeof(int64_t) * (cols + 1), cudaMemcpyHostToDevice, ctx->stream));
+    if (npieces > 1)  // a single piece finds its output positions without next
+      ALS_CUDA(cudaMemcpyAsync(next, ip.data(), sizeof(int64_t) * (cols + 1), cudaMemcpyHostToDevice, ctx->stream));
+    int64_t left = npieces;  // of this window's walk: no column advance after the last piece
     rc = for_each_segment(ctx, in, [&](size_t s, const als_csr *S) -> int {
       for (const Piece &pc : pieces[s]) {
         if (pc.n == 0) continue;
@@ -227,11 +206,14 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
         scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
             vals_out, keys_out, pc.n, S->indptr + pc.r0, (int)(pc.r1 - pc.r0),
             index_base + S->row_offset - in->row_offset + pc.r0,
-            S->data + pc.b0, next, out_indices, out_data, (int32_t)c0, (int32_t)c1, ip[c0]);
+            S->data + pc.b0, next, npieces == 1, out_indices, out_data, (int32_t)c0, (int32_t)c1, ip[c0]);
         ALS_CUDA(cudaGetLastError());
-        advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, pc.n, next);
-        ALS_CUDA(cudaGetLastError());
-        ctx->launches += 2;
+        ctx->launches++;
+        if (--left > 0) {
+          advance_columns_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys_out, pc.n, next);
+          ALS_CUDA(cudaGetLastError());
+          ctx->launches++;
+        }
       }
       return ALS_OK;
     });
@@ -542,11 +524,12 @@ int csr_layout(als_ctx *ctx, als_csr *c, const int64_t *ip, bool schedule) {
   std::vector<int32_t> ip32(ip, ip + c->rows + 1);
   int rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (c->rows + 1));
   if (rc != ALS_OK) return rc;
-  ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * ip32.size(), cudaMemcpyHostToDevice, ctx->stream));
   c->sched_lazy = !schedule;
-  if (schedule) rc = build_schedule(ctx, c, ip32.data());
+  // the schedule first: the copy from pageable memory below may wait for the work queued before it (a transpose's sort)
+  if (schedule && (rc = build_schedule(ctx, c, ip32.data())) != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(c->indptr, ip32.data(), sizeof(int32_t) * ip32.size(), cudaMemcpyHostToDevice, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `ip32` dies here
-  return rc;
+  return ALS_OK;
 }
 
 int csr_alloc(als_ctx *ctx, als_csr *c) {
@@ -580,84 +563,22 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
     return ALS_E_INVALID;
   }
   ALS_CUDA(cudaSetDevice(ctx->device));
-  const int64_t nnz = in->nnz;
-  const int rows = (int)in->rows, cols = (int)in->cols;
   als_csr *t = new als_csr();
   t->ctx = ctx;
-  t->rows = cols;
-  t->cols = rows;
-  t->nnz = nnz;
+  t->rows = in->cols;
+  t->cols = in->rows;
+  t->nnz = in->nnz;
   t->host = in->host;  // the transpose of a host-resident CSR is host-resident, built one column window at a time
+  // a device-resident CSR of one segment is sorted whole, as one piece: one sort, and no search of the output position
+  const int64_t piece_nnz = in->host || !in->segs.empty() ? kPieceNnz : std::max<int64_t>(in->nnz, 1);
+  std::vector<int64_t> ip;
   int rc;
-  if (in->host || !in->segs.empty() || needs_segments(ctx, nnz)) {
-    std::vector<int64_t> ip;
-    if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t, 0, ip)) != ALS_OK ||
-        (rc = csr_layout(ctx, t, ip.data())) != ALS_OK) {
-      cudaStreamSynchronize(ctx->stream);  // D2H copies of a window may still be landing in t's arrays
-      als_csr_destroy(t);
-      return rc;
-    }
-    *out = t;
-    return ALS_OK;
-  }
-  if ((rc = dev_alloc(ctx, (void **)&t->indptr, sizeof(int32_t) * ((int64_t)cols + 1))) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&t->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&t->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK) {
+  if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t, 0, piece_nnz, ip)) != ALS_OK ||
+      (rc = csr_layout(ctx, t, ip.data())) != ALS_OK) {
+    cudaStreamSynchronize(ctx->stream);  // D2H copies of a window may still be landing in t's arrays
     als_csr_destroy(t);
     return rc;
   }
-  // one pinned landing buffer per context: a transposed matrix whose schedule is still pending owns it
-  if (ctx->sched_owner && (rc = ensure_schedule(ctx, ctx->sched_owner)) != ALS_OK) {
-    als_csr_destroy(t);
-    return rc;
-  }
-  const int64_t need = sizeof(int32_t) * ((int64_t)cols + 1);
-  if (need > ctx->sched_pinned_cap) {
-    if (ctx->sched_pinned) ALS_CUDA(cudaFreeHost(ctx->sched_pinned));
-    ctx->sched_pinned = nullptr;
-    ctx->sched_pinned_cap = 0;
-    ALS_CUDA(cudaMallocHost((void **)&ctx->sched_pinned, (size_t)need));
-    ctx->sched_pinned_cap = need;
-  }
-  if (nnz > 0) {
-    int32_t *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr;
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    int end_bit = 1;
-    while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
-    ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, in->indices, keys_out, vals_in, vals_out, (int)nnz, 0,
-                                             end_bit, ctx->stream));
-    if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * nnz)) != ALS_OK ||
-        (rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) {
-      als_csr_destroy(t);
-      return rc;
-    }
-    iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, nnz);
-    ALS_CUDA(cudaGetLastError());
-    ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, in->indices, keys_out, vals_in, vals_out, (int)nnz, 0,
-                                             end_bit, ctx->stream));
-    gather_transposed_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(vals_out, in->indptr, rows, in->data, nnz,
-                                                                        t->indices, t->data);
-    ALS_CUDA(cudaGetLastError());
-    indptr_from_sorted_kernel<<<(cols + 1 + 255) / 256, 256, 0, ctx->stream>>>(keys_out, nnz, cols, t->indptr);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches += 3;
-    dev_free(ctx, keys_out);  // stream ordered: after the kernels above
-    dev_free(ctx, vals_in);
-    dev_free(ctx, vals_out);
-    dev_free(ctx, tmp);
-  } else {
-    ALS_CUDA(cudaMemsetAsync(t->indptr, 0, sizeof(int32_t) * ((int64_t)cols + 1), ctx->stream));
-  }
-  // The schedule needs the row lengths on the host.  The copy is left in flight and the schedule is built at the
-  // first solve over this matrix (ensure_schedule): in a fit that is the item half, so the host-side sort of the
-  // rows overlaps the user half that is already running instead of leaving the GPU idle.
-  ALS_CUDA(cudaMemcpyAsync(ctx->sched_pinned, t->indptr, (size_t)need, cudaMemcpyDeviceToHost, ctx->stream));
-  ALS_CUDA(cudaEventRecord(ctx->sched_ev, ctx->stream));
-  t->sched_pending = true;
-  ctx->sched_owner = t;
   *out = t;
   return ALS_OK;
 }
@@ -690,7 +611,7 @@ int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *
   t->nnz = in->nnz;
   std::vector<int64_t> ip;
   int rc = csr_alloc(ctx, t);
-  if (rc == ALS_OK) rc = transpose_segmented(ctx, in, t, in->row_offset, ip);
+  if (rc == ALS_OK) rc = transpose_segmented(ctx, in, t, in->row_offset, kPieceNnz, ip);
   for (int q = 0; q < n && rc == ALS_OK; ++q) {
     const int64_t r0 = col_bounds[q], r1 = col_bounds[q + 1];
     als_csr *p = new als_csr();

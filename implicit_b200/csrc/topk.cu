@@ -653,7 +653,6 @@ int topk_device(als_ctx *ctx, const als_factors *items, const als_factors *queri
   // Large batches at 64 padded factors go to the wgmma kernel (topk_tc.cu).  It skips filtered items instead of
   // keeping them at -FLT_MAX, which is the same thing as long as every row has k unfiltered items left.
   const bool use_tc = !ctx->knobs.topk_legacy && topk_tc_eligible(items->ld, n_query, I, k_eff, item_norms != nullptr) &&
-                      (!liked || !liked->sched_pending) &&
                       I - n_filter - (liked ? liked->max_row_nnz : 0) >= k_eff;
   const int64_t o_tc = take(use_tc ? topk_tc_scratch_bytes(n_query, I) : 0);
   int rc = ensure_scratch(ctx, off);

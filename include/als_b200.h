@@ -145,7 +145,7 @@ int als_csr_generate(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz_targe
 int als_factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale);
 
 /* Device transpose: out = in^T as CSR (replaces the host `Cui.T.tocsr()`, implicit/cpu/als.py:137).
- * Asynchronous: the launch schedule of `out` is built at the first solve that uses it. */
+ * Returns `out` with its launch schedule, built on the host while the device sorts. */
 int als_csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out);
 /* A view of rows [r0, r1) of `in` as a shard (row_offset = r0) with its own schedule; shares the
  * parent's device arrays, so the parent must outlive it.  The view of a segmented CSR is segmented itself; its shape

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from helpers import KNOB_DEFAULTS, mixed_csr
+from implicit_b200.utils import CudaArray
 
 pytestmark = pytest.mark.gpu
 KNOBS = dict(KNOB_DEFAULTS, segment_nnz=0, host_csr=0)
@@ -135,3 +136,82 @@ def test_refusals(lib, ctx, C, entry):
     for (ip, nnz), want in cases:
         rc, _, msg = call_upload(lib, ctx, entry, C.shape[0], C.shape[1], nnz, ip, C.indices, C.data, 0)
         assert rc == lib.ALS_E_INVALID and msg == want
+
+
+EDGES = ["nnz0", "rows0", "cols1", "cols65536", "cols65537", "column3072", "column3073", "unsorted"]
+
+
+def edge_csr(name):
+    """A CSR at an edge of the transpose of a one-segment device CSR: no entries, no rows, one column, the column counts
+    around 2^16 where the radix sort takes one more bit, a column of 3072 entries (the longest transposed row the
+    schedule keeps whole) or 3073 (chunked), else 4000 random entries.  Each row keeps its entries in the order drawn:
+    unsorted, with repeated columns."""
+    import scipy.sparse as sp
+
+    rng = np.random.default_rng(5)
+    rows, cols, n = (3200 if name.startswith("column") else 500), 300, 4000
+    if name in ("nnz0", "rows0"):
+        rows, n = (0 if name == "rows0" else rows), 0
+    elif name.startswith("cols"):
+        cols = int(name[4:])
+    r, c = (rng.integers(0, rows, n), rng.integers(0, cols, n)) if n else (np.zeros(0, np.int64), np.zeros(0, np.int64))
+    if name.startswith("cols"):
+        c[0] = cols - 1
+    elif name.startswith("column"):  # column 7 holds exactly that many entries, in distinct rows
+        m = int(name[6:])
+        c[c == 7] = 8
+        r, c = np.concatenate([r, rng.permutation(rows)[:m]]), np.concatenate([c, np.full(m, 7)])
+    order = np.argsort(r, kind="stable")
+    indptr = np.concatenate([[0], np.cumsum(np.bincount(r, minlength=rows))]).astype(np.int32)
+    data = (1 + 4 * rng.random(len(r))).astype(np.float32)
+    C = sp.csr_matrix((data, c[order].astype(np.int32), indptr), shape=(rows, cols))
+    if name == "unsorted":
+        merged = C.copy()
+        merged.sum_duplicates()
+        assert not C.has_sorted_indices and merged.nnz < C.nnz
+    return C
+
+
+@pytest.mark.parametrize("name", EDGES)
+def test_device_transpose_edges(lib, ctx, name):
+    """The transpose of a one-segment device CSR is scipy's, and complete when the call returns: solves over it, made
+    after the input is destroyed and after a second transpose, and its use at once as a liked filter (top-k and
+    restrict_columns) give bitwise what the upload of scipy's transpose gives."""
+    C = edge_csr(name)
+    T = C.T.tocsr()
+    f, reg, k = 32, 0.1, 10  # 32 factors: no top-k batch takes the wgmma kernel, which needs 64
+    rng = np.random.default_rng(6)
+    X0 = rng.standard_normal((T.shape[0], f), dtype=np.float32)
+    Y = lib.DeviceFactors.from_host(ctx, rng.standard_normal((T.shape[1], f), dtype=np.float32))
+    subset = np.sort(rng.choice(T.shape[1], T.shape[1] // 2, replace=False)).astype(np.int32)
+    sub = lib.DeviceSnapshot.from_host(ctx, subset) if len(subset) else None
+    sub_ids = sub.cuda() if sub is not None else CudaArray(0, (0,), 4, 1, 0)
+    Q = lib.DeviceFactors.from_host(ctx, X0)
+    u = lib.DeviceCSR.upload(ctx, T)
+    d = lib.DeviceCSR.upload(ctx, C)
+    assert d.segment_count == 1 and not d.host_resident
+
+    liked = d.transpose()
+    got, want = lib.topk(ctx, Y, Q, k, liked=liked), lib.topk(ctx, Y, Q, k, liked=u)
+    assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
+    r_got, r_want = liked.restrict_columns(sub_ids), u.restrict_columns(sub_ids)
+    assert_rows(lib, ctx, r_got, r_want.download())
+
+    t, t2 = d.transpose(), d.transpose()
+    d.close()
+    for use_cg in (False, True):
+        out = []
+        for m in (t, u):
+            X = lib.DeviceFactors.from_host(ctx, X0)
+            if use_cg:
+                lib.least_squares_cg(ctx, m, X, Y, reg)
+            else:
+                lib.least_squares(ctx, m, X, Y, reg)
+            out.append(X.download())
+            X.close()
+        assert np.array_equal(out[0], out[1]), "cg" if use_cg else "cholesky"
+    for h in (liked, t, t2):
+        assert h.segment_count == 1 and not h.host_resident
+        assert_rows(lib, ctx, h, T)
+    for h in (liked, t, t2, u, r_got, r_want, Q, Y) + ((sub,) if sub is not None else ()):
+        h.close()
