@@ -218,7 +218,7 @@ class Context:
 
     def set_knob(self, name, value):
         """Measurement knobs (short_max, short_serial, whiten_fma, gramian_fma, topk_legacy, cg_nv, segment_nnz,
-        host_csr); see include/als_b200.h."""
+        host_csr) and the test-only alloc_fail_at; see include/als_b200.h."""
         check(self.lib.als_ctx_set_knob(self.h, name.encode(), int(value)))
 
     def get_knob(self, name):

@@ -326,118 +326,123 @@ class AlternatingLeastSquares:
                 Cui_host = Cui_host.astype(np.float32)  # cpu/als.py:129-130
         ctx = self.ctx
 
-        s = time.time()
-        # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
-        # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
-        row_cost = 20 if self.use_cg else 60
-        if from_blocks:
-            Cui_s, Ciu_s, usplit, isplit, (users, items, nnz) = self._ingest_row_blocks(user_items, row_cost)
-        elif pg is not None and pg.world > 1:
-            users, items, nnz = *Cui_host.shape, Cui_host.nnz
-            Cui_s, Ciu_s, usplit, isplit = self._ingest_shards(Cui_host, row_cost)
-        elif from_device:
-            # copied on the device into the library's arrays and always device-resident (the host_csr rule is for
-            # host arrays); the same layout, so bitwise the factors of the same scipy CSR
-            Cui_s = _lib.DeviceCSR.from_device(ctx, user_items)
-            users, items, nnz = Cui_s.shape3
-            if self.alpha != 1.0:
-                Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
-            Ciu_s = Cui_s.transpose()
-            usplit = isplit = None
-        else:
-            users, items, nnz = *Cui_host.shape, Cui_host.nnz
-            # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a
-            # single-GPU fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise
-            # the same
-            host = False
-            if self.process_group is None:
-                host = bool(ctx.get_knob("host_csr")) or \
-                    _lib.csr_residency(users, items, Cui_host.nnz, self.factors, ctx.mem_info()[0]) == "host"
-            Cui_s = _lib.DeviceCSR.upload(ctx, Cui_host, host=host)
-            if self.alpha != 1.0:
-                Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
-            Ciu_s = Cui_s.transpose()    # cpu/als.py:137, on device
-            usplit = isplit = None
-        log.debug("Uploaded and transposed in %.3fs", time.time() - s)
-
-        # cpu/als.py:144-147: pre-set factors are kept, otherwise rng.random(...) * 0.01
-        if self.process_group is not None and self.process_group.world > 1 and \
-                (self._factors_shape("user") is None or self._factors_shape("item") is None):
-            # every rank must start from the same replicas: rank 0 draws a seed, everyone initialises from it
-            seed = int(random_state.integers(1, 2**31 - 1)) if self.process_group.rank == 0 else 0
-            seed = int(ctx.allreduce([float(seed)], "max")[0])
-            random_state = np.random.default_rng(seed)
-        if self._factors_shape("user") is None:
-            self._set_host("user", random_state.random((users, self.factors), dtype=np.float32) * np.float32(0.01))
-        if self._factors_shape("item") is None:
-            self._set_host("item", random_state.random((items, self.factors), dtype=np.float32) * np.float32(0.01))
-        if self._factors_shape("user") != (users, self.factors) or self._factors_shape("item") != (items, self.factors):
-            raise ValueError("pre-set factors do not match the shape of user_items / the factors parameter")
-        X = self._device_factors("user")
-        Y = self._device_factors("item")
-        self._user_norms = self._item_norms = self._YtY = self._XtX = None  # cpu/als.py:152-154
-        self._dev_norms = {"user": None, "item": None}
-
-        self._p2p = False
-        if usplit is not None and os.environ.get("ALS_B200_NO_P2P") != "1":
-            # fused exchange: solved rows are stored straight into the peers' replicas over NVLink
-            ctx.attach_peers(X)
-            ctx.attach_peers(Y)
-            self._p2p = True
-            # Gramian of the item factors for the first user half (each rank sums its own rows)
-            _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
-
-        loss = None
-        progress = None
-        if show_progress:
-            try:
-                from tqdm.auto import tqdm
-
-                progress = tqdm(total=self.iterations)
-            except ImportError:
-                progress = None
+        Cui_s = Ciu_s = None
         try:
-            for iteration in range(self.iterations):  # cpu/als.py:162-177
-                s = time.time()
-                self._half(Cui_s, X, Y, usplit)
-                self._half(Ciu_s, Y, X, isplit)
-                if self._p2p and not self.use_cg:
-                    _lib.solver_status(ctx)  # raises on every rank in the same iteration if any rank's half failed
-                if progress is not None:
-                    progress.update(1)
-                if self.calculate_training_loss:
-                    loss = self._loss(Cui_s, X, Y, users, items, nnz)
-                    if self._p2p:  # the loss pass reuses the Gramian buffers: restore Y^T Y for the next half
-                        _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
+            s = time.time()
+            # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
+            # CG-recurrence term worth ~60 (Cholesky) or ~20 (CG) nonzeros
+            row_cost = 20 if self.use_cg else 60
+            if from_blocks:
+                Cui_s, Ciu_s, usplit, isplit, (users, items, nnz) = self._ingest_row_blocks(user_items, row_cost)
+            elif pg is not None and pg.world > 1:
+                users, items, nnz = *Cui_host.shape, Cui_host.nnz
+                Cui_s, Ciu_s, usplit, isplit = self._ingest_shards(Cui_host, row_cost)
+            elif from_device:
+                # copied on the device into the library's arrays and always device-resident (the host_csr rule is for
+                # host arrays); the same layout, so bitwise the factors of the same scipy CSR
+                Cui_s = _lib.DeviceCSR.from_device(ctx, user_items)
+                users, items, nnz = Cui_s.shape3
+                if self.alpha != 1.0:
+                    Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
+                Ciu_s = Cui_s.transpose()
+                usplit = isplit = None
+            else:
+                users, items, nnz = *Cui_host.shape, Cui_host.nnz
+                # Cui / Ciu stay in page-locked host memory, streamed through the device segment by segment, when a
+                # single-GPU fit would not fit in device memory (or the host_csr knob asks for it); the factors are bitwise
+                # the same
+                host = False
+                if self.process_group is None:
+                    host = bool(ctx.get_knob("host_csr")) or \
+                        _lib.csr_residency(users, items, Cui_host.nnz, self.factors, ctx.mem_info()[0]) == "host"
+                Cui_s = _lib.DeviceCSR.upload(ctx, Cui_host, host=host)
+                if self.alpha != 1.0:
+                    Cui_s.scale(self.alpha)  # cpu/als.py:133-134, on device
+                Ciu_s = Cui_s.transpose()    # cpu/als.py:137, on device
+                usplit = isplit = None
+            log.debug("Uploaded and transposed in %.3fs", time.time() - s)
+
+            # cpu/als.py:144-147: pre-set factors are kept, otherwise rng.random(...) * 0.01
+            if self.process_group is not None and self.process_group.world > 1 and \
+                    (self._factors_shape("user") is None or self._factors_shape("item") is None):
+                # every rank must start from the same replicas: rank 0 draws a seed, everyone initialises from it
+                seed = int(random_state.integers(1, 2**31 - 1)) if self.process_group.rank == 0 else 0
+                seed = int(ctx.allreduce([float(seed)], "max")[0])
+                random_state = np.random.default_rng(seed)
+            if self._factors_shape("user") is None:
+                self._set_host("user", random_state.random((users, self.factors), dtype=np.float32) * np.float32(0.01))
+            if self._factors_shape("item") is None:
+                self._set_host("item", random_state.random((items, self.factors), dtype=np.float32) * np.float32(0.01))
+            if self._factors_shape("user") != (users, self.factors) or self._factors_shape("item") != (items, self.factors):
+                raise ValueError("pre-set factors do not match the shape of user_items / the factors parameter")
+            X = self._device_factors("user")
+            Y = self._device_factors("item")
+            self._user_norms = self._item_norms = self._YtY = self._XtX = None  # cpu/als.py:152-154
+            self._dev_norms = {"user": None, "item": None}
+
+            self._p2p = False
+            if usplit is not None and os.environ.get("ALS_B200_NO_P2P") != "1":
+                # fused exchange: solved rows are stored straight into the peers' replicas over NVLink
+                ctx.attach_peers(X)
+                ctx.attach_peers(Y)
+                self._p2p = True
+                # Gramian of the item factors for the first user half (each rank sums its own rows)
+                _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
+
+            loss = None
+            progress = None
+            if show_progress:
+                try:
+                    from tqdm.auto import tqdm
+
+                    progress = tqdm(total=self.iterations)
+                except ImportError:
+                    progress = None
+            try:
+                for iteration in range(self.iterations):  # cpu/als.py:162-177
+                    s = time.time()
+                    self._half(Cui_s, X, Y, usplit)
+                    self._half(Ciu_s, Y, X, isplit)
+                    if self._p2p and not self.use_cg:
+                        _lib.solver_status(ctx)  # raises on every rank in the same iteration if any rank's half failed
                     if progress is not None:
-                        progress.set_postfix({"loss": loss})
-                    elif not show_progress:
-                        log.info("loss %.4f", loss)
-                if not callback:
-                    callback = self.fit_callback  # backward compatibility, cpu/als.py:193-195
-                if callback:
-                    ctx.sync()
-                    callback(iteration, time.time() - s, loss)
-            ctx.sync()
-        except BaseException:
-            if self._p2p:  # failures are raised on every rank in the same half (_raise_together): unmap and leave
+                        progress.update(1)
+                    if self.calculate_training_loss:
+                        loss = self._loss(Cui_s, X, Y, users, items, nnz)
+                        if self._p2p:  # the loss pass reuses the Gramian buffers: restore Y^T Y for the next half
+                            _lib.gramian_shard(ctx, Y, isplit[pg.rank], isplit[pg.rank + 1] - isplit[pg.rank])
+                        if progress is not None:
+                            progress.set_postfix({"loss": loss})
+                        elif not show_progress:
+                            log.info("loss %.4f", loss)
+                    if not callback:
+                        callback = self.fit_callback  # backward compatibility, cpu/als.py:193-195
+                    if callback:
+                        ctx.sync()
+                        callback(iteration, time.time() - s, loss)
+                ctx.sync()
+            except BaseException:
+                if self._p2p:  # failures are raised on every rank in the same half (_raise_together): unmap and leave
+                    ctx.detach_peers(X)
+                    ctx.detach_peers(Y)
+                    self._p2p = False
+                raise
+            finally:
+                if progress is not None:
+                    progress.close()
+            if self.calculate_training_loss and loss is not None:
+                log.info("Final training loss %.4f", loss)
+            if self._p2p:
+                ctx.barrier()
                 ctx.detach_peers(X)
                 ctx.detach_peers(Y)
-                self._p2p = False
-            raise
-        finally:
-            if progress is not None:
-                progress.close()
-        if self.calculate_training_loss and loss is not None:
-            log.info("Final training loss %.4f", loss)
-        if self._p2p:
-            ctx.barrier()
-            ctx.detach_peers(X)
-            ctx.detach_peers(Y)
-        self._mark_device_updated("user")
-        self._mark_device_updated("item")
-        Ciu_s.close()
-        Cui_s.close()
+            self._mark_device_updated("user")
+            self._mark_device_updated("item")
+        finally:  # on every exit: a traceback would otherwise keep both CSRs alive through this frame
+            if Ciu_s is not None:
+                Ciu_s.close()
+            if Cui_s is not None:
+                Cui_s.close()
         self._check_fit_errors()  # cpu/als.py:202
 
     def _ingest_shards(self, Cui_host, row_cost):

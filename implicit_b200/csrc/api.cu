@@ -29,13 +29,74 @@ int cuda_fail(cudaError_t e, const char *what, const char *file, int line) {
   return ALS_E_CUDA;
 }
 
+// the alloc_fail_at knob: ALS_E_CUDA for the n-th allocation since it was set
+static int injected_failure(als_ctx *ctx) {
+  if (ctx->knobs.alloc_fail_at <= 0 || --ctx->knobs.alloc_fail_at > 0) return ALS_OK;
+  set_error("injected allocation failure");
+  return ALS_E_CUDA;
+}
+
 int dev_alloc(als_ctx *ctx, void **ptr, int64_t bytes, cudaStream_t stream) {
+  const int rc = injected_failure(ctx);
+  if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaMallocAsync(ptr, (size_t)std::max<int64_t>(bytes, 16), stream ? stream : ctx->stream));
   return ALS_OK;
 }
 
 void dev_free(als_ctx *ctx, void *ptr) {
   if (ptr) cudaFreeAsync(ptr, ctx->stream);
+}
+
+DeviceBlock &DeviceBlock::operator=(DeviceBlock &&o) noexcept {
+  if (this != &o) {
+    reset();
+    ctx_ = o.ctx_;
+    p_ = o.take();
+    pooled_ = o.pooled_;
+  }
+  return *this;
+}
+
+int DeviceBlock::alloc(als_ctx *ctx, int64_t bytes, cudaStream_t stream) {
+  reset();
+  ctx_ = ctx;
+  pooled_ = true;
+  return dev_alloc(ctx, &p_, bytes, stream);
+}
+
+int DeviceBlock::alloc_cuda(als_ctx *ctx, int64_t bytes) {
+  reset();
+  ctx_ = ctx;
+  pooled_ = false;
+  int rc = injected_failure(ctx);
+  if (rc == ALS_OK) {
+    const cudaError_t e = cudaMalloc(&p_, (size_t)std::max<int64_t>(bytes, 16));
+    if (e != cudaSuccess) {
+      p_ = nullptr;
+      rc = cuda_fail(e, "cudaMalloc", __FILE__, __LINE__);
+    }
+  }
+  return rc;
+}
+
+void DeviceBlock::reset() {
+  void *p = take();
+  if (!p) return;
+  if (pooled_)
+    dev_free(ctx_, p);
+  else
+    cudaFree(p);
+}
+
+void CsrDestroy::operator()(als_csr *c) const {
+  if (c->ctx) cudaStreamSynchronize(c->ctx->stream);  // a copy may still be landing in its arrays
+  als_csr_destroy(c);
+}
+
+CsrHolder new_csr(als_ctx *ctx) {
+  CsrHolder c(new als_csr());
+  c->ctx = ctx;
+  return c;
 }
 
 // Builds the schedules of a CSR laid out without them (csr_layout's schedule = false) from its device indptrs.
@@ -385,7 +446,8 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
               prop.minor);
     return ALS_E_UNSUPPORTED;
   }
-  als_ctx *ctx = new als_ctx();
+  // torn down with whatever it holds on any failure below
+  std::unique_ptr<als_ctx, int (*)(als_ctx *)> ctx(new als_ctx(), als_ctx_destroy);
   ctx->device = device;
   {
     struct { const char *env; const char *name; } table[] = {
@@ -396,10 +458,7 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
       const char *e = getenv(t.env);
       if (!e) continue;
       const int v = *e ? atoi(e) : 1;
-      if (als_ctx_set_knob(ctx, t.name, v) != ALS_OK) {
-        delete ctx;
-        return ALS_E_INVALID;
-      }
+      if (als_ctx_set_knob(ctx.get(), t.name, v) != ALS_OK) return ALS_E_INVALID;
       fprintf(stderr, "libals_b200: %s=%s is set (knob %s = %d)\n", t.env, e, t.name, v);
     }
   }
@@ -443,7 +502,7 @@ ALS_API int als_ctx_create(int device, als_ctx **out) {
   ALS_CUDA(cudaMemset(ctx->status, 0, sizeof(int32_t) * 4));
   ALS_CUDA(cudaMemset(ctx->G, 0, sizeof(float) * (1024 * 1024 + 64)));
   ALS_CUDA(cudaMalloc(&ctx->dscalars, sizeof(double) * 8));
-  *out = ctx;
+  *out = ctx.release();
   return ALS_OK;
 }
 
@@ -463,6 +522,7 @@ ALS_API int als_ctx_set_knob(als_ctx *ctx, const char *name, int value) {
     ALS_REQUIRE(value >= 0 && value < INT32_MAX, "als_ctx_set_knob: segment_nnz must be in [0, 2^31 - 1)");
     k.segment_nnz = value;
   } else if (!strcmp(name, "host_csr")) k.host_csr = value != 0;
+  else if (!strcmp(name, "alloc_fail_at")) k.alloc_fail_at = std::max(value, 0);
   else {
     set_error("als_ctx_set_knob: unknown knob '%s'", name);
     return ALS_E_INVALID;
@@ -482,6 +542,7 @@ ALS_API int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value) {
   else if (!strcmp(name, "cg_nv")) *value = k.cg_nv;
   else if (!strcmp(name, "segment_nnz")) *value = (int)k.segment_nnz;
   else if (!strcmp(name, "host_csr")) *value = k.host_csr;
+  else if (!strcmp(name, "alloc_fail_at")) *value = k.alloc_fail_at;
   else {
     set_error("als_ctx_get_knob: unknown knob '%s'", name);
     return ALS_E_INVALID;
@@ -491,10 +552,16 @@ ALS_API int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value) {
 
 ALS_API int als_ctx_destroy(als_ctx *ctx) {
   if (!ctx) return ALS_OK;
+  // also the teardown of a failed als_ctx_create: members it never created are null and skipped
+  auto stream_destroy = [](cudaStream_t s) {
+    if (s) cudaStreamDestroy(s);
+  };
+  auto event_destroy = [](cudaEvent_t e) {
+    if (e) cudaEventDestroy(e);
+  };
   cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
-  cudaStreamSynchronize(ctx->copy);
-  cudaStreamSynchronize(ctx->aux);
+  for (cudaStream_t s : {ctx->stream, ctx->copy, ctx->aux})
+    if (s) cudaStreamSynchronize(s);
   als_comm_destroy(ctx);
   cudaFree(ctx->G);
   cudaFree(ctx->Greg);
@@ -513,31 +580,31 @@ ALS_API int als_ctx_destroy(als_ctx *ctx) {
   if (ctx->stage_buf) {
     cudaFreeHost(ctx->stage_buf);
     for (int t = 0; t < 4; ++t) {
-      cudaStreamDestroy(ctx->stage_stream[t]);
-      for (int b = 0; b < 2; ++b) cudaEventDestroy(ctx->stage_ev[t][b]);
+      stream_destroy(ctx->stage_stream[t]);
+      for (int b = 0; b < 2; ++b) event_destroy(ctx->stage_ev[t][b]);
     }
-    cudaEventDestroy(ctx->stage_ready);
+    event_destroy(ctx->stage_ready);
   }
   for (int k = 0; k < 2; ++k) {
-    cudaEventDestroy(ctx->ring_loaded[k]);
-    cudaEventDestroy(ctx->ring_free[k]);
+    event_destroy(ctx->ring_loaded[k]);
+    event_destroy(ctx->ring_free[k]);
   }
   for (int i = 0; i < 5; ++i) {
-    if (ctx->class_stream[i]) cudaStreamDestroy(ctx->class_stream[i]);
-    if (ctx->class_join[i]) cudaEventDestroy(ctx->class_join[i]);
+    stream_destroy(ctx->class_stream[i]);
+    event_destroy(ctx->class_join[i]);
   }
-  if (ctx->class_fork) cudaEventDestroy(ctx->class_fork);
+  event_destroy(ctx->class_fork);
   {
     cudaMemPool_t pool;
     if (cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
   }
-  cudaEventDestroy(ctx->ev0);
-  cudaEventDestroy(ctx->ev1);
-  cudaStreamDestroy(ctx->stream);
-  cudaStreamDestroy(ctx->copy);
-  cudaStreamDestroy(ctx->aux);
-  cudaEventDestroy(ctx->ev_fork);
-  cudaEventDestroy(ctx->ev_join);
+  event_destroy(ctx->ev0);
+  event_destroy(ctx->ev1);
+  stream_destroy(ctx->stream);
+  stream_destroy(ctx->copy);
+  stream_destroy(ctx->aux);
+  event_destroy(ctx->ev_fork);
+  event_destroy(ctx->ev_join);
   delete ctx;
   return ALS_OK;
 }
@@ -732,8 +799,7 @@ static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int
   ALS_REQUIRE(bad_row < 0, "%s: indptr is not monotone at row %lld", who, (long long)bad_row);
   *out = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
+  CsrHolder c = new_csr(ctx);
   c->rows = rows;
   c->cols = cols;
   c->nnz = nnz;
@@ -742,19 +808,19 @@ static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int
   const char *ix = (const char *)a.indices + base * a.index_bytes;
   const char *dv = (const char *)a.data + base * a.data_bytes;
   int64_t bad = -1;
-  int rc = csr_alloc(ctx, c);
+  int rc = csr_alloc(ctx, c.get());
   if (rc == ALS_OK && a.device) {
-    rc = device_entries(ctx, c, ix, a.index_bytes, dv, a.data_bytes, &bad);
+    rc = device_entries(ctx, c.get(), ix, a.index_bytes, dv, a.data_bytes, &bad);
   } else if (rc == ALS_OK) {
     const float *data = (const float *)dv;
     rc = int32_entry ? h2d_copy(ctx, c->indices, ix, sizeof(int32_t) * nnz)
                      : h2d_indices(ctx, c->indices, ix, a.index_bytes, nnz, cols, &bad, host);
     if (rc == ALS_OK)
-      rc = host ? fill_host_values(ctx, c, c->data, nnz,
+      rc = host ? fill_host_values(ctx, c.get(), c->data, nnz,
                                    [&](float *v, int64_t i0, int64_t m) { memcpy(v, data + i0, sizeof(float) * m); })
                 : h2d_copy(ctx, c->data, data, sizeof(float) * nnz);
   }
-  if (rc == ALS_OK) rc = csr_layout(ctx, c, ip.data());
+  if (rc == ALS_OK) rc = csr_layout(ctx, c.get(), ip.data());
   if (rc != ALS_OK) {
     if (bad >= 0) {
       int64_t v = 0;
@@ -766,11 +832,9 @@ static int csr_build(const char *who, bool host, als_ctx *ctx, int64_t rows, int
       }
       set_error("%s: indices[%lld] = %lld is outside [0, %lld)", who, (long long)(base + bad), (long long)v, (long long)cols);
     }
-    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    als_csr_destroy(c);
     return rc;
   }
-  *out = c;
+  *out = c.release();
   return ALS_OK;
 }
 
@@ -920,8 +984,7 @@ ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int6
   std::vector<int64_t> ip64;
   int rc = csr_indptr64(ctx, in, ip64);
   if (rc != ALS_OK) return rc;
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
+  CsrHolder c = new_csr(ctx);
   c->rows = r1 - r0;
   c->cols = in->cols;
   c->nnz = ip64[r1] - ip64[r0];
@@ -930,17 +993,14 @@ ALS_API int als_csr_slice_rows(als_ctx *ctx, const als_csr *in, int64_t r0, int6
   c->indices = in->indices;
   c->data = in->data;
   if (!in->segs.empty()) {  // a shard of a segmented CSR can itself exceed 2^31 nonzeros: a segmented view
-    rc = make_segments(ctx, c, ip64.data() + r0);
+    rc = make_segments(ctx, c.get(), ip64.data() + r0);
   } else {  // a view into the parent's indptr: absolute positions into its indices / data
     c->indptr = in->indptr + r0;
     const std::vector<int32_t> ip(ip64.begin() + r0, ip64.begin() + r1 + 1);
-    rc = build_schedule(ctx, c, ip.data());
+    rc = build_schedule(ctx, c.get(), ip.data());
   }
-  if (rc != ALS_OK) {
-    als_csr_destroy(c);
-    return rc;
-  }
-  *out = c;
+  if (rc != ALS_OK) return rc;
+  *out = c.release();
   return ALS_OK;
 }
 
@@ -1201,12 +1261,13 @@ ALS_API int als_factors_ipc_export(als_ctx *ctx, const als_factors *cf, void *ha
   if (f->pooled) {
     // blocks of the stream-ordered pool cannot be exported with cudaIpcGetMemHandle: move the matrix (once)
     const int64_t bytes = sizeof(float) * std::max<int64_t>(f->rows, 1) * f->ld;
-    float *moved = nullptr;
-    ALS_CUDA(cudaMalloc(&moved, bytes));
+    Dev<float> moved;
+    const int rc = moved.alloc_cuda(ctx, bytes);
+    if (rc != ALS_OK) return rc;
     ALS_CUDA(cudaMemcpyAsync(moved, f->d, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-    dev_free(ctx, f->d);
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    f->d = moved;
+    dev_free(ctx, f->d);
+    f->d = moved.release();
     f->pooled = false;
   }
   cudaIpcMemHandle_t h;
@@ -1640,17 +1701,13 @@ ALS_API int als_csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const v
   int rc = m ? require_device_memory(ctx, who, "subset", subset) : ALS_OK;
   if (rc == ALS_OK) rc = wait_for_producer(ctx, producer_stream);
   if (rc != ALS_OK) return rc;
-  int64_t *indptr = nullptr, nnz = 0;
-  int32_t *indices = nullptr;
-  float *data = nullptr;
-  rc = csr_restrict_columns(ctx, liked, subset, subset_bytes, m, &indptr, &indices, &data, &nnz);
+  Dev<int64_t> indptr;
+  Dev<int32_t> indices;
+  Dev<float> data;
+  int64_t nnz = 0;
+  if ((rc = csr_restrict_columns(ctx, liked, subset, subset_bytes, m, indptr, indices, data, &nnz)) != ALS_OK) return rc;
   // the remapped entries go through the one upload path, like every other CSR
-  if (rc == ALS_OK)
-    rc = csr_build(who, false, ctx, liked->rows, m, nnz, CsrArrays{indptr, 8, indices, 4, data, 4, true}, 0, out);
-  dev_free(ctx, indptr);
-  dev_free(ctx, indices);
-  dev_free(ctx, data);
-  return rc;
+  return csr_build(who, false, ctx, liked->rows, m, nnz, CsrArrays{indptr, 8, indices, 4, data, 4, true}, 0, out);
 }
 
 ALS_API int als_topk_into(als_ctx *ctx, const als_factors *items, const als_factors *queries, const void *query_rows,
@@ -1723,19 +1780,14 @@ ALS_API int als_factors_grow(als_ctx *ctx, als_factors *f, int64_t rows) {
   ALS_REQUIRE(rows <= ctx->mem_bytes / row_bytes, "%s: %lld rows of %lld bytes are more than the device's %lld bytes", who,
               (long long)rows, (long long)row_bytes, (long long)ctx->mem_bytes);
   ALS_CUDA(cudaSetDevice(ctx->device));
-  float *d = nullptr;
-  const int rc = dev_alloc(ctx, (void **)&d, row_bytes * rows);
+  Dev<float> d;
+  const int rc = d.alloc(ctx, row_bytes * rows);
   if (rc != ALS_OK) return rc;
-  cudaError_t e = f->rows ? cudaMemcpyAsync(d, f->d, row_bytes * f->rows, cudaMemcpyDeviceToDevice, ctx->stream)
-                          : cudaSuccess;
+  if (f->rows) ALS_CUDA(cudaMemcpyAsync(d, f->d, row_bytes * f->rows, cudaMemcpyDeviceToDevice, ctx->stream));
   // the new rows, padding included, are zero: np.concatenate([host, np.zeros(...)]) uploaded
-  if (e == cudaSuccess) e = cudaMemsetAsync(d + f->rows * f->ld, 0, row_bytes * (rows - f->rows), ctx->stream);
-  if (e != cudaSuccess) {
-    dev_free(ctx, d);
-    return cuda_fail(e, "als_factors_grow", __FILE__, __LINE__);
-  }
+  ALS_CUDA(cudaMemsetAsync(d + f->rows * f->ld, 0, row_bytes * (rows - f->rows), ctx->stream));
   dev_free(ctx, f->d);  // stream-ordered: after the copy has read it
-  f->d = d;
+  f->d = d.release();
   f->rows = rows;
   return ALS_OK;
 }

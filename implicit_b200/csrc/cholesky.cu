@@ -264,6 +264,19 @@ __global__ void reset_segment_counters(int32_t *counters) {
   if (t < 16 && t != kCtrWhitenOk && t != kCtrHasNan && t != kCtrYAbsMax) counters[t] = 0;
 }
 
+// Synchronises the side streams of a Cholesky half (aux and the short-row class streams) unless disarmed: an error
+// return from the section forked onto them leaves launches there that may still read a ring slot of the segment.
+struct JoinSidesOnError {
+  als_ctx *ctx;
+  bool armed = true;
+  ~JoinSidesOnError() {
+    if (!armed) return;
+    cudaStreamSynchronize(ctx->aux);
+    for (cudaStream_t s : ctx->class_stream)
+      if (s) cudaStreamSynchronize(s);
+  }
+};
+
 // The narrow family (ld <= 64) over C, which may be a list of row-block segments.  Everything that affects rounding is
 // decided once for the whole matrix (max |y|, max ||c| - 1|, the long-row kernel, whether short rows take the whitened
 // path, the whitening itself); the deferred list and its counters are per segment.
@@ -352,6 +365,7 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
     const int64_t n_main = short_max > 0 ? S->le_begin[short_class] : S->n_work;
     const bool seg_short = short_max > 0 && S->n_work > n_main;
     if (!S->n_work) return ALS_OK;
+    JoinSidesOnError join{ctx};
     ProfScope prof(ctx, kProfCholesky);
     // The short-row side (whitening, the short-row kernels, the second pass of the full-size kernel over what they
     // hand back) runs on the aux stream.  The single-CTA factorisation of G is launched first and hides behind the
@@ -395,6 +409,7 @@ int run_cholesky(als_ctx *ctx, const als_csr *Cm, als_factors *X, const als_fact
         ALS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
       }
     }
+    join.armed = false;
     return ALS_OK;
   };
   return run_cholesky_half(ctx, Cm, Y, fam);

@@ -181,22 +181,20 @@ int agree(als_ctx *ctx, int rc, const char *who, const char *what) {
   return ALS_OK;
 }
 
-// buffers of one exchange, freed by the caller (stream ordered, after the operations that use them)
-struct Exchange {
-  int64_t *buf = nullptr;  // the shapes out and in (6 W), then the outgoing indptrs
-  int64_t *rip = nullptr;  // the incoming indptrs
-};
-
 // Two grouped rounds of ncclSend / ncclRecv on the compute stream: the shapes (rows, cols, nnz of each piece), then
 // every piece's indptr (64-bit positions from its first nonzero), indices and values straight into the receiving CSR.
 // NCCL matches the operations between one pair of ranks in the order they are issued.  The ranks agree before each
-// round that every one of them is ready for it (its pieces checked and staged, then its incoming pieces allocated).
-int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x) {
+// round that every one of them is ready for it (its pieces checked and staged, then its incoming pieces allocated): the
+// two immediately invoked lambdas collect a rank's failure for that agreement.  recv is set on success only.
+int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv) {
   static const char *who = "als_comm_exchange_csr";
   const int W = ctx->world;
   ncclComm_t comm = (ncclComm_t)ctx->comm;
   std::vector<std::vector<int64_t>> sip(W);
   std::vector<int64_t> head(6 * (size_t)W, 0), base(W), rip_off(W + 1, 0);
+  Dev<int64_t> buf;  // the shapes out and in (6 W), then the outgoing indptrs
+  Dev<int64_t> rip;  // the incoming indptrs
+  std::vector<CsrHolder> got(W);
   int rc = [&]() -> int {
     for (int q = 0; q < W; ++q) {
       ALS_REQUIRE(send[q], "%s: piece %d is NULL", who, q);
@@ -220,14 +218,13 @@ int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x
       base[q] = sip[q][0];
       for (size_t r = 0; r < sip[q].size(); ++r) out[at + r] = sip[q][r] - base[q];
     }
-    const int r = dev_alloc(ctx, (void **)&x.buf, sizeof(int64_t) * out.size());
+    const int r = buf.alloc(ctx, sizeof(int64_t) * out.size());
     if (r != ALS_OK) return r;
-    ALS_CUDA(cudaMemcpyAsync(x.buf, out.data(), sizeof(int64_t) * out.size(), cudaMemcpyHostToDevice, ctx->stream));
+    ALS_CUDA(cudaMemcpyAsync(buf, out.data(), sizeof(int64_t) * out.size(), cudaMemcpyHostToDevice, ctx->stream));
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // `out` dies here
     return ALS_OK;
   }();
   if ((rc = agree(ctx, rc, who, "to stage its pieces")) != ALS_OK) return rc;
-  int64_t *buf = x.buf;
   ALS_NCCL(g_nccl.GroupStart());
   for (int q = 0; q < W; ++q) {
     ALS_NCCL(g_nccl.Send(buf + 3 * q, 3, ncclInt64, q, comm, ctx->stream));
@@ -238,9 +235,8 @@ int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   rc = [&]() -> int {
     for (int p = 0; p < W; ++p) {
-      als_csr *c = new als_csr();
-      recv[p] = c;
-      c->ctx = ctx;
+      got[p] = new_csr(ctx);
+      als_csr *c = got[p].get();
       c->rows = head[3 * W + 3 * p];
       c->cols = head[3 * W + 3 * p + 1];
       c->nnz = head[3 * W + 3 * p + 2];
@@ -248,7 +244,7 @@ int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x
       if (r != ALS_OK) return r;
       rip_off[p + 1] = rip_off[p] + c->rows + 1;
     }
-    return dev_alloc(ctx, (void **)&x.rip, sizeof(int64_t) * rip_off[W]);
+    return rip.alloc(ctx, sizeof(int64_t) * rip_off[W]);
   }();
   if ((rc = agree(ctx, rc, who, "to allocate the pieces it receives")) != ALS_OK) return rc;
   ALS_NCCL(g_nccl.GroupStart());
@@ -261,8 +257,8 @@ int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x
     }
   }
   for (int p = 0; p < W; ++p) {
-    als_csr *c = recv[p];
-    ALS_NCCL(g_nccl.Recv(x.rip + rip_off[p], (size_t)(c->rows + 1), ncclInt64, p, comm, ctx->stream));
+    als_csr *c = got[p].get();
+    ALS_NCCL(g_nccl.Recv(rip + rip_off[p], (size_t)(c->rows + 1), ncclInt64, p, comm, ctx->stream));
     if (c->nnz) {
       ALS_NCCL(g_nccl.Recv(c->indices, (size_t)c->nnz, ncclInt32, p, comm, ctx->stream));
       ALS_NCCL(g_nccl.Recv(c->data, (size_t)c->nnz, ncclFloat, p, comm, ctx->stream));
@@ -270,11 +266,12 @@ int exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv, Exchange &x
   }
   ALS_NCCL(g_nccl.GroupEnd());
   std::vector<int64_t> ip(rip_off[W]);
-  ALS_CUDA(cudaMemcpyAsync(ip.data(), x.rip, sizeof(int64_t) * ip.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaMemcpyAsync(ip.data(), rip, sizeof(int64_t) * ip.size(), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   // the received pieces are only copied by the merge: their schedules wait for a solve that may never come
   for (int p = 0; p < W; ++p)
-    if ((rc = csr_layout(ctx, recv[p], ip.data() + rip_off[p], /*schedule=*/false)) != ALS_OK) return rc;
+    if ((rc = csr_layout(ctx, got[p].get(), ip.data() + rip_off[p], /*schedule=*/false)) != ALS_OK) return rc;
+  for (int p = 0; p < W; ++p) recv[p] = got[p].release();
   return ALS_OK;
 }
 
@@ -293,12 +290,9 @@ ALS_API int als_comm_allreduce_i64(als_ctx *ctx, int64_t *values, int64_t n) {
   if (n == 0 || (ctx->world == 1 && !ctx->comm)) return ALS_OK;
   ALS_REQUIRE(ctx->comm, "als_comm_allreduce_i64: communicator not initialised");
   ALS_CUDA(cudaSetDevice(ctx->device));
-  int64_t *buf = nullptr;
-  int rc = agree(ctx, dev_alloc(ctx, (void **)&buf, sizeof(int64_t) * n), "als_comm_allreduce_i64",
-                 "to allocate its buffer");
-  if (rc == ALS_OK) rc = allreduce_i64(ctx, buf, values, n);
-  dev_free(ctx, buf);
-  return rc;
+  Dev<int64_t> buf;
+  const int rc = agree(ctx, buf.alloc(ctx, sizeof(int64_t) * n), "als_comm_allreduce_i64", "to allocate its buffer");
+  return rc != ALS_OK ? rc : allreduce_i64(ctx, buf, values, n);
 }
 
 ALS_API int als_comm_exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **recv) {
@@ -306,18 +300,7 @@ ALS_API int als_comm_exchange_csr(als_ctx *ctx, als_csr *const *send, als_csr **
   ALS_REQUIRE(ctx->comm, "als_comm_exchange_csr: communicator not initialised");
   for (int p = 0; p < ctx->world; ++p) recv[p] = nullptr;
   ALS_CUDA(cudaSetDevice(ctx->device));
-  Exchange x;
-  const int rc = exchange_csr(ctx, send, recv, x);
-  dev_free(ctx, x.buf);  // stream ordered: after the sends that read them
-  dev_free(ctx, x.rip);
-  if (rc != ALS_OK) {
-    cudaStreamSynchronize(ctx->stream);
-    for (int p = 0; p < ctx->world; ++p) {
-      als_csr_destroy(recv[p]);
-      recv[p] = nullptr;
-    }
-  }
-  return rc;
+  return exchange_csr(ctx, send, recv);
 }
 
 ALS_API int als_comm_allgather_bytes(als_ctx *ctx, const void *send, void *recv, int nbytes) {

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -54,7 +55,8 @@ constexpr int kChunkNnz = 2048;   // ... into chunks of this many nonzeros (mult
 }  // namespace als
 
 // Measurement knobs.  Read from the environment ONCE, in als_ctx_create (which reports every knob that is set on
-// stderr); tools flip them afterwards with als_ctx_set_knob.  None changes results beyond fp32 rounding.
+// stderr); tools flip them afterwards with als_ctx_set_knob.  None changes results beyond fp32 rounding, except the
+// test-only alloc_fail_at.
 struct als_knobs {
   int short_max = 48;         // ALS_B200_SHORT_MAX: longest row (nonzeros) of the n x n short-row path: 0, 8, ..., 48
   int short_serial = 0;       // ALS_B200_SHORT_SERIAL: short-row kernels on the compute stream instead of the aux stream
@@ -68,6 +70,10 @@ struct als_knobs {
                               // CSR).  Changes no bit.
   int host_csr = 0;           // ALS_B200_HOST_CSR: fit() keeps Cui / Ciu in page-locked host memory and streams their
                               // segments through the device even when they fit in device memory.  Changes no bit.
+  int alloc_fail_at = 0;      // test only, set with als_ctx_set_knob alone (no environment variable), and it changes
+                              // results: n > 0 makes the n-th device allocation through dev_alloc or a DeviceBlock,
+                              // counted from the set, return ALS_E_CUDA ("injected allocation failure") without calling
+                              // CUDA; the knob is then 0 again.
 };
 
 struct als_ctx {
@@ -89,7 +95,7 @@ struct als_ctx {
   float *G = nullptr;
   float *Greg = nullptr;
   float *gram_partials = nullptr;
-  int64_t gram_partials_cap = 0;
+  int64_t gram_partials_cap = 0;  // bytes
   // per-launch scalars, see the kCtr* slots below (16 ints, zeroed before every half)
   int32_t *counters = nullptr;
   long long *bad_row = nullptr;   // [0] first non-PD row of the current half, [1] of the halves since als_solver_status
@@ -209,6 +215,52 @@ constexpr int kShortThresholds[kNumShortThresholds] = {48, 40, 32, 24, 16, 8, 0}
 // cudaFree synchronises the device).  Factor matrices exported over CUDA IPC are the exception (api.cu).
 int dev_alloc(als_ctx *ctx, void **ptr, int64_t bytes, cudaStream_t stream = nullptr);  // nullptr: ctx->stream
 void dev_free(als_ctx *ctx, void *ptr);
+
+// The owner of one temporary device block: a pool block (alloc, through dev_alloc) freed stream-ordered on ctx->stream,
+// or a cudaMalloc block (alloc_cuda) freed with cudaFree, when the owner dies or at reset().  release() hands the block
+// to a handle, whose destroy function frees it from then on.  Before an owner dies, every stream that touched its block
+// has been joined into ctx->stream or synchronised: an error return from a section forked onto other streams joins them
+// first.
+class DeviceBlock {
+ public:
+  DeviceBlock() = default;
+  DeviceBlock(const DeviceBlock &) = delete;
+  DeviceBlock &operator=(const DeviceBlock &) = delete;
+  DeviceBlock(DeviceBlock &&o) noexcept : ctx_(o.ctx_), p_(o.p_), pooled_(o.pooled_) { o.p_ = nullptr; }
+  DeviceBlock &operator=(DeviceBlock &&o) noexcept;
+  ~DeviceBlock() { reset(); }
+  int alloc(als_ctx *ctx, int64_t bytes, cudaStream_t stream = nullptr);
+  int alloc_cuda(als_ctx *ctx, int64_t bytes);
+  void reset();
+
+ protected:
+  void *take() {
+    void *p = p_;
+    p_ = nullptr;
+    return p;
+  }
+  als_ctx *ctx_ = nullptr;
+  void *p_ = nullptr;
+  bool pooled_ = true;
+};
+
+// A DeviceBlock of T elements (the byte count is the caller's).
+template <typename T>
+class Dev : public DeviceBlock {
+ public:
+  T *get() const { return static_cast<T *>(p_); }
+  operator T *() const { return get(); }
+  T *release() { return static_cast<T *>(take()); }
+};
+
+// A CSR under construction: destroyed once ctx->stream has finished with it, unless released to the caller.
+struct CsrDestroy {
+  void operator()(als_csr *c) const;
+};
+using CsrHolder = std::unique_ptr<als_csr, CsrDestroy>;
+// a new empty CSR of ctx
+CsrHolder new_csr(als_ctx *ctx);
+
 int ensure_schedule(als_ctx *ctx, als_csr *csr);
 
 int ensure_scratch(als_ctx *ctx, int64_t bytes);
@@ -367,9 +419,9 @@ int launch_row_norms(als_ctx *ctx, const als_factors *F, float zero_value, float
 int launch_gather_rows(als_ctx *ctx, const als_factors *src, const void *rows, int bytes, int64_t n, als_factors *dst);
 int sort_ids(als_ctx *ctx, const void *in, int bytes, int64_t n, void *out);
 // the liked CSR remapped onto positions of the sorted subset[m]: device indptr (int64, rows + 1), indices and values
-// (1) from the pool, *nnz entries; the caller frees them
-int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m, int64_t **indptr,
-                         int32_t **indices, float **data, int64_t *nnz);
+// (1) from the pool, *nnz entries
+int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m,
+                         Dev<int64_t> &indptr, Dev<int32_t> &indices, Dev<float> &data, int64_t *nnz);
 // refit.cu: the device side of partial_fit_* with CUDA ids (als_ids_range, als_factors_scatter_rows).
 // ids_range: min and max of n ids of `bytes` each (n = 0: 0 and -1); synchronises
 int ids_range(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t *min_id, int64_t *max_id);

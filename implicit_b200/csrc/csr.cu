@@ -111,24 +111,23 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
   const int64_t cols = in->cols;
   int end_bit = 1;
   while (end_bit < 32 && (1ll << end_bit) < (long long)cols) ++end_bit;
-  long long *next = nullptr, *out_ip = nullptr;
+  Dev<long long> next, out_ip;
   int rc;
-  if ((rc = dev_alloc(ctx, (void **)&next, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
-  if ((rc = dev_alloc(ctx, (void **)&out_ip, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
+  if ((rc = next.alloc(ctx, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
+  if ((rc = out_ip.alloc(ctx, sizeof(long long) * (cols + 1))) != ALS_OK) return rc;
   ALS_CUDA(cudaMemsetAsync(next, 0, sizeof(long long) * (cols + 1), ctx->stream));
-  if ((rc = column_histogram(ctx, in, (unsigned long long *)next)) != ALS_OK) return rc;
+  if ((rc = column_histogram(ctx, in, (unsigned long long *)next.get())) != ALS_OK) return rc;
   {
-    void *tmp = nullptr;
+    Dev<void> tmp;
     size_t tmp_bytes = 0;
-    ALS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, next, out_ip, (int)(cols + 1), ctx->stream));
-    if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return rc;
-    ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, next, out_ip, (int)(cols + 1), ctx->stream));
-    dev_free(ctx, tmp);
+    ALS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, next.get(), out_ip.get(), (int)(cols + 1), ctx->stream));
+    if ((rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+    ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, next.get(), out_ip.get(), (int)(cols + 1), ctx->stream));
   }
   ip.assign((size_t)cols + 1, 0);
   ALS_CUDA(cudaMemcpyAsync(ip.data(), out_ip, sizeof(int64_t) * (cols + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  dev_free(ctx, out_ip);
+  out_ip.reset();
   // pieces: whole rows of one segment, cut from the segment indptrs (on the device for either residency)
   const std::vector<const als_csr *> segs = segments_of(in);
   struct Piece { int64_t r0, r1, b0, n; };
@@ -152,16 +151,15 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
     }
     max_seg = std::max(max_seg, S->nnz);
   }
-  int32_t *keys_out = nullptr, *vals_in = nullptr, *vals_out = nullptr, *win_indices = nullptr;
-  float *win_data = nullptr;
-  void *tmp = nullptr;
+  Dev<int32_t> keys_out, vals_in, vals_out, win_indices;
+  Dev<float> win_data;
+  Dev<void> tmp;
   size_t tmp_bytes = 0;
-  ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_out, keys_out, vals_in, vals_out, (int)max_piece, 0,
-                                           end_bit, ctx->stream));
-  if ((rc = dev_alloc(ctx, (void **)&keys_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&vals_in, sizeof(int32_t) * max_piece)) != ALS_OK ||
-      (rc = dev_alloc(ctx, (void **)&vals_out, sizeof(int32_t) * max_piece)) != ALS_OK ||
-      (rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK)
+  ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_out.get(), keys_out.get(), vals_in.get(), vals_out.get(),
+                                           (int)max_piece, 0, end_bit, ctx->stream));
+  if ((rc = keys_out.alloc(ctx, sizeof(int32_t) * max_piece)) != ALS_OK ||
+      (rc = vals_in.alloc(ctx, sizeof(int32_t) * max_piece)) != ALS_OK ||
+      (rc = vals_out.alloc(ctx, sizeof(int32_t) * max_piece)) != ALS_OK || (rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK)
     return rc;
   std::vector<std::pair<int64_t, int64_t>> windows{{0, cols}};  // column ranges [c0, c1)
   if (t->host) {
@@ -180,15 +178,15 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
       max_win = std::max(max_win, ip[c1] - ip[c0]);
       c0 = c1;
     }
-    if ((rc = dev_alloc(ctx, (void **)&win_indices, sizeof(int32_t) * max_win)) != ALS_OK ||
-        (rc = dev_alloc(ctx, (void **)&win_data, sizeof(float) * max_win)) != ALS_OK) {
+    if ((rc = win_indices.alloc(ctx, sizeof(int32_t) * max_win)) != ALS_OK ||
+        (rc = win_data.alloc(ctx, sizeof(float) * max_win)) != ALS_OK) {
       set_error("als_csr_transpose: a column window of %lld nonzeros does not fit in device memory (%lld bytes free)",
                 (long long)max_win, (long long)free_bytes);
       return rc;
     }
   }
-  int32_t *out_indices = t->host ? win_indices : t->indices;
-  float *out_data = t->host ? win_data : t->data;
+  int32_t *out_indices = t->host ? win_indices.get() : t->indices;
+  float *out_data = t->host ? win_data.get() : t->data;
   iota_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(vals_in, max_piece);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
@@ -201,8 +199,8 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
     rc = for_each_segment(ctx, in, [&](size_t s, const als_csr *S) -> int {
       for (const Piece &pc : pieces[s]) {
         if (pc.n == 0) continue;
-        ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, S->indices + pc.b0, keys_out, vals_in, vals_out, (int)pc.n,
-                                                 0, end_bit, ctx->stream));
+        ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, S->indices + pc.b0, keys_out.get(), vals_in.get(),
+                                                 vals_out.get(), (int)pc.n, 0, end_bit, ctx->stream));
         scatter_piece_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(
             vals_out, keys_out, pc.n, S->indptr + pc.r0, (int)(pc.r1 - pc.r0),
             index_base + S->row_offset - in->row_offset + pc.r0,
@@ -222,16 +220,6 @@ int transpose_segmented(als_ctx *ctx, const als_csr *in, als_csr *t, int64_t ind
       ALS_CUDA(cudaMemcpyAsync(t->indices + ip[c0], win_indices, sizeof(int32_t) * wn, cudaMemcpyDeviceToHost, ctx->stream));
       ALS_CUDA(cudaMemcpyAsync(t->data + ip[c0], win_data, sizeof(float) * wn, cudaMemcpyDeviceToHost, ctx->stream));
     }
-  }
-  for (void *p : {(void *)next, (void *)keys_out, (void *)vals_in, (void *)vals_out, tmp, (void *)win_indices,
-                  (void *)win_data})
-    dev_free(ctx, p);  // stream ordered: after the kernels and copies above
-  if (t->host) {  // the values are the input's: so is their range
-    if ((rc = dev_alloc(ctx, (void **)&t->wmax_dev, 2 * sizeof(unsigned))) != ALS_OK) return rc;
-    ALS_CUDA(cudaMemcpyAsync(t->wmax_dev, in->wmax_dev, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, ctx->stream));
-    t->wmax_valid = in->wmax_valid;
-    t->neg_w_known = in->neg_w_known;
-    t->has_neg_w = in->has_neg_w;
   }
   return ALS_OK;
 }
@@ -323,14 +311,12 @@ __global__ void narrow_values_kernel(const double *__restrict__ in, int64_t n, f
 
 int device_indptr(als_ctx *ctx, const void *indptr, int indptr_bytes, int64_t rows, std::vector<int64_t> &ip,
                   int64_t *base, int64_t *bad_row) {
-  long long *ip_dev = nullptr;
-  unsigned long long *flags = nullptr;
-  int rc = dev_alloc(ctx, (void **)&ip_dev, sizeof(long long) * (rows + 1));
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&flags, 3 * sizeof(unsigned long long));
-  if (rc != ALS_OK) {
-    dev_free(ctx, ip_dev);
+  Dev<long long> ip_dev;
+  Dev<unsigned long long> flags;
+  int rc;
+  if ((rc = ip_dev.alloc(ctx, sizeof(long long) * (rows + 1))) != ALS_OK ||
+      (rc = flags.alloc(ctx, 3 * sizeof(unsigned long long))) != ALS_OK)
     return rc;
-  }
   ALS_CUDA(cudaMemsetAsync(flags, 0xff, 3 * sizeof(unsigned long long), ctx->stream));
   const int blocks = (int)std::min<int64_t>((rows + 256) / 256, (int64_t)ctx->sm_count * 8);
   if (indptr_bytes == 8)
@@ -344,8 +330,6 @@ int device_indptr(als_ctx *ctx, const void *indptr, int indptr_bytes, int64_t ro
   ALS_CUDA(cudaMemcpyAsync(ip.data(), ip_dev, sizeof(int64_t) * (rows + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaMemcpyAsync(f, flags, sizeof(f), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  dev_free(ctx, ip_dev);
-  dev_free(ctx, flags);
   *base = (int64_t)f[0];
   *bad_row = f[1] == ~0ull ? -1 : (int64_t)f[1];
   return ALS_OK;
@@ -356,8 +340,8 @@ int device_entries(als_ctx *ctx, als_csr *c, const void *indices, int index_byte
   *bad_at = -1;
   const int64_t n = c->nnz;
   if (n == 0) return ALS_OK;
-  unsigned long long *flags = nullptr;
-  int rc = dev_alloc(ctx, (void **)&flags, 3 * sizeof(unsigned long long));
+  Dev<unsigned long long> flags;
+  const int rc = flags.alloc(ctx, 3 * sizeof(unsigned long long));
   if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaMemsetAsync(flags, 0xff, 3 * sizeof(unsigned long long), ctx->stream));
   const int blocks = ctx->sm_count * 8;
@@ -377,7 +361,6 @@ int device_entries(als_ctx *ctx, als_csr *c, const void *indices, int index_byte
   unsigned long long bad = 0;
   ALS_CUDA(cudaMemcpyAsync(&bad, flags + 2, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller's arrays have been read
-  dev_free(ctx, flags);
   if (bad != ~0ull) {
     *bad_at = (int64_t)bad;
     return ALS_E_INVALID;
@@ -397,8 +380,8 @@ int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch
   int64_t slot = 64;  // nonzeros per slot, a multiple of 64 so that every slot array starts 256-byte aligned
   for (const als_csr *S : segs) slot = std::max(slot, (S->nnz + 63) / 64 * 64);
   const int nslots = segs.size() > 1 ? 2 : 1;
-  char *ring = nullptr;
-  int rc = dev_alloc(ctx, (void **)&ring, nslots * slot * (int64_t)(with_data ? 8 : 4));
+  Dev<char> ring;
+  int rc = ring.alloc(ctx, nslots * slot * (int64_t)(with_data ? 8 : 4));
   if (rc != ALS_OK) {
     set_error("streaming a host-resident CSR: the device ring of %d x %lld nonzeros does not fit in device memory; lower "
               "segment_nnz", nslots, (long long)slot);
@@ -406,7 +389,7 @@ int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch
   }
   // the ring comes from the pool on the compute stream: the copy stream starts after that allocation
   for (int k = 0; k < nslots; ++k) ALS_CUDA(cudaEventRecord(ctx->ring_free[k], ctx->stream));
-  auto slot_indices = [&](int k) { return reinterpret_cast<int32_t *>(ring) + (int64_t)k * slot * (with_data ? 2 : 1); };
+  auto slot_indices = [&](int k) { return reinterpret_cast<int32_t *>(ring.get()) + (int64_t)k * slot * (with_data ? 2 : 1); };
   auto stage = [&](size_t s) -> int {
     const int k = (int)(s % nslots);
     const als_csr *S = segs[s];
@@ -431,8 +414,7 @@ int for_each_segment(als_ctx *ctx, const als_csr *C, const SegmentLaunch &launch
     ALS_CUDA(cudaEventRecord(ctx->ring_free[k], ctx->stream));
   }
   if (rc != ALS_OK) cudaStreamSynchronize(ctx->copy);  // a staged copy may still be writing into the ring
-  dev_free(ctx, ring);  // stream ordered: after the last launch, which waited for the last copy
-  return rc;
+  return rc;  // the ring is freed stream ordered: after the last launch, which waited for the last copy
 }
 
 void host_wmax(const float *v, int64_t n, unsigned *wmax_bits, bool *neg) {
@@ -563,8 +545,7 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
     return ALS_E_INVALID;
   }
   ALS_CUDA(cudaSetDevice(ctx->device));
-  als_csr *t = new als_csr();
-  t->ctx = ctx;
+  CsrHolder t = new_csr(ctx);
   t->rows = in->cols;
   t->cols = in->rows;
   t->nnz = in->nnz;
@@ -573,29 +554,31 @@ int csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   const int64_t piece_nnz = in->host || !in->segs.empty() ? kPieceNnz : std::max<int64_t>(in->nnz, 1);
   std::vector<int64_t> ip;
   int rc;
-  if ((rc = csr_alloc(ctx, t)) != ALS_OK || (rc = transpose_segmented(ctx, in, t, 0, piece_nnz, ip)) != ALS_OK ||
-      (rc = csr_layout(ctx, t, ip.data())) != ALS_OK) {
-    cudaStreamSynchronize(ctx->stream);  // D2H copies of a window may still be landing in t's arrays
-    als_csr_destroy(t);
+  if ((rc = csr_alloc(ctx, t.get())) != ALS_OK || (rc = transpose_segmented(ctx, in, t.get(), 0, piece_nnz, ip)) != ALS_OK)
     return rc;
+  if (t->host) {  // the values are the input's: so is their range
+    if ((rc = dev_alloc(ctx, (void **)&t->wmax_dev, 2 * sizeof(unsigned))) != ALS_OK) return rc;
+    ALS_CUDA(cudaMemcpyAsync(t->wmax_dev, in->wmax_dev, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, ctx->stream));
+    t->wmax_valid = in->wmax_valid;
+    t->neg_w_known = in->neg_w_known;
+    t->has_neg_w = in->has_neg_w;
   }
-  *out = t;
+  if ((rc = csr_layout(ctx, t.get(), ip.data())) != ALS_OK) return rc;
+  *out = t.release();
   return ALS_OK;
 }
 
 int csr_column_counts(als_ctx *ctx, const als_csr *in, int64_t *counts) {
   ALS_CUDA(cudaSetDevice(ctx->device));
-  unsigned long long *count = nullptr;
-  int rc = dev_alloc(ctx, (void **)&count, sizeof(long long) * std::max<int64_t>(in->cols, 1));
+  Dev<unsigned long long> count;
+  int rc = count.alloc(ctx, sizeof(long long) * std::max<int64_t>(in->cols, 1));
   if (rc != ALS_OK) return rc;
   ALS_CUDA(cudaMemsetAsync(count, 0, sizeof(long long) * in->cols, ctx->stream));
-  rc = column_histogram(ctx, in, count);
-  if (rc == ALS_OK && in->cols) {
+  if ((rc = column_histogram(ctx, in, count)) != ALS_OK) return rc;
+  if (in->cols)
     ALS_CUDA(cudaMemcpyAsync(counts, count, sizeof(long long) * in->cols, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  dev_free(ctx, count);
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  return rc;
+  return ALS_OK;
 }
 
 // One device transpose of the shard into a scratch CSR, in global row ids; piece q is then copied out of its rows
@@ -604,23 +587,23 @@ int csr_column_counts(als_ctx *ctx, const als_csr *in, int64_t *counts) {
 int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *col_bounds, als_csr **pieces) {
   ALS_CUDA(cudaSetDevice(ctx->device));
   for (int q = 0; q < n; ++q) pieces[q] = nullptr;
-  als_csr *t = new als_csr();
-  t->ctx = ctx;
+  CsrHolder t = new_csr(ctx);
   t->rows = in->cols;
   t->cols = in->row_offset + in->rows;
   t->nnz = in->nnz;
   std::vector<int64_t> ip;
-  int rc = csr_alloc(ctx, t);
-  if (rc == ALS_OK) rc = transpose_segmented(ctx, in, t, in->row_offset, kPieceNnz, ip);
-  for (int q = 0; q < n && rc == ALS_OK; ++q) {
+  int rc;
+  if ((rc = csr_alloc(ctx, t.get())) != ALS_OK || (rc = transpose_segmented(ctx, in, t.get(), in->row_offset, kPieceNnz, ip)) != ALS_OK)
+    return rc;
+  std::vector<CsrHolder> got(n);
+  for (int q = 0; q < n; ++q) {
     const int64_t r0 = col_bounds[q], r1 = col_bounds[q + 1];
-    als_csr *p = new als_csr();
-    pieces[q] = p;
-    p->ctx = ctx;
+    got[q] = new_csr(ctx);
+    als_csr *p = got[q].get();
     p->rows = r1 - r0;
     p->cols = t->cols;
     p->nnz = ip[r1] - ip[r0];
-    if ((rc = csr_alloc(ctx, p)) != ALS_OK) break;
+    if ((rc = csr_alloc(ctx, p)) != ALS_OK) return rc;
     if (p->nnz) {
       ALS_CUDA(cudaMemcpyAsync(p->indices, t->indices + ip[r0], sizeof(int32_t) * p->nnz, cudaMemcpyDeviceToDevice,
                                ctx->stream));
@@ -628,17 +611,12 @@ int csr_transpose_pieces(als_ctx *ctx, const als_csr *in, int n, const int64_t *
     }
     std::vector<int64_t> pip(ip.begin() + r0, ip.begin() + r1 + 1);
     for (int64_t &v : pip) v -= ip[r0];
-    rc = csr_layout(ctx, p, pip.data(), /*schedule=*/false);  // copied by the merge, rarely solved
+    // copied by the merge, rarely solved
+    if ((rc = csr_layout(ctx, p, pip.data(), /*schedule=*/false)) != ALS_OK) return rc;
   }
-  als_csr_destroy(t);  // stream ordered: after the copies above
-  if (rc != ALS_OK) {
-    cudaStreamSynchronize(ctx->stream);
-    for (int q = 0; q < n; ++q) {
-      als_csr_destroy(pieces[q]);
-      pieces[q] = nullptr;
-    }
-  }
-  return rc;
+  als_csr_destroy(t.release());  // stream ordered: after the copies above
+  for (int q = 0; q < n; ++q) pieces[q] = got[q].release();
+  return ALS_OK;
 }
 
 int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t cols, int64_t row_offset, als_csr **out) {
@@ -667,24 +645,19 @@ int csr_merge_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t co
       at[r] += ips[p][r + 1] - ips[p][r];
     }
   }
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
+  CsrHolder c = new_csr(ctx);
   c->rows = rows;
   c->cols = cols;
   c->nnz = oip[rows];
   c->row_offset = row_offset;
-  long long *tables_dev = nullptr;
-  int rc = csr_alloc(ctx, c);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&tables_dev, sizeof(int64_t) * tables.size());
-  if (rc == ALS_OK) rc = merge_pieces(ctx, n, pieces, base, tables, tables_dev, c);
-  dev_free(ctx, tables_dev);
-  if (rc == ALS_OK) rc = csr_layout(ctx, c, oip.data());
-  if (rc != ALS_OK) {
-    cudaStreamSynchronize(ctx->stream);
-    als_csr_destroy(c);
+  Dev<long long> tables_dev;
+  int rc;
+  if ((rc = csr_alloc(ctx, c.get())) != ALS_OK || (rc = tables_dev.alloc(ctx, sizeof(int64_t) * tables.size())) != ALS_OK ||
+      (rc = merge_pieces(ctx, n, pieces, base, tables, tables_dev, c.get())) != ALS_OK)
     return rc;
-  }
-  *out = c;
+  tables_dev.reset();
+  if ((rc = csr_layout(ctx, c.get(), oip.data())) != ALS_OK) return rc;
+  *out = c.release();
   return ALS_OK;
 }
 
@@ -710,44 +683,36 @@ int csr_concat_rows(als_ctx *ctx, int n, const als_csr *const *pieces, int64_t c
     nnz += pieces[p]->nnz;
   }
   const int64_t ns = (int64_t)segs.size();
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
+  CsrHolder c = new_csr(ctx);
   c->rows = rows;
   c->cols = cols;
   c->nnz = nnz;
   c->row_offset = row_offset;
-  long long *ip_dev = nullptr;  // the output indptr (rows + 1), then the segments' first positions (ns)
+  Dev<long long> ip_dev;  // the output indptr (rows + 1), then the segments' first positions (ns)
   std::vector<int64_t> ip((size_t)(rows + 1 + ns));
-  int rc = csr_alloc(ctx, c);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&ip_dev, sizeof(int64_t) * ip.size());
-  for (int64_t k = 0; k < ns && rc == ALS_OK; ++k) {
+  int rc;
+  if ((rc = csr_alloc(ctx, c.get())) != ALS_OK || (rc = ip_dev.alloc(ctx, sizeof(int64_t) * ip.size())) != ALS_OK) return rc;
+  for (int64_t k = 0; k < ns; ++k) {
     const Seg &g = segs[k];
     const int blocks = (int)std::min<int64_t>((g.S->rows + 256) / 256, (int64_t)ctx->sm_count * 8);
     concat_indptr_kernel<<<blocks, 256, 0, ctx->stream>>>(g.S->indptr, g.S->rows, g.pos, ip_dev + g.row, ip_dev + rows + 1 + k);
     ALS_CUDA(cudaGetLastError());
     ctx->launches++;
   }
-  if (rc == ALS_OK) {
-    ALS_CUDA(cudaMemcpyAsync(ip.data(), ip_dev, sizeof(int64_t) * ip.size(), cudaMemcpyDeviceToHost, ctx->stream));
-    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    for (int64_t k = 0; k < ns; ++k) {
-      const Seg &g = segs[k];
-      if (!g.S->nnz) continue;
-      const int64_t first = ip[rows + 1 + k];
-      ALS_CUDA(cudaMemcpyAsync(c->indices + g.pos, g.S->indices + first, sizeof(int32_t) * g.S->nnz,
-                               cudaMemcpyDeviceToDevice, ctx->stream));
-      ALS_CUDA(cudaMemcpyAsync(c->data + g.pos, g.S->data + first, sizeof(float) * g.S->nnz, cudaMemcpyDeviceToDevice,
-                               ctx->stream));
-    }
+  ALS_CUDA(cudaMemcpyAsync(ip.data(), ip_dev, sizeof(int64_t) * ip.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (int64_t k = 0; k < ns; ++k) {
+    const Seg &g = segs[k];
+    if (!g.S->nnz) continue;
+    const int64_t first = ip[rows + 1 + k];
+    ALS_CUDA(cudaMemcpyAsync(c->indices + g.pos, g.S->indices + first, sizeof(int32_t) * g.S->nnz, cudaMemcpyDeviceToDevice,
+                             ctx->stream));
+    ALS_CUDA(cudaMemcpyAsync(c->data + g.pos, g.S->data + first, sizeof(float) * g.S->nnz, cudaMemcpyDeviceToDevice,
+                             ctx->stream));
   }
-  dev_free(ctx, ip_dev);
-  if (rc == ALS_OK) rc = csr_layout(ctx, c, ip.data());
-  if (rc != ALS_OK) {
-    cudaStreamSynchronize(ctx->stream);
-    als_csr_destroy(c);
-    return rc;
-  }
-  *out = c;
+  ip_dev.reset();
+  if ((rc = csr_layout(ctx, c.get(), ip.data())) != ALS_OK) return rc;
+  *out = c.release();
   return ALS_OK;
 }
 

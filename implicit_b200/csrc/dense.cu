@@ -383,20 +383,14 @@ int launch_gramian_tc(als_ctx *ctx, const als_factors *Y) {
   const int64_t rows = std::max<int64_t>(Y->rows, 1);
   const int n_tiles = (int)ceil_div(rows, kTileM);
   const int grid = std::min(n_tiles, ctx->sm_count);
-  const int64_t need = (int64_t)grid * 64 * 64;
-  if (need > ctx->gram_partials_cap) {
-    if (ctx->gram_partials) {
-      ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-      ALS_CUDA(cudaFree(ctx->gram_partials));
-      ctx->gram_partials = nullptr;
-    }
-    const int64_t cap = (int64_t)ctx->sm_count * 2 * 128 * 128;
-    ALS_CUDA(cudaMalloc(&ctx->gram_partials, sizeof(float) * cap));
-    ctx->gram_partials_cap = cap;
-  }
+  const int64_t need = (int64_t)sizeof(float) * grid * 64 * 64;
+  int rc = ALS_OK;
+  if (need > ctx->gram_partials_cap &&
+      (rc = ensure_device_buffer(ctx, (void **)&ctx->gram_partials, &ctx->gram_partials_cap,
+                                 (int64_t)sizeof(float) * ctx->sm_count * 2 * 128 * 128)) != ALS_OK)
+    return rc;
   CUtensorMap my;
-  int rc = make_map(&my, Y->d, rows);
-  if (rc != ALS_OK) return rc;
+  if ((rc = make_map(&my, Y->d, rows)) != ALS_OK) return rc;
   ALS_CUDA(cudaFuncSetAttribute(gramian_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGramSmem));
   gramian_tc_kernel<<<grid, kDenseThreads, kGramSmem, ctx->stream>>>(my, n_tiles, ctx->gram_partials);
   ALS_CUDA(cudaGetLastError());

@@ -85,25 +85,22 @@ __global__ void fill_uniform_kernel(float *x, int64_t rows, int f, int ld, uint6
   }
 }
 
-int random_permutation(als_ctx *ctx, int64_t n, uint64_t seed, uint64_t stream, int32_t **out) {
-  uint64_t *k_in = nullptr, *k_out = nullptr;
-  int32_t *v_in = nullptr, *v_out = nullptr;
-  void *tmp = nullptr;
+int random_permutation(als_ctx *ctx, int64_t n, uint64_t seed, uint64_t stream, Dev<int32_t> &out) {
+  Dev<uint64_t> k_in, k_out;
+  Dev<int32_t> v_in, v_out;
+  Dev<void> tmp;
   size_t tmp_bytes = 0;
-  ALS_CUDA(cudaMalloc(&k_in, n * 8));
-  ALS_CUDA(cudaMalloc(&k_out, n * 8));
-  ALS_CUDA(cudaMalloc(&v_in, n * 4));
-  ALS_CUDA(cudaMalloc(&v_out, n * 4));
+  int rc;
+  if ((rc = k_in.alloc_cuda(ctx, n * 8)) != ALS_OK || (rc = k_out.alloc_cuda(ctx, n * 8)) != ALS_OK ||
+      (rc = v_in.alloc_cuda(ctx, n * 4)) != ALS_OK || (rc = v_out.alloc_cuda(ctx, n * 4)) != ALS_OK)
+    return rc;
   perm_keys_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(k_in, v_in, n, seed, stream);
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in, k_out, v_in, v_out, (int)n, 0, 64, ctx->stream);
-  ALS_CUDA(cudaMalloc(&tmp, std::max<size_t>(tmp_bytes, 16)));
-  cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, k_in, k_out, v_in, v_out, (int)n, 0, 64, ctx->stream);
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n, 0, 64,
+                                  ctx->stream);
+  if ((rc = tmp.alloc_cuda(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+  cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n, 0, 64, ctx->stream);
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  cudaFree(tmp);
-  cudaFree(k_in);
-  cudaFree(k_out);
-  cudaFree(v_in);
-  *out = v_out;
+  out = std::move(v_out);
   return ALS_OK;
 }
 
@@ -115,70 +112,62 @@ int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t n
     set_error("csr_generate: sizes beyond int32 (m = %lld)", (long long)m);
     return ALS_E_UNSUPPORTED;
   }
-  int32_t *pu = nullptr, *pi = nullptr;
+  Dev<int32_t> pu, pi;
   int rc;
-  if ((rc = random_permutation(ctx, users, seed, 1, &pu)) != ALS_OK) return rc;
-  if ((rc = random_permutation(ctx, items, seed, 2, &pi)) != ALS_OK) return rc;
-  uint64_t *k_a = nullptr, *k_b = nullptr;
-  int64_t *d_count = nullptr;
-  ALS_CUDA(cudaMalloc(&k_a, m * 8));
-  ALS_CUDA(cudaMalloc(&k_b, m * 8));
-  ALS_CUDA(cudaMalloc(&d_count, 8));
+  if ((rc = random_permutation(ctx, users, seed, 1, pu)) != ALS_OK) return rc;
+  if ((rc = random_permutation(ctx, items, seed, 2, pi)) != ALS_OK) return rc;
+  Dev<uint64_t> k_a, k_b;
+  Dev<int64_t> d_count;
+  if ((rc = k_a.alloc_cuda(ctx, m * 8)) != ALS_OK || (rc = k_b.alloc_cuda(ctx, m * 8)) != ALS_OK ||
+      (rc = d_count.alloc_cuda(ctx, 8)) != ALS_OK)
+    return rc;
   draw_keys_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(k_a, m, users, items, pu, pi, seed);
-  void *tmp = nullptr;
+  Dev<void> tmp;
   size_t t1 = 0, t2 = 0, t3 = 0;
-  cub::DeviceRadixSort::SortKeys(nullptr, t1, k_a, k_b, (int)m, 0, 64, ctx->stream);
-  cub::DeviceSelect::Unique(nullptr, t2, k_b, k_a, d_count, (int)m, ctx->stream);
+  cub::DeviceRadixSort::SortKeys(nullptr, t1, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream);
+  cub::DeviceSelect::Unique(nullptr, t2, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream);
   KeepKey keep{seed, 0};
-  cub::DeviceSelect::If(nullptr, t3, k_a, k_b, d_count, (int)m, keep, ctx->stream);
-  ALS_CUDA(cudaMalloc(&tmp, std::max(std::max(t1, t2), std::max<size_t>(t3, 16))));
+  cub::DeviceSelect::If(nullptr, t3, k_a.get(), k_b.get(), d_count.get(), (int)m, keep, ctx->stream);
   size_t tb = std::max(std::max(t1, t2), std::max<size_t>(t3, 16));
-  cub::DeviceRadixSort::SortKeys(tmp, tb, k_a, k_b, (int)m, 0, 64, ctx->stream);       // k_b sorted
-  cub::DeviceSelect::Unique(tmp, tb, k_b, k_a, d_count, (int)m, ctx->stream);           // k_a unique
+  if ((rc = tmp.alloc_cuda(ctx, (int64_t)tb)) != ALS_OK) return rc;
+  cub::DeviceRadixSort::SortKeys(tmp, tb, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream);       // k_b sorted
+  cub::DeviceSelect::Unique(tmp, tb, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream);    // k_a unique
   int64_t n_unique = 0;
   ALS_CUDA(cudaMemcpyAsync(&n_unique, d_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  uint64_t *keys = k_a;
+  const uint64_t *keys = k_a;
   int64_t nnz = n_unique;
   if (n_unique > nnz_target) {  // thin to ~nnz_target: every key kept independently with probability nnz_target / n_unique
     const long double p = (long double)nnz_target / (long double)n_unique;
     keep.threshold = (uint64_t)(p * 18446744073709551615.0L);
-    cub::DeviceSelect::If(tmp, tb, k_a, k_b, d_count, (int)n_unique, keep, ctx->stream);
+    cub::DeviceSelect::If(tmp, tb, k_a.get(), k_b.get(), d_count.get(), (int)n_unique, keep, ctx->stream);
     ALS_CUDA(cudaMemcpyAsync(&nnz, d_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
     keys = k_b;
   }
-  cudaFree(tmp);
-  cudaFree(pu);
-  cudaFree(pi);
-  als_csr *c = new als_csr();
-  c->ctx = ctx;
+  tmp.reset();
+  pu.reset();
+  pi.reset();
+  CsrHolder c = new_csr(ctx);
   c->rows = users;
   c->cols = items;
   c->nnz = nnz;
   c->row_offset = 0;
-  int arc;
-  if ((arc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (users + 1))) != ALS_OK ||
-      (arc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
-      (arc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK) {
-    als_csr_destroy(c);
-    return arc;
-  }
+  if ((rc = dev_alloc(ctx, (void **)&c->indptr, sizeof(int32_t) * (users + 1))) != ALS_OK ||
+      (rc = dev_alloc(ctx, (void **)&c->indices, sizeof(int32_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+      (rc = dev_alloc(ctx, (void **)&c->data, sizeof(float) * std::max<int64_t>(nnz, 1))) != ALS_OK)
+    return rc;
   split_keys_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys, nnz, items, c->indices, c->data, seed);
   indptr_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys, nnz, users, items, c->indptr);
   ALS_CUDA(cudaGetLastError());
   std::vector<int32_t> ip((size_t)users + 1);
   ALS_CUDA(cudaMemcpyAsync(ip.data(), c->indptr, sizeof(int32_t) * (users + 1), cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-  cudaFree(k_a);
-  cudaFree(k_b);
-  cudaFree(d_count);
-  rc = build_schedule(ctx, c, ip.data());
-  if (rc != ALS_OK) {
-    als_csr_destroy(c);
-    return rc;
-  }
-  *out = c;
+  k_a.reset();
+  k_b.reset();
+  d_count.reset();
+  if ((rc = build_schedule(ctx, c.get(), ip.data())) != ALS_OK) return rc;
+  *out = c.release();
   return ALS_OK;
 }
 

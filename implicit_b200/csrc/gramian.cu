@@ -223,16 +223,9 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
     int64_t np = std::min<int64_t>(ceil_div(std::max<int64_t>(rows, 1), 64), (int64_t)ctx->sm_count * 4 / (T * T) + 1);
     const int nparts = (int)std::max<int64_t>(1, std::min<int64_t>(np, 64));
     const int64_t rows_per_part = ceil_div(ceil_div(std::max<int64_t>(rows, 1), nparts), 16) * 16;
-    const int64_t need = (int64_t)nparts * F * F;
-    if (need > ctx->gram_partials_cap) {
-      if (ctx->gram_partials) {
-        ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-        ALS_CUDA(cudaFree(ctx->gram_partials));
-        ctx->gram_partials = nullptr;
-      }
-      ALS_CUDA(cudaMalloc(&ctx->gram_partials, sizeof(float) * need));
-      ctx->gram_partials_cap = need;
-    }
+    const int rc = ensure_device_buffer(ctx, (void **)&ctx->gram_partials, &ctx->gram_partials_cap,
+                                        (int64_t)sizeof(float) * nparts * F * F);
+    if (rc != ALS_OK) return rc;
     ProfScope prof(ctx, kProfGramian);
     gramian_wide_kernel<<<dim3(T, T, nparts), 256, 0, ctx->stream>>>(Y->d, rows, F, ctx->gram_partials, rows_per_part);
     ALS_CUDA(cudaGetLastError());
@@ -248,19 +241,13 @@ int launch_gramian(als_ctx *ctx, const als_factors *Y) {
   }
   const int64_t steps = ceil_div(std::max<int64_t>(Y->rows, 1), kGramRows);
   const int grid = (int)std::min<int64_t>(steps, (int64_t)ctx->sm_count * 2);
-  const int64_t need = (int64_t)grid * F * F;
-  if (need > ctx->gram_partials_cap) {
-    if (ctx->gram_partials) {
-      ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-      ALS_CUDA(cudaFree(ctx->gram_partials));
-      ctx->gram_partials = nullptr;
-    }
-    const int64_t cap = std::max<int64_t>(need, (int64_t)ctx->sm_count * 2 * 128 * 128);
-    ALS_CUDA(cudaMalloc(&ctx->gram_partials, sizeof(float) * cap));
-    ctx->gram_partials_cap = cap;
-  }
-  ProfScope prof(ctx, kProfGramian);
+  const int64_t need = (int64_t)sizeof(float) * grid * F * F;
   int rc = ALS_OK;
+  if (need > ctx->gram_partials_cap &&
+      (rc = ensure_device_buffer(ctx, (void **)&ctx->gram_partials, &ctx->gram_partials_cap,
+                                 std::max<int64_t>(need, (int64_t)sizeof(float) * ctx->sm_count * 2 * 128 * 128))) != ALS_OK)
+    return rc;
+  ProfScope prof(ctx, kProfGramian);
   switch (F / 16) {
     case 1: rc = run_gramian<1>(ctx, Y, grid); break;
     case 2: rc = run_gramian<2>(ctx, Y, grid); break;

@@ -121,24 +121,20 @@ int launch_ranking_metrics(als_ctx *ctx, const als_factors *items, const als_fac
   if ((rc = topk_device(ctx, items, queries, rows, n_query, k, nullptr, false, liked, TopkIds(), &t)) != ALS_OK) return rc;
   // the ids stay in ctx->scratch: what this pass needs comes from the pool
   const int grid = (int)ceil_div(n_query, kRowsPerCta);
-  double *buf = nullptr;
-  if ((rc = dev_alloc(ctx, (void **)&buf, (2 * (int64_t)k + (int64_t)(grid + 1) * kSums) * sizeof(double))) != ALS_OK) return rc;
+  Dev<double> buf;
+  if ((rc = buf.alloc(ctx, (2 * (int64_t)k + (int64_t)(grid + 1) * kSums) * sizeof(double))) != ALS_OK) return rc;
   double *gain = buf, *gain_sum = buf + k, *partials = buf + 2 * (int64_t)k, *out = partials + (int64_t)grid * kSums;
-  rc = [&]() -> int {
-    ALS_CUDA(cudaMemcpyAsync(gain, gain_host, k * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    ALS_CUDA(cudaMemcpyAsync(gain_sum, gain_sum_host, k * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    ranking_metrics_kernel<<<grid, 32 * kWarps, 0, ctx->stream>>>(t.ids, t.k_eff, k, (int)n_query, t_indptr, t_indices, gain,
-                                                                 gain_sum, items->rows, partials);
-    ALS_CUDA(cudaGetLastError());
-    sum_partials_kernel<<<1, 256, 0, ctx->stream>>>(partials, grid, out);
-    ALS_CUDA(cudaGetLastError());
-    ctx->launches += 2;
-    ALS_CUDA(cudaMemcpyAsync(sums, out, kSums * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    return ALS_OK;
-  }();
-  dev_free(ctx, buf);
-  return rc;
+  ALS_CUDA(cudaMemcpyAsync(gain, gain_host, k * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  ALS_CUDA(cudaMemcpyAsync(gain_sum, gain_sum_host, k * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  ranking_metrics_kernel<<<grid, 32 * kWarps, 0, ctx->stream>>>(t.ids, t.k_eff, k, (int)n_query, t_indptr, t_indices, gain,
+                                                               gain_sum, items->rows, partials);
+  ALS_CUDA(cudaGetLastError());
+  sum_partials_kernel<<<1, 256, 0, ctx->stream>>>(partials, grid, out);
+  ALS_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  ALS_CUDA(cudaMemcpyAsync(sums, out, kSums * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
 }
 
 }  // namespace als

@@ -55,24 +55,20 @@ int ids_range(als_ctx *ctx, const void *ids, int bytes, int64_t n, int64_t *min_
   *min_id = 0;
   *max_id = -1;
   if (n <= 0) return ALS_OK;
-  long long *range = nullptr;
-  int rc = dev_alloc(ctx, (void **)&range, 2 * sizeof(long long));
+  Dev<long long> range;
+  const int rc = range.alloc(ctx, 2 * sizeof(long long));
   if (rc != ALS_OK) return rc;
   const long long init[2] = {LLONG_MAX, LLONG_MIN};
   long long got[2] = {0, -1};
-  cudaError_t e = cudaMemcpyAsync(range, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) {
-    if (bytes == 8)
-      ids_range_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>((const long long *)ids, n, range);
-    else
-      ids_range_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>((const int32_t *)ids, n, range);
-    ctx->launches++;
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(got, range, sizeof(got), cudaMemcpyDeviceToHost, ctx->stream);
-  dev_free(ctx, range);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) return cuda_fail(e, "ids range", __FILE__, __LINE__);
+  ALS_CUDA(cudaMemcpyAsync(range, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  if (bytes == 8)
+    ids_range_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>((const long long *)ids, n, range);
+  else
+    ids_range_kernel<<<grid_for(ctx, n), 256, 0, ctx->stream>>>((const int32_t *)ids, n, range);
+  ctx->launches++;
+  ALS_CUDA(cudaGetLastError());
+  ALS_CUDA(cudaMemcpyAsync(got, range, sizeof(got), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   *min_id = got[0];
   *max_id = got[1];
   return ALS_OK;
@@ -84,43 +80,34 @@ int scatter_rows(als_ctx *ctx, als_factors *dst, const void *ids, int bytes, int
     set_error("als_factors_scatter_rows: %lld ids, more than one sort takes", (long long)n);
     return ALS_E_UNSUPPORTED;
   }
-  void *keys = nullptr, *tmp = nullptr;
-  int32_t *pos_in = nullptr, *pos = nullptr;
+  Dev<void> keys, tmp;
+  Dev<int32_t> pos_in, pos;
   size_t tmp_bytes = 0;
   auto sort = [&](void *t) -> cudaError_t {
     if (bytes == 8)
-      return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const long long *)ids, (long long *)keys, pos_in, pos, (int)n,
-                                             0, 64, ctx->stream);
-    return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const int32_t *)ids, (int32_t *)keys, pos_in, pos, (int)n, 0, 32,
-                                           ctx->stream);
+      return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const long long *)ids, (long long *)keys.get(), pos_in.get(),
+                                             pos.get(), (int)n, 0, 64, ctx->stream);
+    return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const int32_t *)ids, (int32_t *)keys.get(), pos_in.get(), pos.get(),
+                                           (int)n, 0, 32, ctx->stream);
   };
-  auto done = [&](int code) {
-    dev_free(ctx, keys);
-    dev_free(ctx, pos_in);
-    dev_free(ctx, pos);
-    dev_free(ctx, tmp);
-    return code;
-  };
-  int rc = dev_alloc(ctx, &keys, (int64_t)bytes * n);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&pos_in, sizeof(int32_t) * n);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&pos, sizeof(int32_t) * n);
-  if (rc == ALS_OK) rc = stage_iota(ctx, pos_in, n, 0);
-  if (rc != ALS_OK) return done(rc);
-  cudaError_t e = sort(nullptr);
-  if (e != cudaSuccess) return done(cuda_fail(e, "scatter: sort of the ids", __FILE__, __LINE__));
-  if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return done(rc);
-  if ((e = sort(tmp)) != cudaSuccess) return done(cuda_fail(e, "scatter: sort of the ids", __FILE__, __LINE__));
+  int rc;
+  if ((rc = keys.alloc(ctx, (int64_t)bytes * n)) != ALS_OK || (rc = pos_in.alloc(ctx, sizeof(int32_t) * n)) != ALS_OK ||
+      (rc = pos.alloc(ctx, sizeof(int32_t) * n)) != ALS_OK || (rc = stage_iota(ctx, pos_in, n, 0)) != ALS_OK)
+    return rc;
+  ALS_CUDA(sort(nullptr));
+  if ((rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+  ALS_CUDA(sort(tmp));
   ctx->launches++;
   const int grid = grid_for(ctx, n * dst->ld);
   if (bytes == 8)
-    scatter_last_kernel<<<grid, 256, 0, ctx->stream>>>((const long long *)keys, pos, n, src->d, dst->d, dst->rows, dst->f,
+    scatter_last_kernel<<<grid, 256, 0, ctx->stream>>>((const long long *)keys.get(), pos, n, src->d, dst->d, dst->rows, dst->f,
                                                        dst->ld);
   else
-    scatter_last_kernel<<<grid, 256, 0, ctx->stream>>>((const int32_t *)keys, pos, n, src->d, dst->d, dst->rows, dst->f,
+    scatter_last_kernel<<<grid, 256, 0, ctx->stream>>>((const int32_t *)keys.get(), pos, n, src->d, dst->d, dst->rows, dst->f,
                                                        dst->ld);
   ctx->launches++;
-  if ((e = cudaGetLastError()) != cudaSuccess) return done(cuda_fail(e, "scatter kernel", __FILE__, __LINE__));
-  return done(ALS_OK);
+  ALS_CUDA(cudaGetLastError());
+  return ALS_OK;
 }
 
 }  // namespace als

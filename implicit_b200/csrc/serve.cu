@@ -195,12 +195,10 @@ __global__ void restrict_unique_kernel(const int64_t *__restrict__ off, int64_t 
 int scan_counts(als_ctx *ctx, int64_t *counts, int64_t rows, int64_t *off) {
   size_t tmp_bytes = 0;
   ALS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, off, rows + 1, ctx->stream));
-  void *tmp = nullptr;
-  int rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes);
+  Dev<void> tmp;
+  const int rc = tmp.alloc(ctx, (int64_t)tmp_bytes);
   if (rc != ALS_OK) return rc;
-  const cudaError_t e = cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, off, rows + 1, ctx->stream);
-  dev_free(ctx, tmp);
-  ALS_CUDA(e);
+  ALS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, off, rows + 1, ctx->stream));
   ctx->launches++;
   return ALS_OK;
 }
@@ -280,53 +278,32 @@ int sort_ids(als_ctx *ctx, const void *in, int bytes, int64_t n, void *out) {
     return cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, (const int32_t *)in, (int32_t *)out, (int)n, 0, 32, ctx->stream);
   };
   ALS_CUDA(sort(nullptr));
-  void *tmp = nullptr;
-  int rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes);
+  Dev<void> tmp;
+  const int rc = tmp.alloc(ctx, (int64_t)tmp_bytes);
   if (rc != ALS_OK) return rc;
-  const cudaError_t e = sort(tmp);
-  dev_free(ctx, tmp);
-  ALS_CUDA(e);
+  ALS_CUDA(sort(tmp));
   ctx->launches++;
   return ALS_OK;
 }
 
-int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m, int64_t **indptr,
-                         int32_t **indices, float **data, int64_t *nnz) {
+int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset, int bytes, int64_t m,
+                         Dev<int64_t> &indptr, Dev<int32_t> &indices, Dev<float> &data, int64_t *nnz) {
   const int64_t rows = liked->rows, n = liked->nnz;
-  *indptr = nullptr;
-  *indices = nullptr;
-  *data = nullptr;
   *nnz = 0;
-  int32_t *pos = nullptr, *kept = nullptr, *sorted = nullptr;
-  int64_t *counts = nullptr, *off = nullptr;
-  void *tmp = nullptr;
-  int rc = dev_alloc(ctx, (void **)&counts, sizeof(int64_t) * (rows + 1));
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&off, sizeof(int64_t) * (rows + 1));
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)indptr, sizeof(int64_t) * (rows + 1));
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&pos, sizeof(int32_t) * n);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&kept, sizeof(int32_t) * n);
-  if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&sorted, sizeof(int32_t) * n);
-  auto done = [&](int code) {
-    dev_free(ctx, counts);
-    dev_free(ctx, off);
-    dev_free(ctx, pos);
-    dev_free(ctx, kept);
-    dev_free(ctx, sorted);
-    dev_free(ctx, tmp);
-    if (code != ALS_OK) {
-      dev_free(ctx, *indptr);
-      dev_free(ctx, *indices);
-      dev_free(ctx, *data);
-      *indptr = nullptr;
-      *indices = nullptr;
-      *data = nullptr;
-    }
-    return code;
-  };
-  if (rc != ALS_OK) return done(rc);
+  Dev<int64_t> counts, off, ip;
+  Dev<int32_t> pos, kept, sorted, ix;
+  Dev<float> dv;
+  Dev<void> tmp;
+  int rc;
+  if ((rc = counts.alloc(ctx, sizeof(int64_t) * (rows + 1))) != ALS_OK ||
+      (rc = off.alloc(ctx, sizeof(int64_t) * (rows + 1))) != ALS_OK ||
+      (rc = ip.alloc(ctx, sizeof(int64_t) * (rows + 1))) != ALS_OK ||
+      (rc = pos.alloc(ctx, sizeof(int32_t) * n)) != ALS_OK || (rc = kept.alloc(ctx, sizeof(int32_t) * n)) != ALS_OK ||
+      (rc = sorted.alloc(ctx, sizeof(int32_t) * n)) != ALS_OK)
+    return rc;
   const int grid = grid_for(ctx, 32 * rows);
   // count: the subset positions of the kept entries, and how many each row keeps
-  if (cudaMemsetAsync(counts + rows, 0, sizeof(int64_t), ctx->stream) != cudaSuccess) return done(cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__));
+  ALS_CUDA(cudaMemsetAsync(counts + rows, 0, sizeof(int64_t), ctx->stream));
   if (rows > 0) {
     if (bytes == 8)
       restrict_count_kernel<<<grid, 256, 0, ctx->stream>>>(liked->indptr, liked->indices, liked->data, rows,
@@ -337,22 +314,19 @@ int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset,
     ctx->launches++;
   }
   // scan, scatter in entry order, then each row sorted (CUB segmented radix sort, as rows_in_order)
-  if ((rc = scan_counts(ctx, counts, rows, off)) != ALS_OK) return done(rc);
+  if ((rc = scan_counts(ctx, counts, rows, off)) != ALS_OK) return rc;
   int64_t total = 0;
-  if (cudaMemcpyAsync(&total, off + rows, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-      cudaStreamSynchronize(ctx->stream) != cudaSuccess)
-    return done(cuda_fail(cudaGetLastError(), "restrict: count readback", __FILE__, __LINE__));
+  ALS_CUDA(cudaMemcpyAsync(&total, off + rows, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   if (total > 0) {
     restrict_scatter_kernel<<<grid, 256, 0, ctx->stream>>>(liked->indptr, rows, pos, off, kept);
     ctx->launches++;
     size_t tmp_bytes = 0;
-    if (cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, kept, sorted, (int)total, (int)rows, off, off + 1, 0, 32,
-                                                ctx->stream) != cudaSuccess)
-      return done(cuda_fail(cudaGetLastError(), "restrict: segmented sort", __FILE__, __LINE__));
-    if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return done(rc);
-    if (cub::DeviceSegmentedRadixSort::SortKeys(tmp, tmp_bytes, kept, sorted, (int)total, (int)rows, off, off + 1, 0, 32,
-                                                ctx->stream) != cudaSuccess)
-      return done(cuda_fail(cudaGetLastError(), "restrict: segmented sort", __FILE__, __LINE__));
+    ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, kept.get(), sorted.get(), (int)total, (int)rows,
+                                                     off.get(), off + 1, 0, 32, ctx->stream));
+    if ((rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+    ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(tmp, tmp_bytes, kept.get(), sorted.get(), (int)total, (int)rows,
+                                                     off.get(), off + 1, 0, 32, ctx->stream));
     ctx->launches++;
   }
   // unique per row (scipy's tocsr merges the duplicate positions): count, scan, write
@@ -360,19 +334,20 @@ int csr_restrict_columns(als_ctx *ctx, const als_csr *liked, const void *subset,
     restrict_unique_kernel<<<grid, 256, 0, ctx->stream>>>(off, rows, sorted, counts, nullptr, nullptr, nullptr);
     ctx->launches++;
   }
-  if ((rc = scan_counts(ctx, counts, rows, *indptr)) != ALS_OK) return done(rc);
-  if (cudaMemcpyAsync(nnz, *indptr + rows, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-      cudaStreamSynchronize(ctx->stream) != cudaSuccess)
-    return done(cuda_fail(cudaGetLastError(), "restrict: count readback", __FILE__, __LINE__));
-  if ((rc = dev_alloc(ctx, (void **)indices, sizeof(int32_t) * *nnz)) != ALS_OK) return done(rc);
-  if ((rc = dev_alloc(ctx, (void **)data, sizeof(float) * *nnz)) != ALS_OK) return done(rc);
+  if ((rc = scan_counts(ctx, counts, rows, ip)) != ALS_OK) return rc;
+  ALS_CUDA(cudaMemcpyAsync(nnz, ip + rows, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  if ((rc = ix.alloc(ctx, sizeof(int32_t) * *nnz)) != ALS_OK || (rc = dv.alloc(ctx, sizeof(float) * *nnz)) != ALS_OK)
+    return rc;
   if (*nnz > 0) {
-    restrict_unique_kernel<<<grid, 256, 0, ctx->stream>>>(off, rows, sorted, nullptr, *indptr, *indices, *data);
+    restrict_unique_kernel<<<grid, 256, 0, ctx->stream>>>(off, rows, sorted, nullptr, ip, ix, dv);
     ctx->launches++;
   }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return done(cuda_fail(e, "restrict kernels", __FILE__, __LINE__));
-  return done(ALS_OK);
+  ALS_CUDA(cudaGetLastError());
+  indptr = std::move(ip);
+  indices = std::move(ix);
+  data = std::move(dv);
+  return ALS_OK;
 }
 
 }  // namespace als

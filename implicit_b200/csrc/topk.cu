@@ -474,28 +474,27 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld) {
   const int64_t per_row = I * 24;
   const int rows_per_pass =
       (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)a.n_query, (3ll << 29) / per_row, (int64_t)INT32_MAX / I}));
-  unsigned long long *K_in = nullptr, *K_out = nullptr;
-  int32_t *V_in = nullptr, *V_out = nullptr, *off = nullptr;
-  void *tmp = nullptr;
+  Dev<unsigned long long> K_in, K_out;
+  Dev<int32_t> V_in, V_out, off;
+  Dev<void> tmp;
   size_t tmp_bytes = 0;
   const int64_t n = (int64_t)rows_per_pass * I;
-  cub::DeviceSegmentedRadixSort::SortPairsDescending(nullptr, tmp_bytes, K_in, K_out, V_in, V_out, (int)n, rows_per_pass, off, off + 1, 0,
-                                                     64, ctx->stream);
-  ALS_CUDA(cudaMalloc(&K_in, n * 8));
-  ALS_CUDA(cudaMalloc(&K_out, n * 8));
-  ALS_CUDA(cudaMalloc(&V_in, n * 4));
-  ALS_CUDA(cudaMalloc(&V_out, n * 4));
-  ALS_CUDA(cudaMalloc(&off, (rows_per_pass + 1) * 4));
-  ALS_CUDA(cudaMalloc(&tmp, std::max<size_t>(tmp_bytes, 16)));
+  cub::DeviceSegmentedRadixSort::SortPairsDescending(nullptr, tmp_bytes, K_in.get(), K_out.get(), V_in.get(), V_out.get(),
+                                                     (int)n, rows_per_pass, off.get(), off + 1, 0, 64, ctx->stream);
+  int rc;
+  if ((rc = K_in.alloc_cuda(ctx, n * 8)) != ALS_OK || (rc = K_out.alloc_cuda(ctx, n * 8)) != ALS_OK ||
+      (rc = V_in.alloc_cuda(ctx, n * 4)) != ALS_OK || (rc = V_out.alloc_cuda(ctx, n * 4)) != ALS_OK ||
+      (rc = off.alloc_cuda(ctx, (rows_per_pass + 1) * 4)) != ALS_OK || (rc = tmp.alloc_cuda(ctx, (int64_t)tmp_bytes)) != ALS_OK)
+    return rc;
   segment_offsets_kernel<<<(rows_per_pass + 256) / 256, 256, 0, ctx->stream>>>(off, rows_per_pass, (int)I);
-  int rc = ALS_OK;
   for (int q0 = 0; q0 < a.n_query && rc == ALS_OK; q0 += rows_per_pass) {
     const int nq = std::min(rows_per_pass, a.n_query - q0);
     ProfScope prof(ctx, kProfTopk);
     score_rows_kernel<<<nq, 256, ld * sizeof(float), ctx->stream>>>(a.items, a.n_items, ld, a.queries, a.query_rows, q0, a.norms,
                                                                      a.mask, a.liked_indptr, a.liked_indices, K_in, V_in);
-    cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairsDescending(tmp, tmp_bytes, K_in, K_out, V_in, V_out, (int)((int64_t)nq * I), nq,
-                                                                       off, off + 1, 0, 64, ctx->stream);
+    cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairsDescending(tmp, tmp_bytes, K_in.get(), K_out.get(), V_in.get(), V_out.get(),
+                                                                       (int)((int64_t)nq * I), nq, off.get(), off + 1, 0, 64,
+                                                                       ctx->stream);
     if (e != cudaSuccess || cudaGetLastError() != cudaSuccess) {
       set_error("topk: segmented sort failed (%s)", cudaGetErrorString(e));
       rc = ALS_E_CUDA;
@@ -514,12 +513,6 @@ int topk_by_sort(als_ctx *ctx, const TopkArgs &a, int ld) {
     set_error("topk: fallback pass failed");
     rc = ALS_E_CUDA;
   }
-  cudaFree(K_in);
-  cudaFree(K_out);
-  cudaFree(V_in);
-  cudaFree(V_out);
-  cudaFree(off);
-  cudaFree(tmp);
   return rc;
 }
 
@@ -548,8 +541,8 @@ __global__ void rebase_indptr_kernel(const int32_t *__restrict__ in, int64_t n, 
 int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, const int32_t **indices) {
   als_csr *c = const_cast<als_csr *>(csr);  // the check and the sorted copy are caches of the handle
   if (!c->order_known && c->rows > 0 && c->nnz > 0) {
-    int *flag = nullptr;
-    int rc = dev_alloc(ctx, (void **)&flag, sizeof(int));
+    Dev<int> flag;
+    int rc = flag.alloc(ctx, sizeof(int));
     if (rc != ALS_OK) return rc;
     ALS_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
     csr_unsorted_kernel<<<(unsigned)std::min<int64_t>(ceil_div(c->rows, 256), (int64_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
@@ -559,22 +552,24 @@ int rows_in_order(als_ctx *ctx, const als_csr *csr, const int32_t **indptr, cons
     int unsorted = 0, base = 0;
     ALS_CUDA(cudaMemcpyAsync(&unsorted, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     ALS_CUDA(cudaMemcpyAsync(&base, c->indptr, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    dev_free(ctx, flag);
+    flag.reset();
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (unsorted) {
-      if ((rc = dev_alloc(ctx, (void **)&c->sorted_indptr, (c->rows + 1) * sizeof(int32_t))) != ALS_OK) return rc;
-      if ((rc = dev_alloc(ctx, (void **)&c->sorted_indices, c->nnz * sizeof(int32_t))) != ALS_OK) return rc;
-      rebase_indptr_kernel<<<(unsigned)ceil_div(c->rows + 1, 256), 256, 0, ctx->stream>>>(c->indptr, c->rows + 1, c->sorted_indptr);
+    if (unsorted) {  // built in owners, kept with the handle once complete
+      Dev<int32_t> sorted_indptr, sorted_indices;
+      Dev<void> tmp;
+      if ((rc = sorted_indptr.alloc(ctx, (c->rows + 1) * sizeof(int32_t))) != ALS_OK) return rc;
+      if ((rc = sorted_indices.alloc(ctx, c->nnz * sizeof(int32_t))) != ALS_OK) return rc;
+      rebase_indptr_kernel<<<(unsigned)ceil_div(c->rows + 1, 256), 256, 0, ctx->stream>>>(c->indptr, c->rows + 1, sorted_indptr);
       ALS_CUDA(cudaGetLastError());
-      void *tmp = nullptr;
       size_t tmp_bytes = 0;
-      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, c->indices + base, c->sorted_indices, (int)c->nnz,
-                                                       (int)c->rows, c->sorted_indptr, c->sorted_indptr + 1, 0, 32, ctx->stream));
-      if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return rc;
-      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(tmp, tmp_bytes, c->indices + base, c->sorted_indices, (int)c->nnz,
-                                                       (int)c->rows, c->sorted_indptr, c->sorted_indptr + 1, 0, 32, ctx->stream));
-      dev_free(ctx, tmp);
+      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_bytes, c->indices + base, sorted_indices.get(), (int)c->nnz,
+                                                       (int)c->rows, sorted_indptr.get(), sorted_indptr + 1, 0, 32, ctx->stream));
+      if ((rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+      ALS_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(tmp, tmp_bytes, c->indices + base, sorted_indices.get(), (int)c->nnz,
+                                                       (int)c->rows, sorted_indptr.get(), sorted_indptr + 1, 0, 32, ctx->stream));
       ctx->launches += 2;
+      c->sorted_indptr = sorted_indptr.release();
+      c->sorted_indices = sorted_indices.release();
     }
     c->order_known = true;
   }

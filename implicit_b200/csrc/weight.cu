@@ -248,45 +248,36 @@ int weight_check_indptr(als_ctx *ctx, const void *indptr, int indptr_bytes, int6
 }
 
 int weight_column_counts(als_ctx *ctx, const void *indices, int index_bytes, int64_t nnz, int64_t cols, int64_t *counts) {
-  unsigned long long *d = nullptr;
+  Dev<unsigned long long> d;
   int *flag = nullptr;
-  int rc = dev_alloc(ctx, (void **)&d, sizeof(int64_t) * std::max<int64_t>(cols, 1));
-  if (rc == ALS_OK) rc = clear_flag(ctx, &flag);
-  cudaError_t e = cudaSuccess;
-  if (rc == ALS_OK) e = cudaMemsetAsync(d, 0, sizeof(int64_t) * cols, ctx->stream);
-  if (rc == ALS_OK && e == cudaSuccess && nnz > 0) {
+  int rc;
+  if ((rc = d.alloc(ctx, sizeof(int64_t) * std::max<int64_t>(cols, 1))) != ALS_OK || (rc = clear_flag(ctx, &flag)) != ALS_OK)
+    return rc;
+  ALS_CUDA(cudaMemsetAsync(d, 0, sizeof(int64_t) * cols, ctx->stream));
+  if (nnz > 0) {
     dispatch_index(index_bytes, [&](auto ix) {
       count_kernel<<<grid_for(ctx, nnz), 256, 0, ctx->stream>>>((decltype(ix))indices, nnz, cols, d, flag);
       return 0;
     });
     ctx->launches++;
-    e = cudaGetLastError();
+    ALS_CUDA(cudaGetLastError());
   }
-  if (rc == ALS_OK && e == cudaSuccess && cols > 0)
-    e = cudaMemcpyAsync(counts, d, sizeof(int64_t) * cols, cudaMemcpyDeviceToHost, ctx->stream);
-  if (rc == ALS_OK && e != cudaSuccess) rc = cuda_fail(e, "weight column counts", __FILE__, __LINE__);
-  if (rc == ALS_OK) rc = read_flag(ctx, flag, "als_weight_column_counts: an index is outside [0, cols)");
-  dev_free(ctx, d);
-  return rc;
+  if (cols > 0) ALS_CUDA(cudaMemcpyAsync(counts, d, sizeof(int64_t) * cols, cudaMemcpyDeviceToHost, ctx->stream));
+  return read_flag(ctx, flag, "als_weight_column_counts: an index is outside [0, cols)");
 }
 
 int weight_row_sums(als_ctx *ctx, int64_t rows, int64_t nnz, const void *indptr, int indptr_bytes, const void *row,
                     int row_bytes, const void *data, int value_kind, bool squares, void *sums_host) {
   const char *who = "als_weight_row_sums";
-  void *keys = nullptr, *tmp = nullptr, *sums = nullptr;
-  int64_t *perm_in = nullptr, *perm = nullptr, *ip = nullptr;
-  auto done = [&](int code) {
-    for (void *p : {keys, tmp, sums, (void *)perm_in, (void *)perm, (void *)ip}) dev_free(ctx, p);
-    return code;
-  };
+  Dev<void> keys, tmp, sums;
+  Dev<int64_t> perm_in, perm, ip;
   const int sum_bytes = squares || value_kind != ALS_VALUE_F32 ? 8 : 4;
-  int rc = dev_alloc(ctx, &sums, (int64_t)sum_bytes * std::max<int64_t>(rows, 1));
-  if (rc != ALS_OK) return done(rc);
-  cudaError_t e = cudaSuccess;
+  int rc = sums.alloc(ctx, (int64_t)sum_bytes * std::max<int64_t>(rows, 1));
+  if (rc != ALS_OK) return rc;
   if (row) {
     // COO in any order: a stable radix sort of (row, position) gives every row's positions in entry order
     int *flag = nullptr;
-    if ((rc = clear_flag(ctx, &flag)) != ALS_OK) return done(rc);
+    if ((rc = clear_flag(ctx, &flag)) != ALS_OK) return rc;
     if (nnz > 0) {
       dispatch_index(row_bytes, [&](auto rr) {
         count_kernel<<<grid_for(ctx, nnz), 256, 0, ctx->stream>>>((decltype(rr))row, nnz, rows,
@@ -298,37 +289,37 @@ int weight_row_sums(als_ctx *ctx, int64_t rows, int64_t nnz, const void *indptr,
     }
     char what[96];
     snprintf(what, sizeof(what), "%s: a row index is outside [0, %lld)", who, (long long)rows);
-    if ((rc = read_flag(ctx, flag, what)) != ALS_OK) return done(rc);
+    if ((rc = read_flag(ctx, flag, what)) != ALS_OK) return rc;
     size_t tmp_bytes = 0;
     auto sort = [&](void *t) -> cudaError_t {
       if (row_bytes == 8)
-        return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const long long *)row, (long long *)keys, perm_in, perm, nnz,
-                                               0, 64, ctx->stream);
-      return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const int32_t *)row, (int32_t *)keys, perm_in, perm, nnz, 0,
-                                             32, ctx->stream);
+        return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const long long *)row, (long long *)keys.get(), perm_in.get(),
+                                               perm.get(), nnz, 0, 64, ctx->stream);
+      return cub::DeviceRadixSort::SortPairs(t, tmp_bytes, (const int32_t *)row, (int32_t *)keys.get(), perm_in.get(),
+                                             perm.get(), nnz, 0, 32, ctx->stream);
     };
-    if (rc == ALS_OK) rc = dev_alloc(ctx, &keys, (int64_t)row_bytes * std::max<int64_t>(nnz, 1));
-    if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&perm_in, sizeof(int64_t) * std::max<int64_t>(nnz, 1));
-    if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&perm, sizeof(int64_t) * std::max<int64_t>(nnz, 1));
-    if (rc == ALS_OK) rc = dev_alloc(ctx, (void **)&ip, sizeof(int64_t) * (rows + 1));
-    if (rc != ALS_OK) return done(rc);
+    if ((rc = keys.alloc(ctx, (int64_t)row_bytes * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+        (rc = perm_in.alloc(ctx, sizeof(int64_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+        (rc = perm.alloc(ctx, sizeof(int64_t) * std::max<int64_t>(nnz, 1))) != ALS_OK ||
+        (rc = ip.alloc(ctx, sizeof(int64_t) * (rows + 1))) != ALS_OK)
+      return rc;
     if (nnz > 0) {
       iota64_kernel<<<grid_for(ctx, nnz), 256, 0, ctx->stream>>>(perm_in, nnz);
       ctx->launches++;
-      if ((e = sort(nullptr)) != cudaSuccess) return done(cuda_fail(e, "weight: sort of the rows", __FILE__, __LINE__));
-      if ((rc = dev_alloc(ctx, &tmp, (int64_t)tmp_bytes)) != ALS_OK) return done(rc);
-      if ((e = sort(tmp)) != cudaSuccess) return done(cuda_fail(e, "weight: sort of the rows", __FILE__, __LINE__));
+      ALS_CUDA(sort(nullptr));
+      if ((rc = tmp.alloc(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
+      ALS_CUDA(sort(tmp));
       ctx->launches++;
     }
     dispatch_index(row_bytes, [&](auto rr) {
-      indptr_from_sorted_kernel<<<grid_for(ctx, rows + 1), 256, 0, ctx->stream>>>((decltype(rr))keys, nnz, rows, ip);
+      indptr_from_sorted_kernel<<<grid_for(ctx, rows + 1), 256, 0, ctx->stream>>>((decltype(rr))keys.get(), nnz, rows, ip);
       return 0;
     });
     ctx->launches++;
     indptr = ip;
     indptr_bytes = 8;
   } else if ((rc = weight_check_indptr(ctx, indptr, indptr_bytes, rows, nnz, who)) != ALS_OK) {
-    return done(rc);
+    return rc;
   }
   if (rows > 0) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(rows, kWarps), (int64_t)ctx->sm_count * 8));
@@ -340,19 +331,19 @@ int weight_row_sums(als_ctx *ctx, int64_t rows, int64_t nnz, const void *indptr,
         using IP = std::remove_const_t<std::remove_pointer_t<decltype(ipt)>>;
         if (squares)
           row_sums_kernel<V, double, true, IP><<<grid, kWarps * 32, 0, ctx->stream>>>(
-              (const IP *)indptr, perm, (const V *)data, rows, (double *)sums);
+              (const IP *)indptr, perm, (const V *)data, rows, (double *)sums.get());
         else
           row_sums_kernel<V, S, false, IP><<<grid, kWarps * 32, 0, ctx->stream>>>((const IP *)indptr, perm, (const V *)data,
-                                                                                  rows, (S *)sums);
+                                                                                  rows, (S *)sums.get());
         return 0;
       });
     });
     ctx->launches++;
-    if ((e = cudaGetLastError()) != cudaSuccess) return done(cuda_fail(e, "weight row sums", __FILE__, __LINE__));
-    e = cudaMemcpyAsync(sums_host, sums, (size_t)sum_bytes * rows, cudaMemcpyDeviceToHost, ctx->stream);
+    ALS_CUDA(cudaGetLastError());
+    ALS_CUDA(cudaMemcpyAsync(sums_host, sums, (size_t)sum_bytes * rows, cudaMemcpyDeviceToHost, ctx->stream));
   }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  return done(e == cudaSuccess ? ALS_OK : cuda_fail(e, "weight row sums", __FILE__, __LINE__));
+  ALS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return ALS_OK;
 }
 
 int weight_entries(als_ctx *ctx, int kind, int64_t rows, int64_t cols, int64_t nnz, const void *indptr, int indptr_bytes,
@@ -360,27 +351,20 @@ int weight_entries(als_ctx *ctx, int kind, int64_t rows, int64_t cols, int64_t n
                    const void *row_values_host, const double *idf_host, double k1p1, double k1, int flags, double *out) {
   EntryArgs a{kind, rows, cols, nnz, nullptr, nullptr, k1p1, k1, (flags & ALS_WEIGHT_NUM_F32) != 0,
               (flags & ALS_WEIGHT_DEN_F32) != 0, nullptr};
-  void *rv = nullptr;
-  double *idf = nullptr;
-  auto done = [&](int code) {
-    dev_free(ctx, rv);
-    dev_free(ctx, idf);
-    return code;
-  };
+  Dev<void> rv;
+  Dev<double> idf;
   if (nnz == 0) return ALS_OK;
   int rc = clear_flag(ctx, &a.flag);
   if (rc != ALS_OK) return rc;
-  cudaError_t e = cudaSuccess;
   if (kind != ALS_WEIGHT_TFIDF) {
     const int64_t bytes = (kind == ALS_WEIGHT_BM25 && a.den32 ? 4 : 8) * rows;
-    if ((rc = dev_alloc(ctx, &rv, std::max<int64_t>(bytes, 8))) != ALS_OK) return done(rc);
-    e = cudaMemcpyAsync(rv, row_values_host, (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if ((rc = rv.alloc(ctx, std::max<int64_t>(bytes, 8))) != ALS_OK) return rc;
+    ALS_CUDA(cudaMemcpyAsync(rv, row_values_host, (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (kind != ALS_WEIGHT_NORMALIZE && e == cudaSuccess) {
-    if ((rc = dev_alloc(ctx, (void **)&idf, sizeof(double) * std::max<int64_t>(cols, 1))) != ALS_OK) return done(rc);
-    e = cudaMemcpyAsync(idf, idf_host, sizeof(double) * cols, cudaMemcpyHostToDevice, ctx->stream);
+  if (kind != ALS_WEIGHT_NORMALIZE) {
+    if ((rc = idf.alloc(ctx, sizeof(double) * std::max<int64_t>(cols, 1))) != ALS_OK) return rc;
+    ALS_CUDA(cudaMemcpyAsync(idf, idf_host, sizeof(double) * cols, cudaMemcpyHostToDevice, ctx->stream));
   }
-  if (e != cudaSuccess) return done(cuda_fail(e, "weight: upload of the row / column vectors", __FILE__, __LINE__));
   a.row_values = rv;
   a.idf = idf;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nnz, kTile), (int64_t)ctx->sm_count * 8));
@@ -401,8 +385,8 @@ int weight_entries(als_ctx *ctx, int kind, int64_t rows, int64_t cols, int64_t n
     });
   });
   ctx->launches++;
-  if ((e = cudaGetLastError()) != cudaSuccess) return done(cuda_fail(e, "weight entries", __FILE__, __LINE__));
-  return done(read_flag(ctx, a.flag, "als_weight_entries: a row or column index is outside the matrix"));
+  ALS_CUDA(cudaGetLastError());
+  return read_flag(ctx, a.flag, "als_weight_entries: a row or column index is outside the matrix");
 }
 
 }  // namespace als

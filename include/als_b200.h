@@ -64,7 +64,9 @@ int als_ctx_destroy(als_ctx *ctx);
  * fit() keeps Cui / Ciu host-resident even when they fit in device memory).  The
  * environment variables ALS_B200_<KNOB> are read once, in als_ctx_create, and reported on stderr when set; this
  * call changes a knob afterwards (A/B tools).  Results do not depend on any knob beyond fp32 rounding; segment_nnz and
- * host_csr change no bit.  als_ctx_get_knob reads one back.
+ * host_csr change no bit.  als_ctx_get_knob reads one back.  "alloc_fail_at" is for tests only, has no environment
+ * variable and does change results: n > 0 makes the n-th device allocation after the set return ALS_E_CUDA ("injected
+ * allocation failure") without calling CUDA, and the knob is then 0 again.
  * (No reference equivalent.) */
 int als_ctx_set_knob(als_ctx *ctx, const char *name, int value);
 int als_ctx_get_knob(als_ctx *ctx, const char *name, int *value);

@@ -53,6 +53,35 @@ def test_product_does_not_import_the_oracle():
                 assert "import oracle" not in src and "from oracle" not in src and "oracle/" not in src, f
 
 
+def test_device_memory_is_freed_by_its_owners_only():
+    """Temporary device blocks are held by a DeviceBlock (common.h), so no error return can leak one: outside the owner,
+    the handle destroy functions, the caller's free entries, the context growers and the functions that replace a
+    handle's own array or a static buffer, nothing in csrc/ frees device memory, and no function frees through a
+    `done` lambda."""
+    allowed = {
+        "dev_free", "DeviceBlock::reset",
+        "als_ctx_destroy", "als_csr_destroy", "als_factors_destroy", "als_factors_ipc_detach", "als_factors_ipc_export",
+        "als_device_free", "als_pool_free",
+        "ensure_scratch", "ensure_device_buffer",
+        "als_factors_grow", "als_flush_l2",
+    }
+    header = re.compile(r"^(?:ALS_API\s+|static\s+)?[A-Za-z_][\w<>\s\*&]*?\b([A-Za-z_]\w*(?:::\w+)?)\s*\(")
+    csrc = os.path.join(ROOT, "implicit_b200", "csrc")
+    found = []
+    for f in sorted(os.listdir(csrc)):
+        if not f.endswith((".cu", ".h", ".cuh")):
+            continue
+        func = None
+        for n, line in enumerate(open(os.path.join(csrc, f)), 1):
+            code = line.split("//")[0]
+            m = header.match(code)
+            if m and not code.startswith((" ", "\t", "#", "}")):
+                func = m.group(1)
+            if re.search(r"\b(dev_free|cudaFree)\(|auto done =", code) and (func not in allowed or "auto done =" in code):
+                found.append(f"{f}:{n} ({func}): {line.strip()}")
+    assert not found, "device memory freed outside its owners:\n" + "\n".join(found)
+
+
 def test_graft_entry_build_runs():
     """build() compiles (or finds up to date) the library, the oracle port and, where the reference is present,
     oracle/_ref -- and every header symbol resolves."""
