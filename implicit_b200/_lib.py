@@ -54,6 +54,8 @@ SIGNATURES = {
     "als_csr_transpose": (c_int, [c_void_p, c_void_p, P(c_void_p)]),
     "als_csr_generate": (c_int, [c_void_p, c_i64, c_i64, c_i64, ctypes.c_uint64, P(c_void_p)]),
     "als_factors_fill_uniform": (c_int, [c_void_p, c_void_p, ctypes.c_uint64, ctypes.c_float]),
+    "als_factors_fill_pcg64": (c_int, [c_void_p, c_void_p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64,
+                                       ctypes.c_uint64, c_int, ctypes.c_uint32, ctypes.c_float]),
     "als_csr_slice_rows": (c_int, [c_void_p, c_void_p, c_i64, c_i64, P(c_void_p)]),
     "als_csr_scale": (c_int, [c_void_p, c_void_p, c_f32]),
     "als_csr_shape": (c_int, [c_void_p, P(c_i64), P(c_i64), P(c_i64)]),
@@ -674,6 +676,15 @@ class DeviceFactors:
     def fill_uniform(self, seed, scale):
         """factors = scale * U[0,1) generated on the device (the distribution of implicit/cpu/als.py:144-147)."""
         check(self.ctx.lib.als_factors_fill_uniform(self.ctx.h, self.h, int(seed), float(scale)))
+
+    def fill_pcg64(self, state, scale):
+        """factors = numpy's Generator(PCG64).random((rows, factors), dtype=np.float32) * np.float32(scale) from state =
+        (state, inc, has_uint32, uinteger) of pcg64.get_state, bit for bit, drawn on the device; the caller's generator
+        is not advanced (pcg64.after_float32_draws gives the state it would reach)."""
+        s, inc, has, u = state
+        m64 = (1 << 64) - 1
+        check(self.ctx.lib.als_factors_fill_pcg64(self.ctx.h, self.h, s >> 64, s & m64, inc >> 64, inc & m64, int(has),
+                                                  int(u), float(scale)))
 
     def has_nan(self):
         flag = c_int(0)

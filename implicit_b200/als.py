@@ -14,7 +14,7 @@ import time
 import numpy as np
 from scipy.sparse import csr_matrix
 
-from . import _lib
+from . import _lib, pcg64
 from .distributed import RowBlock
 from .utils import CudaArray
 from .utils import (BLOCK_FIELDS, ModelFitError, block_cuts, check_block_table, check_csr, check_random_state,
@@ -245,7 +245,10 @@ class AlternatingLeastSquares:
     def _set_device(self, side, value):
         """Assignment of a CUDA float32 2-D array: the device replica is filled device to device and the host copy is
         stale until a getter downloads it."""
-        d = _lib.DeviceFactors.from_cuda(self.ctx, value, f"{side}_factors")
+        self._adopt_device(side, _lib.DeviceFactors.from_cuda(self.ctx, value, f"{side}_factors"))
+
+    def _adopt_device(self, side, d):
+        """d (a DeviceFactors the model now owns) becomes the device replica; the host copy is dropped."""
         if self._dev[side] is not None:
             self._dev[side].close()
         self._dev[side] = d
@@ -327,6 +330,7 @@ class AlternatingLeastSquares:
         ctx = self.ctx
 
         Cui_s = Ciu_s = None
+        drawn = {}  # side -> (generator state its device draw starts from, rows)
         try:
             s = time.time()
             # shards balanced by estimated cost: a row costs its nonzeros plus a fixed factorisation /
@@ -369,12 +373,31 @@ class AlternatingLeastSquares:
                 seed = int(random_state.integers(1, 2**31 - 1)) if self.process_group.rank == 0 else 0
                 seed = int(ctx.allreduce([float(seed)], "max")[0])
                 random_state = np.random.default_rng(seed)
-            if self._factors_shape("user") is None:
-                self._set_host("user", random_state.random((users, self.factors), dtype=np.float32) * np.float32(0.01))
-            if self._factors_shape("item") is None:
-                self._set_host("item", random_state.random((items, self.factors), dtype=np.float32) * np.float32(0.01))
-            if self._factors_shape("user") != (users, self.factors) or self._factors_shape("item") != (items, self.factors):
+            if pcg64.device_drawable(random_state):
+                # numpy's PCG64 draw is computed on the device: the generator is moved to the state the host draws
+                # would leave before anything is allocated, and no host copy is made
+                state = pcg64.get_state(random_state)
+                for side, rows in (("user", users), ("item", items)):
+                    if self._factors_shape(side) is None:
+                        drawn[side] = (state, rows)
+                        state = pcg64.after_float32_draws(state, rows * self.factors)
+                pcg64.set_state(random_state, state)
+            else:
+                if self._factors_shape("user") is None:
+                    self._set_host("user", random_state.random((users, self.factors), dtype=np.float32) * np.float32(0.01))
+                if self._factors_shape("item") is None:
+                    self._set_host("item", random_state.random((items, self.factors), dtype=np.float32) * np.float32(0.01))
+            if any(self._factors_shape(side) not in (None, (rows, self.factors)) for side, rows in (("user", users),
+                                                                                                   ("item", items))):
                 raise ValueError("pre-set factors do not match the shape of user_items / the factors parameter")
+            for side, (state, rows) in drawn.items():
+                d = _lib.DeviceFactors(ctx, rows, self.factors)
+                try:
+                    d.fill_pcg64(state, np.float32(0.01))
+                except BaseException:
+                    d.close()
+                    raise
+                self._adopt_device(side, d)
             X = self._device_factors("user")
             Y = self._device_factors("item")
             self._user_norms = self._item_norms = self._YtY = self._XtX = None  # cpu/als.py:152-154
@@ -438,6 +461,15 @@ class AlternatingLeastSquares:
                 ctx.detach_peers(Y)
             self._mark_device_updated("user")
             self._mark_device_updated("item")
+        except BaseException:
+            # the getters of a failed fit return its initial factors, as when they were drawn on the host: numpy draws
+            # them again from the saved states (the device replica, if filled, stays the current one, as after an upload)
+            for side, (state, rows) in drawn.items():
+                fresh = self._dev_fresh[side]
+                self._set_host(side, pcg64.generator_at(state).random((rows, self.factors), dtype=np.float32) *
+                               np.float32(0.01))
+                self._dev_fresh[side] = fresh
+            raise
         finally:  # on every exit: a traceback would otherwise keep both CSRs alive through this frame
             if Ciu_s is not None:
                 Ciu_s.close()

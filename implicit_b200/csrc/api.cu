@@ -894,6 +894,14 @@ ALS_API int als_factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed
   return als::factors_fill_uniform(ctx, f, seed, scale);
 }
 
+ALS_API int als_factors_fill_pcg64(als_ctx *ctx, als_factors *f, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi,
+                                   uint64_t inc_lo, int has_uint32, uint32_t uinteger, float scale) {
+  ALS_REQUIRE(ctx && f, "als_factors_fill_pcg64: NULL argument");
+  ALS_REQUIRE(has_uint32 == 0 || has_uint32 == 1, "als_factors_fill_pcg64: has_uint32=%d is not 0 or 1", has_uint32);
+  ALS_CUDA(cudaSetDevice(ctx->device));
+  return als::factors_fill_pcg64(ctx, f, state_hi, state_lo, inc_hi, inc_lo, has_uint32, uinteger, scale);
+}
+
 ALS_API int als_csr_transpose(als_ctx *ctx, const als_csr *in, als_csr **out) {
   ALS_REQUIRE(ctx && in && out, "als_csr_transpose: NULL argument");
   return als::csr_transpose(ctx, in, out);

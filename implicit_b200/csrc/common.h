@@ -326,6 +326,8 @@ int device_entries(als_ctx *ctx, als_csr *c, const void *indices, int index_byte
 // synthetic inputs generated on the device (gen.cu)
 int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t nnz_target, uint64_t seed, als_csr **out);
 int factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale);
+int factors_fill_pcg64(als_ctx *ctx, als_factors *f, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi,
+                       uint64_t inc_lo, int has_uint32, uint32_t uinteger, float scale);
 
 // kernels' host launchers (each returns an ALS_* code)
 int launch_gramian(als_ctx *ctx, const als_factors *Y);                  // -> ctx->G

@@ -85,6 +85,74 @@ __global__ void fill_uniform_kernel(float *x, int64_t rows, int f, int ld, uint6
   }
 }
 
+// ---- numpy's PCG64 float32 stream (implicit_b200/pcg64.py restates it in Python ints) --------------------------------
+// A 64-bit draw steps the 128-bit LCG, s = s * MULT + inc (mod 2^128), and outputs rotr64(hi ^ lo, hi >> 58) of the new
+// state; random(..., dtype=float32) takes its low 32-bit half, then its high half, each as (u32 >> 8) * 2^-24.
+typedef unsigned __int128 u128;
+
+constexpr u128 PCG_MULT = ((u128)0x2360ED051FC65DA4ull << 64) | 0x4385DF649FCCF645ull;
+constexpr int PCG_THREADS = 128;
+constexpr int PCG_DRAWS = 16;                                // 64-bit draws per thread and tile: 32 consecutive values
+constexpr int PCG_TILE = PCG_THREADS * PCG_DRAWS * 2;        // values per tile
+constexpr int PCG_BITS = 64;
+
+struct PcgJumps {
+  u128 mult[PCG_BITS], plus[PCG_BITS];  // s -> mult[j] s + plus[j] advances 2^j draws
+  u128 stride_mult, stride_plus;        // advances gridDim.x tiles
+};
+
+__device__ __forceinline__ float pcg_value(uint32_t u, float scale) {
+  return __fmul_rn((float)(u >> 8) * 0x1p-24f, scale);  // numpy's float32 product, never contracted into an FMA
+}
+
+// Value p of m (p = 0, 1, ...: the low then the high half of draw p / 2 + 1 after s0) goes to element first + p of the
+// C-order (rows, f) matrix x of row stride ld; with first = 1, element 0 is the buffered half u0.  Each thread owns the
+// 32 values of PCG_DRAWS consecutive draws of a tile: it jumps to its first draw once, then by the grid's stride, and the
+// block stages the tile in shared memory so the stores are coalesced.  fdiv = ceil(2^32 / f) for f >= 2:
+// __umulhi(c, fdiv) = c / f for every c < 2^19 (the error c (fdiv - 2^32 / f) / 2^32 stays below 1 / f).
+__global__ void __launch_bounds__(PCG_THREADS) fill_pcg64_kernel(float *__restrict__ x, int64_t m, int first, uint32_t u0,
+                                                                  int f, int ld, uint32_t fdiv, u128 s0, u128 inc,
+                                                                  float scale, const __grid_constant__ PcgJumps jumps) {
+  __shared__ float tile[PCG_TILE + PCG_TILE / 32];  // one pad word per 32 values: conflict-free both ways
+  if (first && blockIdx.x == 0 && threadIdx.x == 0) x[0] = pcg_value(u0, scale);
+  const int64_t tiles = (m + PCG_TILE - 1) / PCG_TILE;
+  u128 start = s0;  // the state before this thread's first draw of the current tile
+  {
+    uint64_t k = (uint64_t)blockIdx.x * (PCG_TILE / 2) + threadIdx.x * PCG_DRAWS;
+    for (int j = 0; k; ++j, k >>= 1)
+      if (k & 1) start = jumps.mult[j] * start + jumps.plus[j];
+  }
+  for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const int64_t p0 = t * PCG_TILE;
+    if (p0 + threadIdx.x * 2 * PCG_DRAWS < m) {
+      u128 s = start;
+#pragma unroll
+      for (int d = 0; d < PCG_DRAWS; ++d) {
+        s = s * PCG_MULT + inc;
+        const uint64_t hi = (uint64_t)(s >> 64), v0 = hi ^ (uint64_t)s;
+        const unsigned rot = (unsigned)(hi >> 58);
+        const uint64_t v = (v0 >> rot) | (v0 << ((64 - rot) & 63));
+        const int l = threadIdx.x * 2 * PCG_DRAWS + 2 * d;  // even: l and l + 1 share their 32-value group
+        tile[l + l / 32] = pcg_value((uint32_t)v, scale);
+        tile[l + 1 + l / 32] = pcg_value((uint32_t)(v >> 32), scale);
+      }
+    }
+    start = jumps.stride_mult * start + jumps.stride_plus;
+    __syncthreads();
+    const int64_t e0 = p0 + first;
+    const int64_t r0 = e0 / f;
+    const uint32_t c0 = (uint32_t)(e0 - r0 * f);
+    float *const row = x + r0 * ld;  // the tile's rows lie within 2^32 elements of its first row
+    const int valid = m - p0 < PCG_TILE ? (int)(m - p0) : PCG_TILE;
+    for (int l = threadIdx.x; l < valid; l += PCG_THREADS) {
+      const uint32_t c = c0 + l;
+      const uint32_t q = f == 1 ? c : __umulhi(c, fdiv);
+      row[q * (uint32_t)ld + (c - q * (uint32_t)f)] = tile[l + l / 32];
+    }
+    __syncthreads();
+  }
+}
+
 int random_permutation(als_ctx *ctx, int64_t n, uint64_t seed, uint64_t stream, Dev<int32_t> &out) {
   Dev<uint64_t> k_in, k_out;
   Dev<int32_t> v_in, v_out;
@@ -173,6 +241,40 @@ int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t n
 
 int factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale) {
   fill_uniform_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(f->d, f->rows, f->f, f->ld, seed, scale);
+  ALS_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return ALS_OK;
+}
+
+int factors_fill_pcg64(als_ctx *ctx, als_factors *f, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi,
+                       uint64_t inc_lo, int has_uint32, uint32_t uinteger, float scale) {
+  const int64_t n = f->rows * f->f;
+  if (n == 0) return ALS_OK;
+  const int first = has_uint32 ? 1 : 0;
+  const int64_t m = n - first;
+  const u128 inc = ((u128)inc_hi << 64) | inc_lo;
+  PcgJumps jumps;
+  u128 mult = PCG_MULT, plus = inc;  // the map of 2^j draws, j = 0, 1, ...
+  for (int j = 0; j < PCG_BITS; ++j) {
+    jumps.mult[j] = mult;
+    jumps.plus[j] = plus;
+    plus = (mult + 1) * plus;
+    mult = mult * mult;
+  }
+  const int64_t tiles = (m + PCG_TILE - 1) / PCG_TILE;
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 8));
+  // the stride of a grid-stride step, grid * PCG_TILE / 2 draws, composed from the maps of its bits
+  u128 sm = 1, sp = 0;
+  for (uint64_t k = (uint64_t)grid * (PCG_TILE / 2), j = 0; k; ++j, k >>= 1)
+    if (k & 1) {
+      sm = jumps.mult[j] * sm;
+      sp = jumps.mult[j] * sp + jumps.plus[j];
+    }
+  jumps.stride_mult = sm;
+  jumps.stride_plus = sp;
+  const uint32_t fdiv = f->f == 1 ? 0 : (uint32_t)(((1ull << 32) + (uint64_t)f->f - 1) / (uint64_t)f->f);
+  fill_pcg64_kernel<<<grid, PCG_THREADS, 0, ctx->stream>>>(f->d, m, first, uinteger, f->f, f->ld, fdiv,
+                                                            ((u128)state_hi << 64) | state_lo, inc, scale, jumps);
   ALS_CUDA(cudaGetLastError());
   ctx->launches++;
   return ALS_OK;

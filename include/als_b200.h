@@ -145,6 +145,14 @@ int als_csr_segment_count(const als_csr *csr, int64_t *n);
  * (No reference equivalent: it reads datasets from disk, implicit/datasets/.) */
 int als_csr_generate(als_ctx *ctx, int64_t rows, int64_t cols, int64_t nnz_target, uint64_t seed, als_csr **out);
 int als_factors_fill_uniform(als_ctx *ctx, als_factors *f, uint64_t seed, float scale);
+/* factors = scale * U[0,1) drawn exactly as numpy's Generator(PCG64).random((rows, factors), dtype=np.float32) *
+ * np.float32(scale) from the given bit generator state (its `state`, `inc`, `has_uint32` and `uinteger`): the default
+ * initialisation of implicit/cpu/als.py:144-147, bit for bit, computed on the device.  Values are taken in C order, the
+ * buffered high half first when has_uint32 = 1; each 64-bit draw supplies its low 32-bit half, then its high half, and a
+ * value is (u32 >> 8) * 2^-24 times scale, rounded once.  The padding columns are left as they are (zero from
+ * als_factors_create).  The caller advances its generator itself (implicit_b200/pcg64.py). */
+int als_factors_fill_pcg64(als_ctx *ctx, als_factors *f, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi,
+                           uint64_t inc_lo, int has_uint32, uint32_t uinteger, float scale);
 
 /* Device transpose: out = in^T as CSR (replaces the host `Cui.T.tocsr()`, implicit/cpu/als.py:137).
  * Returns `out` with its launch schedule, built on the host while the device sorts. */
