@@ -5,7 +5,9 @@
 // required of it (its parity is 8 GPUs against 1 GPU plus an oracle check on a row sample).  Same recipe, counter-based
 // hashing instead of numpy's PCG64:  m = 1.25 nnz draws of (user ~ plaw(0.5), item ~ plaw(0.8)) through two random
 // permutations, keys = user * items + item sorted and de-duplicated (cub), thinned to ~nnz by an independent
-// Bernoulli draw per key, values 1 + 4 U[0,1).  Deterministic for a given seed, independent of the grid.
+// Bernoulli draw per key, values 1 + 4 u with u = U[0,1) rounded to float, so in [1, 5]: 5 itself for 3 keys in 2^25,
+// where u rounds to 1.0f or to 1 - 2^-24 (whose 1 + 4 u ties to 5).  Deterministic for a given seed, independent of
+// the grid; tests/_gen_restate.py restates it in numpy.
 // (No reference equivalent: the reference loads datasets from disk, implicit/datasets/.)
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_select.cuh>
@@ -163,10 +165,12 @@ int random_permutation(als_ctx *ctx, int64_t n, uint64_t seed, uint64_t stream, 
       (rc = v_in.alloc_cuda(ctx, n * 4)) != ALS_OK || (rc = v_out.alloc_cuda(ctx, n * 4)) != ALS_OK)
     return rc;
   perm_keys_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(k_in, v_in, n, seed, stream);
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n, 0, 64,
-                                  ctx->stream);
+  ALS_CUDA(cudaGetLastError());
+  ALS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n,
+                                           0, 64, ctx->stream));
   if ((rc = tmp.alloc_cuda(ctx, (int64_t)tmp_bytes)) != ALS_OK) return rc;
-  cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n, 0, 64, ctx->stream);
+  ALS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, k_in.get(), k_out.get(), v_in.get(), v_out.get(), (int)n, 0, 64,
+                                           ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
   out = std::move(v_out);
   return ALS_OK;
@@ -190,16 +194,17 @@ int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t n
       (rc = d_count.alloc_cuda(ctx, 8)) != ALS_OK)
     return rc;
   draw_keys_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(k_a, m, users, items, pu, pi, seed);
+  ALS_CUDA(cudaGetLastError());
   Dev<void> tmp;
   size_t t1 = 0, t2 = 0, t3 = 0;
-  cub::DeviceRadixSort::SortKeys(nullptr, t1, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream);
-  cub::DeviceSelect::Unique(nullptr, t2, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream);
+  ALS_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t1, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream));
+  ALS_CUDA(cub::DeviceSelect::Unique(nullptr, t2, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream));
   KeepKey keep{seed, 0};
-  cub::DeviceSelect::If(nullptr, t3, k_a.get(), k_b.get(), d_count.get(), (int)m, keep, ctx->stream);
+  ALS_CUDA(cub::DeviceSelect::If(nullptr, t3, k_a.get(), k_b.get(), d_count.get(), (int)m, keep, ctx->stream));
   size_t tb = std::max(std::max(t1, t2), std::max<size_t>(t3, 16));
   if ((rc = tmp.alloc_cuda(ctx, (int64_t)tb)) != ALS_OK) return rc;
-  cub::DeviceRadixSort::SortKeys(tmp, tb, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream);       // k_b sorted
-  cub::DeviceSelect::Unique(tmp, tb, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream);    // k_a unique
+  ALS_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, k_a.get(), k_b.get(), (int)m, 0, 64, ctx->stream));     // k_b sorted
+  ALS_CUDA(cub::DeviceSelect::Unique(tmp, tb, k_b.get(), k_a.get(), d_count.get(), (int)m, ctx->stream));  // k_a unique
   int64_t n_unique = 0;
   ALS_CUDA(cudaMemcpyAsync(&n_unique, d_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
   ALS_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -208,7 +213,7 @@ int csr_generate_power_law(als_ctx *ctx, int64_t users, int64_t items, int64_t n
   if (n_unique > nnz_target) {  // thin to ~nnz_target: every key kept independently with probability nnz_target / n_unique
     const long double p = (long double)nnz_target / (long double)n_unique;
     keep.threshold = (uint64_t)(p * 18446744073709551615.0L);
-    cub::DeviceSelect::If(tmp, tb, k_a.get(), k_b.get(), d_count.get(), (int)n_unique, keep, ctx->stream);
+    ALS_CUDA(cub::DeviceSelect::If(tmp, tb, k_a.get(), k_b.get(), d_count.get(), (int)n_unique, keep, ctx->stream));
     ALS_CUDA(cudaMemcpyAsync(&nnz, d_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
     ALS_CUDA(cudaStreamSynchronize(ctx->stream));
     keys = k_b;

@@ -1,4 +1,5 @@
 """Shared helpers for the test-suite: parity metric and golden-case reconstruction."""
+import ctypes
 import os
 import sys
 
@@ -336,6 +337,38 @@ def select_h(scores, k):
         sel = sel[np.lexsort((-sel, -s[sel]))]
         ids[r, :kk], out[r, :kk] = sel, s[sel]
     return ids, out
+
+
+class _FactorsHead(ctypes.Structure):
+    """The leading fields of csrc/common.h's als_factors (ctx, rows, f, ld, d): the tests read the padding columns,
+    which no ABI call hands out."""
+    _fields_ = [("ctx", ctypes.c_void_p), ("rows", ctypes.c_int64), ("f", ctypes.c_int), ("ld", ctypes.c_int),
+                ("d", ctypes.c_void_p)]
+
+
+class _Raw:
+    def __init__(self, ptr, shape):
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": "<f4", "data": (ptr, False), "version": 3,
+                                         "strides": None, "stream": None}
+
+
+def padded_view(d):
+    """The whole (rows, ld) device matrix of a DeviceFactors, padding included, as a torch tensor over its memory, with
+    ld checked against a snapshot.  The context's queued work is done when it returns; work queued through the view
+    is the caller's to synchronise."""
+    import torch
+
+    head = ctypes.cast(d.h, ctypes.POINTER(_FactorsHead)).contents
+    snap = d.snapshot()
+    d.ctx.sync()
+    assert (head.rows, head.f, head.ld) == (d.rows, d.factors, snap.ld)
+    assert snap.__cuda_array_interface__["strides"] == (4 * snap.ld, 4)
+    return torch.as_tensor(_Raw(head.d, (d.rows, snap.ld)), device="cuda")
+
+
+def padded(d):
+    """The whole (rows, ld) device matrix of a DeviceFactors, padding included, copied to the host."""
+    return padded_view(d).cpu().numpy()
 
 
 def golden_cases():

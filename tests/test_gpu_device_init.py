@@ -4,7 +4,6 @@ past 2^32 values of the stream; fit(iterations=0) for every random_state kind, t
 fits against the same fit from pre-set numpy factors, failing fits and allocation failures against the host draw (a
 PCG64 subclass keeps fit on the host path, on the same stream).  PyTorch plays the producer of the CUDA inputs."""
 import copy
-import ctypes
 import gc
 
 import numpy as np
@@ -45,28 +44,6 @@ def bits(a):
     return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
 
 
-class _FactorsHead(ctypes.Structure):
-    """The leading fields of csrc/common.h's als_factors (ctx, rows, f, ld, d): the test reads the padding columns,
-    which no ABI call hands out."""
-    _fields_ = [("ctx", ctypes.c_void_p), ("rows", ctypes.c_int64), ("f", ctypes.c_int), ("ld", ctypes.c_int),
-                ("d", ctypes.c_void_p)]
-
-
-class _Raw:
-    def __init__(self, ptr, shape):
-        self.__cuda_array_interface__ = {"shape": shape, "typestr": "<f4", "data": (ptr, False), "version": 3,
-                                         "strides": None, "stream": None}
-
-
-def padded(d):
-    """The whole (rows, ld) device matrix of a DeviceFactors, padding included, with ld checked against a snapshot."""
-    head = ctypes.cast(d.h, ctypes.POINTER(_FactorsHead)).contents
-    snap = d.snapshot()
-    assert (head.rows, head.f, head.ld) == (d.rows, d.factors, snap.ld)
-    assert snap.__cuda_array_interface__["strides"] == (4 * snap.ld, 4)
-    return torch.as_tensor(_Raw(head.d, (d.rows, snap.ld)), device="cuda").cpu().numpy()
-
-
 @pytest.mark.parametrize("has", [0, 1])
 @pytest.mark.parametrize("f", WIDTHS)
 def test_fill_is_numpys_draw(ctx, f, has):
@@ -80,7 +57,7 @@ def test_fill_is_numpys_draw(ctx, f, has):
             d.fill_pcg64(st, SCALE)
             want = g.random((rows, f), dtype=np.float32) * SCALE
             if rows:
-                full = padded(d)
+                full = helpers.padded(d)
                 assert np.array_equal(bits(full[:, :f]), bits(want)), (rows, f, has)
                 assert not full[:, f:].any(), "padding columns must stay zero"
                 assert np.array_equal(bits(d.download()), bits(want))

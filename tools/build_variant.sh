@@ -9,7 +9,8 @@ ROOT=$(cd "$(dirname "$0")/.." && pwd)
 OUT=$ROOT/variants; mkdir -p $OUT/obj_$NAME
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden -ccbin /usr/bin/g++ --expt-relaxed-constexpr -I /usr/include"
 SRC=${VARIANT_SRC:-cholesky}
-for f in api csr gen gramian cholesky cholesky_tc cholesky_short dense cholesky_wide cholesky_xwide cg loss topk topk_tc metrics comm; do
+for s in $ROOT/implicit_b200/csrc/*.cu; do
+  f=$(basename $s .cu)
   if [ "$f" = "$SRC" ]; then
     /usr/local/cuda/bin/nvcc $FLAGS "$@" -Xptxas -v -I $ROOT/implicit_b200/csrc -c ${VARIANT_FILE:-$ROOT/implicit_b200/csrc/$f.cu} -o $OUT/obj_$NAME/$f.o 2>&1 | grep -E "cholesky_half_kernelILi4" -A2 | grep -E "Used|spill" | head -2
   else
